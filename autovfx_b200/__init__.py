@@ -1,4 +1,4 @@
-"""autovfx_b200 — B200-native (sm_100a) 3D-Gaussian-splatting rasterizer hot path for haoyuhsu/autovfx.
+"""autovfx_b200 — H100-native (sm_90a) 3D-Gaussian-splatting rasterizer hot path for haoyuhsu/autovfx.
 
 Only what the path needs: ``csrc/`` (hand-written CUDA + the C ABI of include/gsr_b200.h), the host-side
 mirror of the reference's Python interface (``rasterizer``, ``knn``), the per-frame loop (``render_loop``) and

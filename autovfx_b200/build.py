@@ -1,6 +1,6 @@
 """Builds the C-ABI CUDA library in-tree: autovfx_b200/csrc/*.cu -> autovfx_b200/lib/libgsr_b200.so.
 
-Plain nvcc, sm_100a only, no torch headers (the library has no torch dependency; the boundary is
+Plain nvcc, sm_90a (H100) only, no torch headers (the library has no torch dependency; the boundary is
 include/gsr_b200.h).  The .so is git-ignored but travels to the GPU box with the repo snapshot.
 """
 from __future__ import annotations
@@ -18,7 +18,7 @@ OBJDIR = os.path.join(HERE, "lib", "obj")
 SO_PATH = os.path.join(LIBDIR, "libgsr_b200.so")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
-NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-Xcompiler", "-fPIC",
+NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-Xcompiler", "-fPIC",
               "--expt-relaxed-constexpr"]
 
 
@@ -66,7 +66,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     with ThreadPoolExecutor(max_workers=4) as ex:
         objs = list(ex.map(compile_one, sources()))
     tmp = SO_PATH + ".tmp"
-    subprocess.check_call([nvcc, "-shared", "-o", tmp] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"])
+    subprocess.check_call([nvcc, "-shared", "-o", tmp] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"])
     os.replace(tmp, SO_PATH)
     return SO_PATH
 

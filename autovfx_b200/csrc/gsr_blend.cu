@@ -9,7 +9,7 @@
 //   gather : 32 survivors per batch, one per lane: ring -> position -> id (point_list) -> 48-byte record (three 16-byte loads);
 //            the next batch's records and the batch-after-next's ids are in flight while the current batch is blended
 //   stage  : the batch is transposed into the warp's shared-memory queue, two splats per 112-byte "pair" so that the
-//            per-splat arithmetic runs on both halves of packed fp32 registers (FADD2 / FMUL2 / FFMA2)
+//            per-splat arithmetic runs on both lanes of two-lane fp32 values (f32x2, gsr_packed.cuh)
 //   drain  : every lane evaluates every queued splat for its pixel (broadcast LDS.128), front to back.
 //
 // Two drains share the queue:
@@ -17,7 +17,7 @@
 //           colour*alpha then *T) — bit-identical images (GSR_FLAG_EXACT_IMAGES, and the repair path of the default mode).
 //   fast  : (default) the same bit-exact `power`, then alpha = min(0.99, ex2.approx(power*log2e + log2(opacity))) — one FFMA
 //           and one MUFU instead of expf's eight instructions and the opacity multiply — and a shorter serial part
-//           (T' = fma(-T, alpha, T), weight = T*alpha, colours accumulated as two FFMA2).  alpha differs from the reference's by
+//           (T' = fma(-T, alpha, T), weight = T*alpha, colours accumulated as two fma2).  alpha differs from the reference's by
 //           < 1.3e-6 relative, which cannot move an image by 1e-4 — unless it flips a DECISION.  The two decisions are guarded:
 //             * alpha < 1/255 (skip): each lane tracks min |log2(255*alpha)| over its evaluations; below BL_QBAND the
 //               decision is inside the approximation's error band;
@@ -349,9 +349,8 @@ __global__ void __launch_bounds__(WARPS * 32, OCC / WARPS) k_blend_lists(const B
 
 // Persistent variant (gsr_set_option("blend_persist", K), off by default): K CTAs per SM draw work items from
 // counters->blend_next, so the kernel never holds more than K * WARPS warps of an SM and kernels of the NEXT frame, issued on
-// another stream, can co-reside with it.  Measured (profiles/r02_experiments.md, r02_sweep_overlap.jsonl): with 2 - 3 streams
-// the frame time is the same within 2 % for K = 3 ... 8 — every kernel of the frame loads the LSU pipe, co-residency only trades
-// slots — so this stays an experiment knob; it renders the same bits (tests/test_gpu_options.py).
+// another stream, can co-reside with it.  An experiment knob (tools/sweep_options.py compares it per kernel); it renders the
+// same bits (tests/test_gpu_options.py).
 template <int NX, bool NC, bool EXACT, int WARPS, int OCC>
 __global__ void __launch_bounds__(WARPS * 32, OCC / WARPS) k_blend_lists_persistent(const BlendArgs a) {
     __shared__ __align__(16) unsigned char sq[WARPS * ListCfg<NX>::WB];
@@ -400,14 +399,14 @@ static int blend_persist() {
     if (g_blend_persist > 0 && g_sm_count == 0) {
         int dev = 0;
         cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || g_sm_count <= 0) g_sm_count = 148;
+        if (cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || g_sm_count <= 0) g_sm_count = 132;
     }
     return g_blend_persist;
 }
 
 template <int NX, bool NC, bool EXACT>
 static void launch_w(const BlendArgs& a, cudaStream_t st) {
-    constexpr int WARPS = 4;  // footprints per CTA: 2, 4 and 8 measured equal (0.317 / 0.315 / 0.319 ms)
+    constexpr int WARPS = 4;  // footprints per CTA
     const dim3 grid(a.gx * (GSR_FOOTS / WARPS), a.gy);
     const int persist = blend_persist();
     if (persist > 0) {

@@ -1,4 +1,4 @@
-// gsr_b200 — shared device/host helpers.  sm_100a only.
+// gsr_b200 — shared device/host helpers.  sm_90a (H100) only.
 //
 // Arithmetic note (bit-exact tile/key indexing, SURVEY §7 "hard parts"): every quantity that feeds an
 // integer output of the reference (radii, tile rectangles, depth key bits) is computed with the same

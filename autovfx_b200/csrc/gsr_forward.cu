@@ -152,7 +152,7 @@ __device__ __forceinline__ void sh_eval(const float* sh, float3 pos, const float
 
 // 3D covariance from scale / rotation (forward.cu:118-152: Sigma = (S R)^T (S R), quaternion not normalised).
 // The roundings (which product of each sum is fused into an FMA, which terms multiply the structural zeros of
-// S) are pinned with intrinsics to what nvcc 12.9 emits for the reference's GLM expression on sm_100a
+// S) are pinned with intrinsics to what nvcc 12.9 emits for the reference's GLM expression on sm_90a
 // (read from the SASS of oracle/_ref), because the compiler's contraction choices depend on common
 // sub-expression sharing and cannot be reproduced by writing "the same" C++ expression in another kernel.
 // A 1-ulp difference here changes conic -> alpha -> the T < 1e-4 termination of a pixel now and then.
@@ -1133,7 +1133,7 @@ __device__ void sort_tile(const uint2 rg, unsigned long long* __restrict__ pairs
     }
 }
 
-// stand-alone per-tile sort kernel (fusing it into the blend prologue was measured and dropped, profiles/r01_experiments.md)
+// stand-alone per-tile sort kernel
 template <bool PACKED>
 __global__ void __launch_bounds__(SORT_THREADS, 5) k_sort_tiles(const uint2* __restrict__ ranges, unsigned long long* __restrict__ pairs,
                                                              uint32_t* __restrict__ point_list,

@@ -339,7 +339,7 @@ int dist2_impl(int P, const float* points, float* out, void* ws, size_t ws_bytes
     uint32_t* hist = (uint32_t*)(w + L.hist);
     float* boxes = (float*)(w + L.boxes);
     k_bbox_init<<<1, 32, 0, st>>>(bbox);
-    k_bbox<<<min(148 * 8, (P + 255) / 256), 256, 0, st>>>(P, points, bbox);
+    k_bbox<<<min(132 * 8, (P + 255) / 256), 256, 0, st>>>(P, points, bbox);
     k_morton<<<(P + 255) / 256, 256, 0, st>>>(P, points, bbox, k0, v0);
     const int rs_blocks = (L.nchunks + RS_WARPS - 1) / RS_WARPS;
     for (int pass = 0; pass < 4; pass++) {

@@ -1,4 +1,4 @@
-// gsr_b200 — shared-memory vector accessors and Blackwell packed-fp32 (f32x2) helpers shared by the blend kernels.
+// gsr_b200 — shared-memory vector accessors and two-lane fp32 (f32x2) helpers shared by the blend kernels.
 #pragma once
 #include "gsr_common.cuh"
 
@@ -19,30 +19,20 @@ __device__ __forceinline__ float2 lds64(uint32_t a) {
     return v;
 }
 
-// Blackwell packed fp32: one FFMA2 / FMUL2 / FADD2 performs two IEEE round-to-nearest operations, one per 32-bit half
-// of a 64-bit register pair.  The blend evaluates TWO queued splats per iteration in the two halves.
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pk2(float lo, float hi) {
-    f32x2 r;
-    asm("mov.b64 %0, {%1,%2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
+// Two-lane fp32: the blend evaluates TWO queued splats per iteration, one per lane.  Hopper has no packed fp32
+// instruction, so each lane is one IEEE round-to-nearest FFMA / FMUL / FADD; the _rn intrinsics keep nvcc from
+// contracting a multiply and an add into one FMA, so every lane rounds exactly as the scalar formula it mirrors.
+struct f32x2 {
+    float lo, hi;
+};
+__device__ __forceinline__ f32x2 pk2(float lo, float hi) { return f32x2{lo, hi}; }
+__device__ __forceinline__ void upk2(f32x2 v, float& lo, float& hi) {
+    lo = v.lo;
+    hi = v.hi;
 }
-__device__ __forceinline__ void upk2(f32x2 v, float& lo, float& hi) { asm("mov.b64 {%0,%1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-    f32x2 r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
-}
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) {
-    f32x2 r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) {
-    f32x2 r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
+__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { return f32x2{__fmaf_rn(a.lo, b.lo, c.lo), __fmaf_rn(a.hi, b.hi, c.hi)}; }
+__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { return f32x2{__fmul_rn(a.lo, b.lo), __fmul_rn(a.hi, b.hi)}; }
+__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { return f32x2{__fadd_rn(a.lo, b.lo), __fadd_rn(a.hi, b.hi)}; }
 __device__ __forceinline__ float ex2_approx(float x) {
     float r;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));

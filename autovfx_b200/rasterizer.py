@@ -7,7 +7,7 @@ diff_gaussian_rasterization/__init__.py`` (reference lines in brackets):
 * ``GaussianRasterizer(nn.Module)``  ``.forward(...)`` -> (color, depth, alpha, radii), ``.markVisible``  [:174-223]
 * ``rasterize_gaussians(...)`` and ``_RasterizeGaussians`` (autograd.Function)     [:21-158]
 
-Host code stays Python/PyTorch; all device work happens in the hand-written sm_100a library behind the C ABI
+Host code stays Python/PyTorch; all device work happens in the hand-written sm_90a library behind the C ABI
 of ``include/gsr_b200.h`` (loaded through ctypes by ``_lib``).  PyTorch only provides memory (the caching
 allocator), the current stream and autograd plumbing.  There is no CPU path.
 

@@ -27,8 +27,7 @@ CAM_FLOATS = 37  # view(16) | proj(16) | campos(3) | tanfovx | tanfovy
 def bind_to_gpu_numa_node(index: int) -> str:
     """Pin the calling process to the CPUs NVML reports as closest to GPU ``index`` so that pinned host buffers (the D2H ring
     of ``FrameLoop``) are first-touched on that NUMA node.  With one process per GPU on an 8-GPU node this decides whether the
-    eight frame streams share one socket's memory controllers: measured 6,080 -> 7,572 end-to-end frames/s at N=8
-    (profiles/r01_bench_n8_final.json).  Call it before creating the loop; returns a short description, never raises."""
+    eight frame streams share one socket's memory controllers.  Call it before creating the loop; returns a short description, never raises."""
     try:
         import os
         import pynvml

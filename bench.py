@@ -28,7 +28,7 @@ Keys of the JSON line (rank 0 prints exactly one line on stdout):
                    MEASURED_PEAKS.json; ``frame_*`` keys give the same for the whole frame (B_fwd of SURVEY §8d).
 * ``cpu_baseline``  the CPU oracle (oracle/gsr_oracle.c, OpenMP) on one frame of the same workload (rank 0, N=1);
                    ``torch_cpu_baseline``: the pure-CPU PyTorch rasterize loop (oracle/torch_cpu_raster.py) on BASELINE config 1.
-* ``--impl reference``  the UNMODIFIED reference CUDA rasterizer (oracle/_ref, compiled from /root/reference) on the same GPU and
+* ``--impl reference``  the UNMODIFIED reference CUDA rasterizer (oracle/_ref, compiled from the reference sources) on the same GPU and
                    workload; its line carries the same metric plus ``train_step``, ``product_frame`` (the reference's own render()
                    executed from oracle/_ref_py on its own rasterizer) and ``config2``.  The reference's implementation of this
                    path *is* CUDA (it has no CPU implementation), so the reference arm runs on the device; BASELINE.md names it as the
@@ -65,7 +65,7 @@ def measured_hbm_peak():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s)"
 
 
 class ClockSampler:
@@ -171,6 +171,27 @@ def config2_tensors(dev):
     return g, scene.config2_camera().to(dev)
 
 
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(outdir, arrays):
+    """DIR/<name>.npy as float32, at most DUMP_BYTES in all: each array whole while it fits (at 1080p the images and up to ~5.7M
+    radii do), else a fixed seeded sample of its elements in the remaining budget, their sorted indices in <name>_index.npy (float64)."""
+    import numpy as np
+    os.makedirs(outdir, exist_ok=True)
+    left = DUMP_BYTES
+    for name, t in arrays.items():
+        a = t.float().cpu().numpy()
+        if a.nbytes > left:
+            n = left // 12  # 4 bytes per value + 8 per index
+            idx = np.sort(np.random.default_rng(0).choice(a.size, n, replace=False))
+            a = a.reshape(-1)[idx]
+            np.save(os.path.join(outdir, name + "_index.npy"), idx.astype(np.float64))
+            left -= idx.size * 8
+        np.save(os.path.join(outdir, name + ".npy"), a)
+        left -= a.nbytes
+
+
 # ===================================================================================================== reference arm
 def reference_arm(args, K, Wm, dev, g, cams, my_cams, my_cams_host, workload, g_cpu):
     from oracle import ref_cuda
@@ -273,7 +294,7 @@ def reference_arm(args, K, Wm, dev, g, cams, my_cams, my_cams_host, workload, g_
         knn = {"value": None, "error": str(ex)}
     emit_result({"impl": "reference", "metric": METRIC, "value": fps, "unit": "frames/s", "n_gpus": 1, "steps": K, "warmup": Wm, "ms_per_step": ms,
                  "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
-                 "config": {"workload": workload, "reference": "unmodified diff-gaussian-rasterization CUDA (oracle/_ref) on the same B200",
+                 "config": {"workload": workload, "reference": "unmodified diff-gaussian-rasterization CUDA (oracle/_ref) on the same GPU",
                             "avg_num_rendered": sum(outs) / len(outs), "l2": "inputs larger than L2 (708 MB of SH per frame)"},
                  "clocks": clocks,
                  "train_step": {"value": 1000.0 / ms_tr, "unit": "iterations/s", "ms": ms_tr, "iterations": n_tr,
@@ -295,7 +316,10 @@ def main():
     ap.add_argument("--gaussians", type=int, default=3_000_000, help="override only for debugging; the metric is quoted at 3M")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--quick", action="store_true", help="headline + e2e only (skip the secondary measurements)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed headline frame (color, depth, alpha, radii) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs writes the outputs of this implementation's timed path: use it with --impl ours")
     # stdout carries exactly ONE line, the JSON result: everything else that writes to file descriptor 1 (NCCL's version
     # banner, library chatter) is sent to stderr for the duration of the run
     sys.stdout.flush()
@@ -475,6 +499,8 @@ def main():
         ms, clocks2 = ms_single, clocks
     value = frames_total / (ms * 1e-3)
     clocks = clocks2
+    if args.dump_outputs and rank == 0:  # the frame the last timed step rendered, before later measurements reuse its output slot
+        dump_outputs(args.dump_outputs, dict(zip(("color", "depth", "alpha", "radii"), out_ring[(Wm + K - 1) % 2])))
     avg_R = sum(x["num_rendered"] for x in st) / len(st)
     avg_vis = sum(x["num_visible"] for x in st) / len(st)
     avg_redo = sum(x["exact_redos"] for x in st) / len(st)
@@ -498,15 +524,15 @@ def main():
                 "kernel_share": {k: (v / sum(kms.values()) if sum(kms.values()) else 0) for k, v in kms.items()},
                 "per_kernel_gbs": {k: (ab[k] / (v * 1e-3) / 1e9 if v > 0 else 0) for k, v in kms.items()},
                 "frame_algorithmic_bytes": ab["frame"], "frame_achieved": frame_gbs, "frame_frac": frame_gbs / peak,
-                "note": "k_blend_lists is bound by the shared-memory data pipe (every lane of a warp reads the 40 bytes of every splat it evaluates: ncu "
-                        "l1tex__data_pipe_lsu_wavefronts 89 % of peak, profiles/r02_ncu_forward.md), not by HBM; its HBM fraction is reported because the "
-                        "metric names the HBM roofline. The HBM-streaming kernels are k_project and k_color_emit (per_kernel_gbs)"}
+                "note": "k_blend_lists reads the 40 bytes of every splat it evaluates from shared memory in every lane of a warp, so its HBM "
+                        "fraction is low by design; it is reported because the metric names the HBM roofline. The HBM-streaming kernels are "
+                        "k_project and k_color_emit (per_kernel_gbs)"}
 
     line = {"metric": METRIC, "value": value, "unit": "frames/s", "n_gpus": world, "steps": K, "warmup": Wm,
             "ms_per_step": ms / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": {"workload": workload, "gaussians": P, "avg_visible": avg_vis, "avg_num_rendered": avg_R, "frames_per_rank": K,
                        "parallelism": "frame-sharded x%d (round-robin cameras, NCCL only for parameter broadcast + camera scatter)" % world,
-                       "l2": "inputs larger than L2 (708 MB of SH read per frame; 126 MB L2)",
+                       "l2": "inputs larger than L2 (708 MB of SH read per frame; 50 MB L2 on H100)",
                        "streams": "frames alternate between 2 CUDA streams (value); value_single_stream and roofline.kernel_ms come from the same K frames "
                                   "on one stream",
                        "api": "rasterizer.PreparedForward.launch per frame (the call FrameLoop makes), device-resident camera rows",

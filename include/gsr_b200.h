@@ -1,4 +1,4 @@
-/* gsr_b200 — C ABI of the B200-native 3D-Gaussian-splatting rasterizer hot path.
+/* gsr_b200 — C ABI of the H100-native 3D-Gaussian-splatting rasterizer hot path.
  *
  * This is the drop-in boundary for the reference's native entry points ("DGR/" =
  * sugar/gaussian_splatting/submodules/diff-gaussian-rasterization, "KNN/" = .../simple-knn of
@@ -237,7 +237,7 @@ int gsr_get_views(const gsr_workspace* ws, int32_t P, int32_t W, int32_t H, gsr_
 /* Per-kernel device timing of gsr_forward (CUDA events on the launching stream), for roofline reports.
  * ms_per_kernel[5] = average ms of {preprocess, tile_scan, emit, sort_tiles, blend} over the profiled frames. */
 int gsr_profile_begin(int max_frames);
-/* Same, timing only every stride-th gsr_forward call (the six event records per timed frame cost about 1.5 % of a 0.9 ms frame). */
+/* Same, timing only every stride-th gsr_forward call. */
 int gsr_profile_begin_strided(int max_frames, int stride);
 int gsr_profile_end(float* ms_per_kernel, int* frames);
 

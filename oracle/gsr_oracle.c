@@ -8,7 +8,7 @@
  *
  * Parity pinning: the reference ships no golden vectors (SURVEY §4), so this restatement is
  * pinned against outputs of the reference's own CUDA code (oracle/_ref/libref_dgr.so) run on a
- * B200 and committed under tests/golden/ (tests/golden/make_golden.py).  Arithmetic is fp32
+ * GPU and committed under tests/golden/ (tests/golden/make_golden.py).  Arithmetic is fp32
  * without FMA contraction (-ffp-contract=off); the GPU reference contracts to FMA, so float
  * outputs agree to ~1e-6 relative, not bitwise.
  *

@@ -2,7 +2,7 @@
 
 Only tests/, bench.py's cpu_baseline / reference legs and __graft_entry__.smoke() may import this
 module; the product package (autovfx_b200) never does.  Parity status: pinned against golden vectors
-produced by the reference's own CUDA code on a B200 (tests/golden/, see tests/golden/make_golden.py).
+produced by the reference's own CUDA code (tests/golden/, see tests/golden/make_golden.py).
 """
 from __future__ import annotations
 

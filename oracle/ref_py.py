@@ -35,9 +35,16 @@ STAGE = os.path.join(_HERE, "_ref_py")
 GS = os.path.join(STAGE, "sugar", "gaussian_splatting")
 
 
+# every staged file load() imports (oracle/Makefile: refpy); a partly staged tree counts as absent
+STAGED = [os.path.join(GS, "gaussian_renderer", "__init__.py"), os.path.join(GS, "scene", "gaussian_model.py"),
+          os.path.join(GS, "scene", "cameras.py"), os.path.join(GS, "utils", "general_utils.py"), os.path.join(GS, "utils", "graphics_utils.py"),
+          os.path.join(GS, "utils", "sh_utils.py"), os.path.join(GS, "utils", "system_utils.py"), os.path.join(STAGE, "gaussians_utils.py"),
+          os.path.join(STAGE, "rotation_utils.py"), os.path.join(STAGE, "ref_dgr", "__init__.py")]
+
+
 def available() -> bool:
     from . import ref_cuda
-    return os.path.exists(os.path.join(GS, "gaussian_renderer", "__init__.py")) and ref_cuda.available()
+    return all(os.path.exists(p) for p in STAGED) and ref_cuda.available()
 
 
 # ------------------------------------------------------------------------------------------------ third-party stand-ins

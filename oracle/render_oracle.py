@@ -8,7 +8,7 @@ conversions of its frame loop.  Never imported by the product (autovfx_b200/); u
 Parity status: the reference ships no golden vectors for these functions and they cannot be imported here (GR/ imports
 kornia, GU/:83 hard-codes device='cuda'); this restatement is pinned by tests/wrapper_ref.py — the same functions
 restated op for op in torch and executed with torch's own CUDA kernels on the GPU box (tests/test_gpu_wrapper.py) —, by the
-golden vectors that combination produced on a B200 around the compiled reference rasterizer (tests/golden/wrapper_small_sh.npz,
+golden vectors that combination produced around the compiled reference rasterizer (tests/golden/wrapper_small_sh.npz,
 tests/golden/make_golden.py) and by torch-CPU execution of the restatement in the CPU suite.
 """
 from __future__ import annotations

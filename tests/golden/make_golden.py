@@ -1,7 +1,7 @@
 """Generates the golden vectors under tests/golden/ by running the reference's OWN CUDA rasterizer
-(oracle/_ref/libref_dgr.so = unmodified diff-gaussian-rasterization compiled from /root/reference) on a B200.
+(oracle/_ref/libref_dgr.so = unmodified diff-gaussian-rasterization compiled from the reference sources) on the GPU.
 
-    gpurun -- 'python tests/golden/make_golden.py gpurun_out/golden'     # then copy gpurun_out/golden/*.npz here
+    python tests/golden/make_golden.py OUTDIR     # on an H100 with oracle/_ref built; then copy OUTDIR/*.npz here
 
 Inputs are the deterministic named cases of tests/helpers.py (seeded torch generators), so only outputs are stored.
 """
@@ -34,8 +34,7 @@ def main(outdir):
         torch.cuda.synchronize()
         out = {"case": np.array(name), "radii": fw["radii"].cpu().numpy(), "num_rendered": np.array(fw["num_rendered"]),
                "color": fw["color"].cpu().numpy(), "depth": fw["depth"].cpu().numpy(), "alpha": fw["alpha"].cpu().numpy(),
-               "point_list": st["point_list"].cpu().numpy(), "ranges": st["ranges"].cpu().numpy(), "n_contrib": st["n_contrib"].cpu().numpy(),
-               "means2D": st["means2D"].cpu().numpy(), "depths": st["depths"].cpu().numpy(), "conic_opacity": st["conic_opacity"].cpu().numpy()}
+               "point_list": st["point_list"].cpu().numpy(), "ranges": st["ranges"].cpu().numpy(), "n_contrib": st["n_contrib"].cpu().numpy()}
         if mode != "fw":
             dc, dd, da = Hh.image_grads(a, device=dev)
             g = ref_cuda.backward(fw, dc, dd, da)
@@ -47,6 +46,10 @@ def main(outdir):
                 out[k] = g[k].cpu().numpy()
         path = os.path.join(outdir, name + ".npz")
         np.savez_compressed(path, **out)
+        if os.path.getsize(path) > 1_000_000:  # files stay below 1 MB: gradients go beside the case (tests: helpers.load_golden)
+            os.makedirs(os.path.join(outdir, "grads"), exist_ok=True)
+            np.savez_compressed(os.path.join(outdir, "grads", name + ".npz"), **{k: out.pop(k) for k in list(out) if k.startswith("dL_")})
+            np.savez_compressed(path, **out)
         print(name, "->", path, "%.0f KB" % (os.path.getsize(path) / 1024), "R =", fw["num_rendered"])
 
 
@@ -82,6 +85,6 @@ def wrapper_golden(outdir, name="small_sh"):
 
 
 if __name__ == "__main__":
-    out = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "gpurun_out", "golden")
+    out = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "tests", "golden")
     main(out)
     wrapper_golden(out)

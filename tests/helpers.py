@@ -59,6 +59,15 @@ def case_inputs(name: str) -> Dict:
     raise KeyError(name)
 
 
+def load_golden(path: str) -> Dict:
+    """A golden case; the gradients of the larger cases are stored beside it under golden/grads/ (same file name)."""
+    gold = dict(np.load(path))
+    grads = os.path.join(os.path.dirname(path), "grads", os.path.basename(path))
+    if os.path.exists(grads):
+        gold.update(np.load(grads))
+    return gold
+
+
 def cov3d_from(scales: torch.Tensor, rotations: torch.Tensor, mod: float) -> torch.Tensor:
     """Python-side precomputed covariance (what gaussian_model.get_covariance builds, gaussian_model.py:47-52,117-118)."""
     r, x, y, z = rotations.unbind(-1)
@@ -106,11 +115,27 @@ def run_ours(a: Dict, for_backward=False, sorted_keys=False, debug=True, tight=N
 
 
 def run_ref(a: Dict):
+    """The compiled reference's forward on the same tensors, or None where it is not built: comparisons against its outputs
+    go through the ref_* helpers below, which replay stored digests of them in that case."""
     from oracle import ref_cuda
+    if not ref_cuda.available():
+        return None
     fw = ref_cuda.forward(a["means3D"], a["opacities"], a["view"], a["proj"], a["campos"], a["W"], a["H"], a["tanfovx"], a["tanfovy"],
                           shs=a["shs"], colors_precomp=a["colors_precomp"], scales=a["scales"], rotations=a["rotations"],
                           cov3D_precomp=a["cov3D_precomp"], sh_degree=a["sh_degree"], scale_modifier=a["scale_modifier"], bg=a["bg"])
     return fw
+
+
+def ref_state(device):
+    """ref_cuda.state() after run_ref, or None where the reference is not built."""
+    from oracle import ref_cuda
+    return ref_cuda.state(device) if ref_cuda.available() else None
+
+
+def ref_backward(a: Dict, dc, dd, da):
+    """The reference's gradients for run_ref(a), or None where the reference is not built."""
+    from oracle import ref_cuda
+    return ref_cuda.backward(run_ref(a), dc, dd, da) if ref_cuda.available() else None
 
 
 def run_oracle(a: Dict, stop_after="render"):
@@ -184,3 +209,148 @@ def relerr(a, b) -> float:
     if a.numel() == 0:
         return 0.0
     return float((a - b).abs().max() / (b.abs().max() + 1e-30))
+
+
+# ---- comparisons against the compiled reference (oracle/_ref), live or replayed ---------------------------------------------
+# Each ref_* call compares one of our tensors with a value of the reference, passed as a function that computes it.  Where the
+# reference library is built the function runs and the comparison is exact, and with GSR_REF_RECORD=<dir> every value is also
+# stored, in call order, as <dir>/<test id>.npz: a SHA-256 of its bytes for bit-identity checks, a seeded sample of REF_SAMPLE
+# elements (plus its max |value|) for tolerance checks: one per block of the flattened tensor.  Where
+# an exact-mode image is shown bit-identical to the reference, tests also compare the default-mode image with it in full.  Where the library is absent the functions are never called and the same
+# comparisons run against tests/golden/ref/<test id>.npz, recorded by the reference on an H100.
+REF_GOLDEN = os.path.join(ROOT, "tests", "golden", "ref")
+REF_SAMPLE = 2048
+_ref_log: Dict = {"test": None, "i": 0, "rec": {}}
+
+
+def _test_id() -> str:
+    tid = os.environ.get("PYTEST_CURRENT_TEST", "").rsplit(" (", 1)[0]
+    return "".join(c if c.isalnum() or c in "-_." else "_" for c in tid.replace("tests/", "", 1))
+
+
+def use_ref_python():
+    """Declares that the running test's reference values come from the reference's Python code (oracle/ref_py): its comparisons
+    run live only where that code is staged (not merely the compiled library) and replay the stored values elsewhere."""
+    _ref_log["py_test"] = _test_id()
+
+
+def ref_live() -> bool:
+    """Whether the running test's reference values are computed here (else they are replayed)."""
+    from oracle import ref_cuda, ref_py
+    return ref_py.available() if _ref_log.get("py_test") == _test_id() else ref_cuda.available()
+
+
+def have_ref() -> bool:
+    """The reference is built here, or its values are stored for the running test."""
+    return ref_live() or os.path.exists(os.path.join(REF_GOLDEN, _test_id() + ".npz"))
+
+
+def _canon(t) -> torch.Tensor:
+    t = torch.as_tensor(t).detach()
+    t = t.float() if t.is_floating_point() else t.long()
+    return t.contiguous().cpu()
+
+
+def _digest(t: torch.Tensor) -> str:
+    import hashlib
+    return hashlib.sha256(str(tuple(t.shape)).encode() + t.numpy().tobytes()).hexdigest()
+
+
+def _sample_idx(n: int) -> np.ndarray:
+    """Stratified: one seeded element from each of REF_SAMPLE equal blocks of the flattened tensor, so every region is covered."""
+    if n <= REF_SAMPLE:
+        return np.arange(n)
+    edges = (np.arange(REF_SAMPLE + 1, dtype=np.int64) * n) // REF_SAMPLE
+    return edges[:-1] + np.random.default_rng(n).integers(0, edges[1:] - edges[:-1])
+
+
+def _ref_entry(kind: str, fn):
+    """The reference's record for the next comparison of the running test: computed by fn (and stored when recording) or replayed."""
+    tid = _test_id()
+    if _ref_log["test"] != tid:
+        _ref_log.update(test=tid, i=0, rec={})
+    i = _ref_log["i"]
+    _ref_log["i"] += 1
+    if not ref_live():
+        path = os.path.join(REF_GOLDEN, tid + ".npz")
+        if tid not in _ref_log["rec"]:
+            assert os.path.exists(path), "no compiled reference and no stored reference values (%s)" % path
+            _ref_log["rec"][tid] = dict(np.load(path))
+        rec = _ref_log["rec"][tid]
+        assert "%d_kind" % i in rec and str(rec["%d_kind" % i]) == kind, "stored reference values do not match comparison %d" % i
+        return None, {k.split("_", 1)[1]: v for k, v in rec.items() if k.split("_", 1)[0] == str(i)}
+    v = fn()
+    out = os.environ.get("GSR_REF_RECORD")
+    if out:
+        e = {"kind": np.str_(kind)}
+        if kind == "value":
+            e["value"] = np.asarray(v)
+        else:
+            c = _canon(v)
+            e["shape"] = np.asarray(c.shape, dtype=np.int64)
+            if kind == "same":
+                e["sha"] = np.str_(_digest(c))
+            else:
+                flat = c.double().reshape(-1)
+                e["sample"] = flat[torch.from_numpy(_sample_idx(flat.numel()))].float().numpy()
+                e["absmax"] = np.asarray(float(flat.abs().max()) if flat.numel() else 0.0)
+        rec = _ref_log["rec"].setdefault(tid, {})
+        rec.update({"%d_%s" % (i, k): x for k, x in e.items()})
+        os.makedirs(out, exist_ok=True)
+        np.savez_compressed(os.path.join(out, tid + ".npz"), **rec)
+    return v, None
+
+
+def ref_value(fn):
+    """A scalar of the reference (e.g. num_rendered)."""
+    v, rec = _ref_entry("value", fn)
+    return v if rec is None else rec["value"].item()
+
+
+def ref_same(x, fn) -> bool:
+    """Bit identity with a tensor of the reference (integers compared as int64, floats as float32)."""
+    v, rec = _ref_entry("same", fn)
+    if rec is None:
+        a, b = _canon(x), _canon(v)
+        return a.shape == b.shape and torch.equal(a, b)
+    c = _canon(x)
+    return list(c.shape) == rec["shape"].tolist() and _digest(c) == str(rec["sha"])
+
+
+def _ref_pair(x, fn):
+    v, rec = _ref_entry("sample", fn)
+    a = _canon(x).double().reshape(-1)
+    if rec is None:
+        return a, _canon(v).double().reshape(-1), None
+    assert a.numel() == int(np.prod(rec["shape"])), "shape differs from the stored reference values"
+    return a[torch.from_numpy(_sample_idx(a.numel()))], torch.from_numpy(rec["sample"]).double(), float(rec["absmax"])
+
+
+def ref_maxabs(x, fn) -> float:
+    a, b, _ = _ref_pair(x, fn)
+    return float((a - b).abs().max()) if a.numel() else 0.0
+
+
+def ref_meanabs(x, fn) -> float:
+    a, b, _ = _ref_pair(x, fn)
+    return float((a - b).abs().mean()) if a.numel() else 0.0
+
+
+def ref_allclose(x, fn, rtol: float) -> bool:
+    a, b, _ = _ref_pair(x, fn)
+    return bool(((a - b).abs() <= rtol * b.abs()).all())
+
+
+def ref_relerr(x, fn) -> float:
+    a, b, bmax = _ref_pair(x, fn)
+    if a.numel() == 0:
+        return 0.0
+    return float((a - b).abs().max() / ((float(b.abs().max()) if bmax is None else bmax) + 1e-30))
+
+
+def ref_images_close(got: Dict, ref, tol=None):
+    """assert_images_close against the reference's forward (run_ref's result, None where replayed)."""
+    for k in ("color", "depth", "alpha"):
+        t = FAST_TOL[k] if tol is None else tol
+        e = ref_maxabs(got[k], lambda: ref[k])
+        assert e <= t, "%s: max abs %.3g > %.3g" % (k, e, t)

@@ -1,20 +1,23 @@
-"""The reference's OWN Python callers of the hot path, executed on the GPU box against the drop-in (SURVEY §8 rows a17, a19, b, f-1..f-4).
+"""The reference's OWN Python callers of the hot path against the drop-in (SURVEY §8 rows a17, a19, b, f-1..f-4).
 
-``oracle/_ref_py`` holds unmodified copies of the reference's ``render()`` (gaussian_renderer/__init__.py:83-218), ``GaussianModel``
-(scene/gaussian_model.py: activations, get_normal, create_from_pcd -> distCUDA2, save_ply / load_ply), ``Camera``
-(scene/cameras.py), ``transform_gaussians`` / ``merge_two_gaussians`` (gaussians_utils.py:71-125) and the reference's Python autograd
-front end of the rasterizer, staged by ``make -C oracle refpy``; ``oracle/ref_py.py`` binds them either to this repository's drop-in
-packages (``diff_gaussian_rasterization``, ``simple_knn._C``: zero edits to the reference files) or to the reference's own
-CUDA (oracle/_ref).  Every comparison below is therefore "reference code on the drop-in" against "reference code on the reference".
+``make -C oracle ref refpy`` stages unmodified copies of the reference's ``render()`` (gaussian_renderer/__init__.py:83-218),
+``GaussianModel`` (scene/gaussian_model.py), ``Camera`` (scene/cameras.py), ``transform_gaussians`` / ``merge_two_gaussians``
+(gaussians_utils.py:71-125) and its Python autograd front end into the git-ignored ``oracle/_ref_py`` where the reference sources are
+available; ``oracle/ref_py.py`` binds them either to this repository's drop-in packages or to the reference's own CUDA (oracle/_ref).
+Tests taking ``ref_ns`` compare our code with values the reference code computes, through the Hh.ref_* helpers: live where the
+reference is staged, replayed from tests/golden/ref/ elsewhere.  Tests taking ``rp`` execute the reference's code ON the drop-in and
+need it staged.
 """
 import math
 import os
+import types
 
 import numpy as np
 import pytest
 import torch
 
 from tests import helpers as Hh
+from tests import wrapper_ref as WR
 from tests.test_wrapper_cpu import _raw, _rot
 from autovfx_b200 import scene
 
@@ -25,13 +28,64 @@ DEV = "cuda:0"
 def _ref():
     from oracle import ref_py
     if not ref_py.available():
-        pytest.skip("oracle/_ref_py or oracle/_ref not staged (run `make -C oracle ref refpy` where /root/reference exists)")
+        pytest.skip("oracle/_ref_py or oracle/_ref not staged (make -C oracle ref refpy REF=<reference checkout>)")
     return ref_py
 
 
 @pytest.fixture(scope="module")
 def rp():
+    """For the tests that execute the reference's Python code on the drop-in: they need that code staged."""
     return _ref()
+
+
+@pytest.fixture
+def ref_ns():
+    """The reference's Python modules, loaded on first use.  The tests taking this fixture only call it inside the functions
+    they pass to the Hh.ref_* comparisons, which replay stored reference values where the reference is not staged."""
+    Hh.use_ref_python()
+    if not Hh.have_ref():
+        pytest.skip("no staged reference and no stored reference values")
+    cache = {}
+
+    def load():
+        from oracle import ref_py
+        if "ns" not in cache:
+            cache["rp"], cache["ns"] = ref_py, ref_py.load("ref")
+        return cache["rp"], cache["ns"]
+    return load
+
+
+def _once(fn):
+    """fn() evaluated at most once (a reference computation several comparisons read from)."""
+    box = []
+    return lambda: box[0] if box else (box.append(fn()) or box[0])
+
+
+class _Model:
+    """What the reference's GaussianModel exposes to render(): its get_* activations (tests/wrapper_ref.activate, the same torch
+    ops on the same device, hence the same bits) and get_normal (gaussian_model.py:120-128)."""
+
+    def __init__(self, raw, max_sh_degree, active_sh_degree):
+        a = WR.activate({k: v.to(DEV).float().contiguous() for k, v in raw.items()})
+        self.get_xyz, self.get_features, self.get_opacity = a["means3D"], a["shs"], a["opacities"]
+        self.get_scaling, self.get_rotation = a["scales"], a["rotations"]
+        self.max_sh_degree, self.active_sh_degree = max_sh_degree, active_sh_degree
+
+    def get_normal(self, dir_pp_normalized=None):
+        n, _ = WR.flip_align_view(WR.get_minimum_axis(self.get_scaling, self.get_rotation), dir_pp_normalized)
+        return n / n.norm(dim=1, keepdim=True)
+
+
+def _camera(c2w, fx, W, H):
+    """The reference Camera's fields for a c2w pose: matrices from scene.camera_from_c2w (identical, see the camera test) and
+    camera_center = world_view_transform.inverse()[3, :3] on the GPU, as scene/cameras.py computes it."""
+    cam = scene.camera_from_c2w(c2w, fx, fx, W, H)
+    view = cam.world_view_transform.to(DEV)
+    return types.SimpleNamespace(FoVx=cam.FoVx, FoVy=cam.FoVy, image_width=W, image_height=H, world_view_transform=view,
+                                 full_proj_transform=cam.full_proj_transform.to(DEV), camera_center=view.inverse()[3, :3])
+
+
+PIPE = types.SimpleNamespace(debug=False, compute_cov3D_python=False, convert_SHs_python=False)
 
 
 def _scene_raw(N, M, seed, spread=1.0, log_scale=-3.3):
@@ -100,33 +154,39 @@ def test_reference_render_on_dropin_equals_reference_render_on_reference(rp, M, 
 
 
 @pytest.mark.parametrize("M,deg", [(16, 3), (25, 2)])
-def test_fused_render_matches_reference_render(rp, M, deg):
-    """autovfx_b200.renderer.render (axis normals + ONE 6-channel pass + normal-map kernel) fed the reference's own GaussianModel
-    and Camera objects, against the reference's render() on the reference rasterizer."""
+def test_fused_render_matches_reference_render(ref_ns, M, deg):
+    """autovfx_b200.renderer.render (axis normals + ONE 6-channel pass + normal-map kernel) on the parameters and camera of a
+    reference GaussianModel / Camera, against the reference's render() on the reference rasterizer."""
     from autovfx_b200 import rasterizer as R, renderer as RD
-    ref = rp.load("ref")
     raw = _scene_raw(6000, M, 5)
-    Rm, T, fovx, fovy, W, H, _, _ = _cam_args(eye=(-2.0, -2.4, 1.1), W=176, H=96)
+    Rm, T, fovx, fovy, W, H, c2w, fx = _cam_args(eye=(-2.0, -2.4, 1.1), W=176, H=96)
     bg = torch.tensor([0.0, 0.0, 0.0], device=DEV)
-    pc = rp.make_model(ref, raw, int(math.isqrt(M)) - 1, deg)
-    cam = rp.make_camera(ref, Rm, T, fovx, fovy, W, H)
+    pc, cam = _Model(raw, int(math.isqrt(M)) - 1, deg), _camera(c2w, fx, W, H)
+
+    @_once
+    def want():
+        rp, ns = ref_ns()
+        with torch.no_grad():
+            return ns.renderer.render(rp.make_camera(ns, Rm, T, fovx, fovy, W, H), rp.make_model(ns, raw, int(math.isqrt(M)) - 1, deg), rp.Pipe(), bg)
     with torch.no_grad():
-        want = ref.renderer.render(cam, pc, rp.Pipe(), bg)
         R.set_exact_images(True)
         try:
-            got = RD.render(cam, pc, rp.Pipe(), bg)
+            got = RD.render(cam, pc, PIPE, bg)
         finally:
             R.set_exact_images(False)
-        fast = RD.render(cam, pc, rp.Pipe(), bg)
-    assert torch.equal(got["render"], want["render"]) and torch.equal(got["depth"], want["depth"]) and torch.equal(got["radii"], want["radii"])
-    assert torch.equal(got["visibility_filter"], want["visibility_filter"])
-    assert Hh.maxabs(got["normal"], want["normal"]) <= 1e-4  # blended normal image: the per-Gaussian normals differ in the last bit (torch norm reduction order)
-    # pseudo normal: normalised cross product of depth differences (cancellation): compare directions where the normal is defined
-    a, b = got["pseudo_normal"], want["pseudo_normal"]
+        fast = RD.render(cam, pc, PIPE, bg)
+    for k in ("render", "depth", "radii", "visibility_filter"):
+        assert Hh.ref_same(got[k], lambda: want()[k]), k
+    assert Hh.ref_maxabs(got["normal"], lambda: want()["normal"]) <= 1e-4  # blended normal image: per-Gaussian normals differ in the last bit
+    # pseudo normal: normalised cross product of depth differences (cancellation): compare directions where the normal is defined,
+    # against the reference's expression (tests/wrapper_ref.pseudo_normal) on the depth image, which equals the reference's bit for bit
+    a = got["pseudo_normal"]
+    b = WR.pseudo_normal(got["depth"].reshape(H, W), cam.world_view_transform, cam.FoVx, cam.FoVy)
     defined = (b.norm(dim=-1) > 0.5) & (a.norm(dim=-1) > 0.5)
     cos = (a * b).sum(-1)[defined]
     assert defined.float().mean() > 0.5 and float((cos > 1 - 5e-3).float().mean()) > 0.999
-    assert Hh.maxabs(fast["render"], want["render"]) <= 1e-5 and Hh.maxabs(fast["depth"], want["depth"]) <= 5e-5
+    assert Hh.ref_maxabs(fast["render"], lambda: want()["render"]) <= 1e-5 and Hh.ref_maxabs(fast["depth"], lambda: want()["depth"]) <= 5e-5
+    assert Hh.maxabs(fast["render"], got["render"]) <= 1e-5 and Hh.maxabs(fast["depth"], got["depth"]) <= 5e-5  # every pixel
 
 
 def test_training_step_through_reference_render_gradients(rp):
@@ -171,70 +231,84 @@ def test_create_from_pcd_uses_distcuda2(rp):
 
 
 @pytest.mark.parametrize("M", [16, 25])
-def test_activations_match_reference_gaussian_model(rp, M):
+def test_activations_match_reference_gaussian_model(ref_ns, M):
     """edit.activate (gsr_activate_gaussians) vs the reference GaussianModel's get_* properties (gaussian_model.py:95-115)."""
     from autovfx_b200 import edit
-    ns = rp.load("ref")
     raw = _scene_raw(40000, M, 9)
-    pc = rp.make_model(ns, raw, int(math.isqrt(M)) - 1, 0)
+
+    @_once
+    def pc():
+        rp, ns = ref_ns()
+        return rp.make_model(ns, raw, int(math.isqrt(M)) - 1, 0)
     got = edit.activate({k: v.to(DEV) for k, v in raw.items()}, DEV)
     with torch.no_grad():
-        assert torch.equal(got["means3D"], pc.get_xyz) and torch.equal(got["shs"], pc.get_features)
-        assert torch.equal(got["scales"], pc.get_scaling)
-        assert Hh.maxabs(got["opacities"], pc.get_opacity) <= 1.2e-7
-        assert Hh.maxabs(got["rotations"], pc.get_rotation) <= 2.4e-7
+        assert Hh.ref_same(got["means3D"], lambda: pc().get_xyz) and Hh.ref_same(got["shs"], lambda: pc().get_features)
+        assert Hh.ref_same(got["scales"], lambda: pc().get_scaling)
+        assert Hh.ref_maxabs(got["opacities"], lambda: pc().get_opacity) <= 1.2e-7
+        assert Hh.ref_maxabs(got["rotations"], lambda: pc().get_rotation) <= 2.4e-7
 
 
-def test_get_normal_matches_reference(rp):
-    """renderer.axis_normals (gsr_axis_normals) vs GaussianModel.get_normal (gaussian_model.py:120-128)."""
+def test_get_normal_matches_reference(ref_ns):
+    """renderer.axis_normals (gsr_axis_normals) vs GaussianModel.get_normal (gaussian_model.py:120-128), on the model's activations."""
     from autovfx_b200 import renderer as RD
-    ns = rp.load("ref")
     raw = _scene_raw(50000, 16, 13)
-    pc = rp.make_model(ns, raw, 3, 3)
     campos = torch.tensor([0.3, -2.0, 0.7], device=DEV)
+
+    def want():
+        rp, ns = ref_ns()
+        pc = rp.make_model(ns, raw, 3, 3)
+        with torch.no_grad():
+            d = pc.get_xyz - campos
+            return pc.get_normal(dir_pp_normalized=d / d.norm(dim=1, keepdim=True))
+    pc = _Model(raw, 3, 3)
     with torch.no_grad():
-        d = pc.get_xyz - campos
-        d = d / d.norm(dim=1, keepdim=True)
-        want = pc.get_normal(dir_pp_normalized=d)
         got = RD.axis_normals(pc.get_xyz, pc.get_scaling, pc.get_rotation, campos, remap01=False)
-    assert Hh.maxabs(got, want) <= 5e-7
+    assert Hh.ref_maxabs(got, want) <= 5e-7
 
 
-def test_transform_and_merge_match_reference(rp):
+def test_transform_and_merge_match_reference(ref_ns):
     """edit.ResidentScene.compose vs the reference's transform_gaussians + merge_two_gaussians executed from gaussians_utils.py
     (:71-125), then both scenes through the rasterizer."""
-    from autovfx_b200 import edit, rasterizer as R
-    ns = rp.load("ref")
+    from autovfx_b200 import edit
     M = 25
     scene_raw, obj_raw = _scene_raw(8000, M, 1), _scene_raw(1500, M, 2, spread=0.3)
     Rot = _rot(5)
     center, init_c, scaling = torch.tensor([0.4, -0.2, 0.3]), torch.tensor([0.05, 0.02, -0.01]), 1.7
-    bg_model, obj_model = rp.make_model(ns, scene_raw, 4, 0), rp.make_model(ns, obj_raw, 4, 0)
-    with torch.no_grad():
-        moved = ns.gaussians_utils.transform_gaussians(obj_model, center.to(DEV), Rot.to(DEV), scaling, init_c.to(DEV))
-        merged = ns.gaussians_utils.merge_two_gaussians(bg_model, moved)
-        want = {"means3D": merged.get_xyz, "shs": merged.get_features, "opacities": merged.get_opacity, "scales": merged.get_scaling,
-                "rotations": merged.get_rotation}
+
+    @_once
+    def want():
+        rp, ns = ref_ns()
+        bg_model, obj_model = rp.make_model(ns, scene_raw, 4, 0), rp.make_model(ns, obj_raw, 4, 0)
+        with torch.no_grad():
+            moved = ns.gaussians_utils.transform_gaussians(obj_model, center.to(DEV), Rot.to(DEV), scaling, init_c.to(DEV))
+            merged = ns.gaussians_utils.merge_two_gaussians(bg_model, moved)
+            assert merged.active_sh_degree == 0
+            return {"means3D": merged.get_xyz, "shs": merged.get_features, "opacities": merged.get_opacity, "scales": merged.get_scaling,
+                    "rotations": merged.get_rotation}
     rs = edit.ResidentScene({k: v.to(DEV) for k, v in scene_raw.items()}, {"obj": {k: v.to(DEV) for k, v in obj_raw.items()}}, DEV)
     got = rs.compose({"obj": (center, Rot, scaling, init_c)})
-    assert got["means3D"].shape == want["means3D"].shape
-    assert Hh.maxabs(got["means3D"], want["means3D"]) <= 2e-6 and torch.equal(got["shs"], want["shs"])
-    assert Hh.maxabs(got["scales"], want["scales"]) <= 1e-6 * float(want["scales"].max()) + 1e-9
-    assert Hh.maxabs(got["opacities"], want["opacities"]) <= 1.2e-7 and Hh.maxabs(got["rotations"], want["rotations"]) <= 1e-6
+    assert Hh.ref_maxabs(got["means3D"], lambda: want()["means3D"]) <= 2e-6 and Hh.ref_same(got["shs"], lambda: want()["shs"])
+    smax = Hh.ref_value(lambda: float(want()["scales"].max()))
+    assert Hh.ref_maxabs(got["scales"], lambda: want()["scales"]) <= 1e-6 * smax + 1e-9
+    assert Hh.ref_maxabs(got["opacities"], lambda: want()["opacities"]) <= 1.2e-7
+    assert Hh.ref_maxabs(got["rotations"], lambda: want()["rotations"]) <= 1e-6
     # the merged model renders at active_sh_degree 0 (gaussians_utils.py:75 builds GaussianModel(4): active degree 0)
     Rm, T, fovx, fovy, W, H, c2w, fx = _cam_args(W=144, H=96)
     cam = scene.camera_from_c2w(c2w, fx, fx, W, H).to(DEV)
     a = dict(means3D=None, opacities=None, view=cam.world_view_transform, proj=cam.full_proj_transform, campos=cam.camera_center, W=W, H=H,
-             tanfovx=cam.tanfovx, tanfovy=cam.tanfovy, sh_degree=merged.active_sh_degree, scale_modifier=1.0, bg=torch.zeros(3, device=DEV),
+             tanfovx=cam.tanfovx, tanfovy=cam.tanfovy, sh_degree=0, scale_modifier=1.0, bg=torch.zeros(3, device=DEV),
              shs=None, colors_precomp=None, scales=None, rotations=None, cov3D_precomp=None)
-    imgs = []
-    for src in (got, want):
-        b = dict(a)
-        b.update({k: src[k].contiguous() for k in ("means3D", "opacities", "shs", "scales", "rotations")})
-        imgs.append((Hh.run_ours(b, exact=True), Hh.run_ref(b)))
-    for ours_o, ref_o in imgs:  # each parameter set: drop-in == reference rasterizer, bit for bit
-        assert torch.equal(ours_o["color"], ref_o["color"]) and torch.equal(ours_o["radii"], ref_o["radii"])
-    assert Hh.maxabs(imgs[0][0]["color"], imgs[1][1]["color"]) <= 2e-4  # composed on the GPU vs composed by the reference's torch ops
+    b = dict(a)
+    b.update({k: got[k].contiguous() for k in ("means3D", "opacities", "shs", "scales", "rotations")})
+    ours = Hh.run_ours(b, exact=True)
+    ref = Hh.run_ref(b)  # the composed parameters: drop-in == reference rasterizer, bit for bit
+    assert Hh.ref_same(ours["color"], lambda: ref["color"]) and Hh.ref_same(ours["radii"], lambda: ref["radii"])
+
+    def ref_of_reference_merge():  # the reference rasterizer on the scene composed by the reference's torch ops
+        c = dict(a)
+        c.update({k: want()[k].contiguous() for k in ("means3D", "opacities", "shs", "scales", "rotations")})
+        return Hh.run_ref(c)["color"]
+    assert Hh.ref_maxabs(ours["color"], ref_of_reference_merge) <= 2e-4
 
 
 def test_ply_round_trip_with_reference_gaussian_model(rp, tmp_path):
@@ -258,11 +332,11 @@ def test_ply_round_trip_with_reference_gaussian_model(rp, tmp_path):
     assert torch.equal(back._opacity, pc._opacity) and torch.equal(back._scaling, pc._scaling) and torch.equal(back._rotation, pc._rotation)
 
 
-def test_sugar_style_call_offcentre_projection_and_python_sh(rp):
+def test_sugar_style_call_offcentre_projection_and_python_sh(ref_ns):
     """The SuGaR wrapper's call shape (sugar_model.py:2010-2071): M = 25 storage, colours from the reference's Python eval_sh
     (utils/sh_utils.py) passed as colors_precomp, and a projection matrix whose principal point is patched off-centre
     (proj[2,0], proj[2,1] overwritten, sugar_model.py:2029-2030) — drop-in vs compiled reference, bit for bit."""
-    ns = rp.load("ref")
+    from autovfx_b200 import renderer as RD
     g = scene.synthetic_gaussians(20000, seed=77, extent=(1.2, 1.2, 0.6), log_scale_mean=math.log(0.02), log_scale_std=0.5, sh_degree=4)
     cam = scene.lookat_camera((0.5, -3.0, 0.8), (0, 0, 0), 208, 144, 62.0)
     view = cam.world_view_transform.clone()
@@ -275,19 +349,23 @@ def test_sugar_style_call_offcentre_projection_and_python_sh(rp):
         d = a["means3D"] - a["campos"]
         d = d / d.norm(dim=1, keepdim=True)
         shs_view = a["shs"].transpose(1, 2).reshape(-1, 3, 25)
-        rgb = torch.clamp_min(ns.sh_utils.eval_sh(3, shs_view, d) + 0.5, 0.0).contiguous()
+        rgb = torch.clamp_min(RD._eval_sh_torch(3, shs_view, d) + 0.5, 0.0).contiguous()
+        # the reference's Python eval_sh (utils/sh_utils.py), restated in renderer.py for pipe.convert_SHs_python: equal to float rounding
+        assert Hh.ref_maxabs(rgb, lambda: torch.clamp_min(ref_ns()[1].sh_utils.eval_sh(3, shs_view, d) + 0.5, 0.0)) <= 2e-6
     b = dict(a)
     b["shs"], b["colors_precomp"] = None, rgb
     for case in (a, b):  # SH evaluated by the rasterizer at an off-centre projection, and the Python-SH colors_precomp call
         ours, ref = Hh.run_ours(case, exact=True, for_backward=True), Hh.run_ref(case)
         for k in ("color", "depth", "alpha", "radii"):
-            assert torch.equal(ours[k], ref[k]), k
-        Hh.assert_images_close(Hh.run_ours(case), ref)
+            assert Hh.ref_same(ours[k], lambda: ref[k]), k
+        fast = Hh.run_ours(case)
+        Hh.ref_images_close(fast, ref)
+        Hh.assert_images_close(fast, ours)  # every pixel, against the exact images that equal the reference's
     # the CUDA SH evaluation agrees with the reference's Python eval_sh to float rounding
     assert Hh.maxabs(Hh.run_ours(a)["color"], Hh.run_ours(b)["color"]) <= 2e-5
 
 
-def test_config2_one_million_through_the_ply_path(rp, tmp_path):
+def test_config2_one_million_through_the_ply_path(ref_ns, tmp_path):
     """BASELINE config 2 stand-in (SURVEY §8d): P = 1,000,000, seed 1, 4-unit scene, written and re-read through the 3DGS .ply vertex
     layout, activated on the GPU, one 1920x1080 camera, forward — drop-in vs compiled reference, bit for bit (exact image mode),
     and the default mode within tolerance."""
@@ -304,16 +382,22 @@ def test_config2_one_million_through_the_ply_path(rp, tmp_path):
     cam = scene.config2_camera()
     a = Hh.resolve(dict(g=g, cam=cam, sh_degree=3, bg=(0.0, 0.0, 0.0), scale_modifier=1.0), DEV)
     ours, ref = Hh.run_ours(a, exact=True, debug=False), Hh.run_ref(a)
-    assert ref["num_rendered"] == ours["stats"]["num_rendered"] > 1_000_000
+    assert Hh.ref_value(lambda: ref["num_rendered"]) == ours["stats"]["num_rendered"] > 1_000_000
     for k in ("color", "depth", "alpha", "radii"):
-        assert torch.equal(ours[k], ref[k]), k
-    Hh.assert_images_close(Hh.run_ours(a, debug=False), ref)
+        assert Hh.ref_same(ours[k], lambda: ref[k]), k
+    fast = Hh.run_ours(a, debug=False)
+    Hh.ref_images_close(fast, ref)
+    Hh.assert_images_close(fast, ours)  # every pixel, against the exact images that equal the reference's
     # the reference's own loader reads the same file to the same parameters (subset check: its per-property Python loops are slow)
-    ns = rp.load("ref")
     small = str(tmp_path / "small.ply")
     sl = slice(0, 20000)
     scene.save_ply(small, loaded["xyz"][sl], loaded["f_dc"][sl], loaded["f_rest"][sl], loaded["opacity"][sl], loaded["scale"][sl], loaded["rot"][sl])
-    m = ns.gaussian_model.GaussianModel(3)
-    m.load_ply(small)
+
+    @_once
+    def m():
+        mm = ref_ns()[1].gaussian_model.GaussianModel(3)
+        mm.load_ply(small)
+        return mm
     with torch.no_grad():
-        assert torch.equal(m.get_xyz, g["means3D"][sl]) and torch.equal(m.get_features, g["shs"][sl]) and torch.equal(m.get_scaling, g["scales"][sl])
+        assert Hh.ref_same(g["means3D"][sl], lambda: m().get_xyz) and Hh.ref_same(g["shs"][sl], lambda: m().get_features)
+        assert Hh.ref_same(g["scales"][sl], lambda: m().get_scaling)

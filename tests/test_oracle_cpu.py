@@ -132,12 +132,12 @@ def _golden_files():
 
 @pytest.mark.parametrize("path", _golden_files() or [None])
 def test_oracle_against_reference_golden(path):
-    """Golden vectors = outputs of the reference's own CUDA rasterizer (oracle/_ref) on a B200 for the named cases
+    """Golden vectors = outputs of the reference's own CUDA rasterizer (oracle/_ref) for the named cases
     (tests/golden/make_golden.py).  fp32 images agree to 1e-4 (FMA contraction differs between nvcc and gcc);
     integer outputs may differ only where a float sits within an ulp of a rounding boundary."""
     if path is None:
         pytest.skip("no golden fixtures committed yet")
-    gold = np.load(path)
+    gold = Hh.load_golden(path)
     name = str(gold["case"])
     a = Hh.resolve(Hh.case_inputs(name))
     fw = Hh.run_oracle(a)

@@ -135,7 +135,7 @@ def test_transform_and_activate_oracle_vs_torch():
 
 
 def test_wrapper_oracle_against_golden_from_the_gpu():
-    """tests/golden/wrapper_small_sh.npz: the reference's two rasterizer passes (compiled reference, B200) around the wrapper's
+    """tests/golden/wrapper_small_sh.npz: the reference's two rasterizer passes (compiled reference) around the wrapper's
     helper functions executed with torch's CUDA kernels (tests/golden/make_golden.py).  Pins oracle/render_oracle.py."""
     import os
     path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "wrapper_small_sh.npz")
