@@ -59,6 +59,130 @@ def case_inputs(name: str) -> Dict:
     raise KeyError(name)
 
 
+def sh_layout(shs: torch.Tensor, M: int, D: int, offset: bool, tail_seed: int, device=None) -> torch.Tensor:
+    """shs [P,>=16,3] restored in a [P,M,3] layout: the (min(D,3)+1)^2 coefficients degree D reads, then a seeded random tail
+    the rasterizer must ignore.  offset: the rows start 4 bytes past a 16-byte boundary (a [1:] view of a flat buffer of
+    P*M*3+1 floats), the alignment a sliced or concatenated parameter tensor can have."""
+    P = shs.shape[0]
+    n = (min(D, 3) + 1) ** 2
+    out = torch.randn(P, M, 3, generator=torch.Generator().manual_seed(tail_seed)) * 0.3
+    out[:, :n] = shs[:, :n]
+    buf = torch.empty(P * M * 3 + 1, device=device)
+    base = buf[1:] if offset else buf[:-1]
+    base.copy_(out.reshape(-1).to(base.device))
+    return base.view(P, M, 3)
+
+
+def layout_case() -> Dict:
+    """Scene of the SH layout matrix: 3000 Gaussians with 25 stored coefficients, a ragged 123x85 image, DC terms wide enough
+    that about a fifth of the colour channels are clamped at 0."""
+    g = scene.synthetic_gaussians(3000, seed=41, extent=(1, 1, 1), log_scale_mean=math.log(0.035), log_scale_std=0.5, sh_degree=4)
+    g["shs"][:, 0] *= 4.0
+    cam = scene.lookat_camera((0.8, -2.6, 0.9), (0, 0, 0), 123, 85, 62.0)
+    return dict(g=g, cam=cam, sh_degree=3, bg=(0.2, 0.4, 0.1), scale_modifier=1.0)
+
+
+def sort_regimes_case() -> Dict:
+    """16,000 Gaussians in a thin column seen end-on (80x72 image, 25 tiles): tiles of <= 2048 instances (single-pass sort),
+    one of 2048..4096 (one shared-memory sort) and four of > 4096 (chunked sort through global memory)."""
+    g = scene.synthetic_gaussians(16000, seed=13, extent=(0.08, 0.08, 1.0), log_scale_mean=math.log(0.004), log_scale_std=0.3,
+                                  opacity_mean=-3.0, opacity_std=1.0)
+    cam = scene.lookat_camera((0.0, -3.0, 0.0), (0, 0, 0), 80, 72, 40.0)
+    return dict(g=g, cam=cam, sh_degree=3, bg=(0.0, 0.0, 0.0), scale_modifier=1.0)
+
+
+def layout_args(M: Optional[int], D: int, offset: bool, device=None) -> Dict:
+    """The layout case rendered from shs [P,M,3] at degree D (M None: colours precomputed from the degree-3 SH, with scales and
+    rotations)."""
+    a = resolve(layout_case(), device)
+    a["sh_degree"] = D
+    if M is None:
+        gen = torch.Generator().manual_seed(43)
+        a["colors_precomp"] = (torch.rand(a["means3D"].shape[0], 3, generator=gen) * 1.2 - 0.1).to(a["means3D"].device)
+        a["shs"] = None
+    else:
+        a["shs"] = sh_layout(a["shs"].cpu(), M, D, offset, tail_seed=1000 + 31 * M + D + (7 if offset else 0), device=device)
+    return a
+
+
+# Small cases of the per-Gaussian gradient checks, one per SH storage family: (M, D, shs offset by 4 bytes, scale_modifier);
+# "precomp" renders colors_precomp + cov3D_precomp.  Opacity is capped at 0.95 so alpha stays below the 0.99 clamp, whose
+# derivative the reference drops by design.
+GRAD_FAMILIES = {"M1_D0": (1, 0, False, 1.0), "M4_D1": (4, 1, False, 0.9), "M9_D2": (9, 2, False, 1.0), "M16_D3": (16, 3, False, 1.1),
+                 "M25_D3": (25, 3, False, 1.0), "M25_D2_off": (25, 2, True, 1.0), "precomp": (None, 0, False, 1.0)}
+
+
+def grad_args(family: str, device=None, opacity_cap: float = 0.95) -> Dict:
+    M, D, offset, mod = GRAD_FAMILIES[family]
+    g = scene.synthetic_gaussians(400, seed=61 + len(family), extent=(1.6, 1.6, 1), log_scale_mean=math.log(0.07), log_scale_std=0.5,
+                                  sh_degree=4, opacity_mean=0.0, opacity_std=1.5)
+    g["shs"][:, 0] *= 4.0
+    g["opacities"] = g["opacities"].clamp(max=opacity_cap)
+    cam = scene.lookat_camera((0.5, -2.4, 0.7), (0, 0, 0), 70, 54, 50.0)  # a fifth of the Gaussians fall outside the view
+    case = dict(g=g, cam=cam, sh_degree=D, bg=(0.3, 0.1, 0.6), scale_modifier=mod, precomp=M is None)
+    a = resolve(case, device)
+    if M is None:
+        a["colors_precomp"] = (a["colors_precomp"] * 1.2 - 0.1).contiguous()
+    else:
+        a["shs"] = sh_layout(g["shs"], M, D, offset, tail_seed=77, device=device)
+    return a
+
+
+def isolated_image_grads(a: Dict, term: str, device=None):
+    """image_grads with all but one of dL/dcolor, dL/ddepth, dL/dalpha set to zero (term "all" keeps the three)."""
+    dc, dd, da = image_grads(a, device=device)
+    keep = {"color": (1, 0, 0), "depth": (0, 1, 0), "alpha": (0, 0, 1), "all": (1, 1, 1)}[term]
+    return dc * keep[0], dd * keep[1], da * keep[2]
+
+
+def row_errors(g, g64) -> np.ndarray:
+    """Per-Gaussian relative error ||g - g64|| / ||g64|| over the rows whose ||g64|| exceeds 1e-6 of the largest row."""
+    g = torch.as_tensor(g).detach().double().cpu().reshape(g64.shape[0], -1)
+    g64 = torch.as_tensor(g64).detach().double().cpu().reshape(g64.shape[0], -1)
+    n = g64.norm(dim=1)
+    keep = n > 1e-6 * n.max()
+    return ((g - g64).norm(dim=1)[keep] / n[keep]).numpy()
+
+
+def fp64_grads(a: Dict, fw, terms) -> Dict:
+    """{term: {name: fp64 autograd gradient}} of torch_ref.render on the oracle's decisions, for each isolated loss term.  Names
+    follow the oracle's dL_d* keys; dL_dmeans2D holds the pixel gradient scaled to the reference's units (0.5 W, 0.5 H).  The
+    frustum clamp is differentiated as the reference does (Gaussians near the image border differ from the true gradient)."""
+    from tests import torch_ref
+    color, depth, alpha, leaves, m2d = torch_ref.render(a, fw, reference_clamp_grad=True)
+    names = {"means3D": "dL_dmeans3D", "opacities": "dL_dopacity", "shs": "dL_dsh", "scales": "dL_dscales", "rotations": "dL_drotations",
+             "colors_precomp": "dL_dcolors", "cov3D_precomp": "dL_dcov3D"}
+    inputs = [(k, v) for k, v in leaves.items() if v is not None] + [("means2D", m2d)]
+    out = {}
+    for term in terms:
+        dc, dd, da = isolated_image_grads(a, term)
+        loss = (color * dc.double()).sum() + (depth * dd.double()).sum() + (alpha * da.double()).sum()
+        gs = torch.autograd.grad(loss, [v for _, v in inputs], retain_graph=True, allow_unused=True)
+        res = {}
+        for (k, v), gr in zip(inputs, gs):
+            gr = torch.zeros_like(v) if gr is None else gr
+            if k == "means2D":
+                res["dL_dmeans2D"] = gr * torch.tensor([0.5 * a["W"], 0.5 * a["H"]], dtype=torch.float64)
+            else:
+                res[names[k]] = gr
+        out[term] = res
+    return out
+
+
+def comparable_grads(g: Dict, a: Dict) -> Dict:
+    """An oracle-style gradient dict (dL_d* keys) reduced to what fp64_grads holds: dL_dmeans2D without its unused third column, and
+    dL_dscales times scale_modifier (the reference reports the gradient w.r.t. scale_modifier * scale, backward.cu:318-321)."""
+    out = {}
+    for k, v in g.items():
+        v = torch.as_tensor(v).detach().double().cpu()
+        if k == "dL_dmeans2D":
+            v = v[:, :2]
+        elif k == "dL_dscales":
+            v = v * a["scale_modifier"]
+        out[k] = v
+    return out
+
+
 def load_golden(path: str) -> Dict:
     """A golden case; the gradients of the larger cases are stored beside it under golden/grads/ (same file name)."""
     gold = dict(np.load(path))

@@ -35,8 +35,12 @@ def eval_sh(deg, sh, dirs):
     return res
 
 
-def preprocess(means3D, scales, rotations, opacities, shs, view, proj, campos, W, H, tanfovx, tanfovy, sh_degree, scale_modifier):
-    """Continuous per-Gaussian quantities in fp64: means2D [P,2], conic [P,3], rgb [P,3] (clamped at 0), depth [P]."""
+def preprocess(means3D, scales, rotations, opacities, shs, view, proj, campos, W, H, tanfovx, tanfovy, sh_degree, scale_modifier,
+               colors_precomp=None, cov3D_precomp=None, reference_clamp_grad=False):
+    """Continuous per-Gaussian quantities in fp64: means2D [P,2], conic [P,3], rgb [P,3] (SH colours clamped at 0, precomputed
+    colours as given), depth [P].  cov3D_precomp [P,6] (upper triangle, row by row) replaces scales / rotations.
+    reference_clamp_grad: differentiate the +-1.3 tan(fov) clamp of the view-space position as the reference does (the values
+    are the same either way)."""
     P = means3D.shape[0]
     hom = torch.cat([means3D, torch.ones(P, 1, dtype=means3D.dtype)], dim=1)
     p_hom = hom @ proj  # row-vector convention on the row-major buffer (auxiliary.h:58-77)
@@ -45,14 +49,25 @@ def preprocess(means3D, scales, rotations, opacities, shs, view, proj, campos, W
     t = (hom @ view)[:, :3]
     depth = t[:, 2]
     fx, fy = W / (2.0 * tanfovx), H / (2.0 * tanfovy)
-    r, x, y, z = rotations.unbind(-1)
-    R = torch.stack([1 - 2 * (y * y + z * z), 2 * (x * y - r * z), 2 * (x * z + r * y), 2 * (x * y + r * z), 1 - 2 * (x * x + z * z), 2 * (y * z - r * x),
-                     2 * (x * z - r * y), 2 * (y * z + r * x), 1 - 2 * (x * x + y * y)], dim=-1).view(P, 3, 3)
-    L = R * (scales * scale_modifier).unsqueeze(1)
-    Sigma = L @ L.transpose(1, 2)
+    if cov3D_precomp is None:
+        r, x, y, z = rotations.unbind(-1)
+        R = torch.stack([1 - 2 * (y * y + z * z), 2 * (x * y - r * z), 2 * (x * z + r * y), 2 * (x * y + r * z), 1 - 2 * (x * x + z * z),
+                         2 * (y * z - r * x), 2 * (x * z - r * y), 2 * (y * z + r * x), 1 - 2 * (x * x + y * y)], dim=-1).view(P, 3, 3)
+        L = R * (scales * scale_modifier).unsqueeze(1)
+        Sigma = L @ L.transpose(1, 2)
+    else:
+        c = cov3D_precomp
+        Sigma = torch.stack([c[:, 0], c[:, 1], c[:, 2], c[:, 1], c[:, 3], c[:, 4], c[:, 2], c[:, 4], c[:, 5]], dim=-1).view(P, 3, 3)
     limx, limy = 1.3 * tanfovx, 1.3 * tanfovy
     tx = torch.clamp(t[:, 0] / t[:, 2], -limx, limx) * t[:, 2]
     ty = torch.clamp(t[:, 1] / t[:, 2], -limy, limy) * t[:, 2]
+    if reference_clamp_grad:
+        # the reference's backward (backward.cu:175-176, 262-264) treats a clamped t.x (t.y) as a constant: no gradient to t.x and
+        # none through the clamped value's dependence on t.z
+        cx = (t[:, 0] / t[:, 2]).abs() > limx
+        cy = (t[:, 1] / t[:, 2]).abs() > limy
+        tx = torch.where(cx, tx.detach(), tx)
+        ty = torch.where(cy, ty.detach(), ty)
     tz = t[:, 2]
     zero = torch.zeros_like(tz)
     J = torch.stack([fx / tz, zero, -(fx * tx) / (tz * tz), zero, fy / tz, -(fy * ty) / (tz * tz)], dim=-1).view(P, 2, 3)
@@ -66,9 +81,12 @@ def preprocess(means3D, scales, rotations, opacities, shs, view, proj, campos, W
     conic = torch.stack([c / det, -b / det, a / det], dim=-1)
     px = ((p_proj[:, 0] + 1.0) * W - 1.0) * 0.5
     py = ((p_proj[:, 1] + 1.0) * H - 1.0) * 0.5
-    d = means3D - campos[None]
-    d = d / d.norm(dim=1, keepdim=True)
-    rgb = torch.clamp_min(eval_sh(sh_degree, shs, d) + 0.5, 0.0)
+    if colors_precomp is not None:
+        rgb = colors_precomp
+    else:
+        d = means3D - campos[None]
+        d = d / d.norm(dim=1, keepdim=True)
+        rgb = torch.clamp_min(eval_sh(sh_degree, shs, d) + 0.5, 0.0)
     return torch.stack([px, py], dim=-1), conic, rgb, depth
 
 
@@ -112,15 +130,18 @@ def blend(means2D, conic, opac, rgb, depth, ranges, point_list, W, H, bg):
     return color, dimg, aimg
 
 
-def render(a, oracle_fw):
-    """a: resolved case (tests/helpers.resolve) with scales/rotations/shs; returns images + the fp64 leaf tensors."""
-    f64 = lambda t: t.detach().double().clone().requires_grad_(True)  # noqa: E731
-    leaves = {k: f64(a[k]) for k in ("means3D", "scales", "rotations", "opacities", "shs")}
-    view, proj, campos = a["view"].double(), a["proj"].double(), a["campos"].double()
+def render(a, oracle_fw, reference_clamp_grad=False):
+    """a: resolved case (tests/helpers.resolve): shs or colors_precomp, scales/rotations or cov3D_precomp.  Returns the images and
+    the fp64 leaf tensors (one per input the case provides; the absent ones are None)."""
+    f64 = lambda t: None if t is None else t.detach().cpu().double().clone().requires_grad_(True)  # noqa: E731
+    leaves = {k: f64(a[k]) for k in ("means3D", "scales", "rotations", "opacities", "shs", "colors_precomp", "cov3D_precomp")}
+    view, proj, campos = a["view"].cpu().double(), a["proj"].cpu().double(), a["campos"].cpu().double()
     m2d, conic, rgb, depth = preprocess(leaves["means3D"], leaves["scales"], leaves["rotations"], leaves["opacities"], leaves["shs"], view, proj,
-                                        campos, a["W"], a["H"], a["tanfovx"], a["tanfovy"], a["sh_degree"], a["scale_modifier"])
+                                        campos, a["W"], a["H"], a["tanfovx"], a["tanfovy"], a["sh_degree"], a["scale_modifier"],
+                                        colors_precomp=leaves["colors_precomp"], cov3D_precomp=leaves["cov3D_precomp"],
+                                        reference_clamp_grad=reference_clamp_grad)
     m2d.retain_grad()
     ranges = torch.from_numpy(oracle_fw["ranges"].astype(np.int64))
     plist = torch.from_numpy(oracle_fw["point_list"].astype(np.int64))
-    color, dimg, aimg = blend(m2d, conic, leaves["opacities"].reshape(-1), rgb, depth, ranges, plist, a["W"], a["H"], a["bg"].double())
+    color, dimg, aimg = blend(m2d, conic, leaves["opacities"].reshape(-1), rgb, depth, ranges, plist, a["W"], a["H"], a["bg"].cpu().double())
     return color, dimg, aimg, leaves, m2d
