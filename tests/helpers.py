@@ -91,6 +91,201 @@ def sort_regimes_case() -> Dict:
     return dict(g=g, cam=cam, sh_degree=3, bg=(0.0, 0.0, 0.0), scale_modifier=1.0)
 
 
+def faint_slab_case(device=None) -> Dict:
+    """5,000 faint splats (opacity 0.02..0.05) in a slab in front of a wall of 1,400 larger, nearly opaque ones (0.85..0.95), on a
+    ragged 100x74 image.  The wall has a gap on the right, so in the footprints along its edge some pixels terminate at the wall
+    (T < 1e-4) while their neighbours blend to the end of the list; the slab puts over 1,024 entries in front of the wall on the
+    centre tiles.  Stored as SuGaR SH rows (M = 25) 4 bytes off 16-byte alignment, rendered at degree 3 with scale_modifier 1.15.
+    Returns resolved arguments."""
+    gen = torch.Generator().manual_seed(85)
+    slab = scene.synthetic_gaussians(5000, seed=83, extent=(0.45, 0.25, 0.35), log_scale_mean=math.log(0.022), log_scale_std=0.4, sh_degree=4)
+    slab["opacities"] = 0.02 + 0.03 * torch.rand(5000, 1, generator=gen)
+    wall = scene.synthetic_gaussians(2000, seed=89, extent=(1.3, 0.02, 1.0), log_scale_mean=math.log(0.06), log_scale_std=0.3, sh_degree=4)
+    wall["means3D"][:, 1] += 0.7
+    wall["opacities"] = 0.85 + 0.1 * torch.rand(2000, 1, generator=gen)
+    keep = wall["means3D"][:, 0] < 0.25 + 0.2 * wall["means3D"][:, 2]  # the gap: a slanted edge, so it crosses footprints at all offsets
+    g = {k: torch.cat([slab[k], wall[k][keep]]).contiguous() for k in slab}
+    cam = scene.lookat_camera((0.0, -3.0, 0.0), (0, 0, 0), 100, 74, 50.0)
+    a = resolve(dict(g=g, cam=cam, sh_degree=3, bg=(0.1, 0.3, 0.2), scale_modifier=1.15), device)
+    a["shs"] = sh_layout(g["shs"], 25, 3, True, tail_seed=87, device=device)
+    return a
+
+
+BAND_ULPS = 2.0 ** -31  # one ulp of fp32 at 1/255
+BAND_SPLATS = 240
+
+
+def skip_band_case(device=None) -> Dict:
+    """Small splats (their screen footprint is the 0.3-pixel low-pass filter) whose centres lie within 0.3 pixel of a pixel
+    centre on both axes, at least 2 pixels apart, each with the opacity that puts opacity * exp(power) at that pixel on 1/255
+    (fp32), or 1 ulp above or below it, for three in four of them, and 2..34 ulp (up to 4e-6 relative) above or below for the
+    rest.  Every other pixel is at least 0.7 pixel from the centre and far below 1/255, so each splat contributes at its one
+    pixel or nowhere, and no other splat reaches that pixel.  power is evaluated with the GPU forward's rounding sequence
+    (forward_power) on the records the forward computes: the GPU's own (debug_views) when device is a CUDA device, else the
+    oracle's, and exp(power) correctly rounded.  At 0 and 1 ulp the backward's first evaluation (ex2.approx, about 1.5 ulp) often
+    reaches the other decision than expf; its redo with expf must restore the forward's.
+    The first tile holds none of them but a stack of 1,030 faint splats (opacity 0.006) around one pixel, so that one footprint's
+    last contributor is at list position 1,025..1,056: its ballot column ends on a 32-row block of exactly 32 rows.
+    The band splats are the first BAND_SPLATS Gaussians.  Returns resolved arguments."""
+    g = scene.synthetic_gaussians(4000, seed=97, extent=(1.0, 0.3, 0.75), log_scale_mean=math.log(0.002), log_scale_std=0.2, sh_degree=3)
+    cam = scene.lookat_camera((0.0, -3.0, 0.0), (0, 0, 0), 72, 56, 50.0)
+    case = dict(g=g, cam=cam, sh_degree=3, bg=(0.0, 0.0, 0.0), scale_modifier=1.0)
+    if device is not None and torch.device(device).type == "cuda":
+        o = run_ours(resolve(case, device), for_backward=True)
+        rec, vis = o["views"]["records"].cpu().numpy()[:, :6], o["radii"].cpu().numpy() > 0
+    else:
+        pre = run_oracle(resolve(case), stop_after="preprocess")
+        rec, vis = np.concatenate([pre["means2D"], pre["conic_opacity"]], axis=1), pre["radii"] > 0
+    m2 = rec[:, :2]
+    pix = np.rint(m2)
+    cand = np.flatnonzero(vis & (np.abs(m2 - pix) < 0.3).all(axis=1) & (pix >= 1).all(axis=1) & (pix[:, 0] <= 70) &
+                          (pix[:, 1] <= 54) & (pix > 19).any(axis=1))
+    taken, sel = set(), []
+    for i in cand:  # no two centres within one pixel of each other's pixel
+        x, y = int(pix[i, 0]), int(pix[i, 1])
+        if any((x + u, y + v) in taken for u in (-1, 0, 1) for v in (-1, 0, 1)):
+            continue
+        taken.add((x, y))
+        sel.append(i)
+        if len(sel) == BAND_SPLATS:
+            break
+    sel = np.asarray(sel)
+    assert len(sel) == BAND_SPLATS, len(sel)
+    g = {k: v[torch.from_numpy(sel)].contiguous() for k, v in g.items()}
+    E = np.exp(forward_power(rec[sel], pix[sel].astype(np.float32)).astype(np.float64)).astype(np.float32)
+    n = np.arange(BAND_SPLATS)
+    k = np.where(n % 4 < 3, (n % 4) - 1, (2 + (n * 7) % 33) * np.where((n // 4) % 2 == 0, 1, -1)).astype(np.float64)
+    target = np.float32(1.0 / 255.0).astype(np.float64) + k * BAND_ULPS
+    o = (target / E.astype(np.float64)).astype(np.float32)
+    for _ in range(4):  # nudge each opacity until the fp32 product is the target exactly
+        got = (o.astype(np.float64) * E).astype(np.float32).astype(np.float64)
+        o = np.where(got < target, np.nextafter(o, np.float32(1)), np.where(got > target, np.nextafter(o, np.float32(0)), o))
+    g["opacities"] = torch.from_numpy(o.reshape(-1, 1))
+    stack = scene.synthetic_gaussians(1030, seed=101, extent=(0.004, 0.2, 0.004), log_scale_mean=math.log(0.003), log_scale_std=0.2,
+                                      sh_degree=3)
+    stack["means3D"] += torch.tensor([-1.2, 0.0, 0.85])  # near pixel (5, 6)
+    stack["opacities"] = torch.full((1030, 1), 0.006)
+    g = {k: torch.cat([g[k], stack[k]]).contiguous() for k in g}
+    return resolve(dict(case, g=g), device)
+
+
+def band_pixels(a: Dict) -> np.ndarray:
+    """[BAND_SPLATS, 2] (x, y) pixel of each band splat of skip_band_case: the nearest to its projected centre."""
+    from oracle import gsr_oracle  # noqa: F401
+    pre = run_oracle({k: (v.cpu() if isinstance(v, torch.Tensor) else v) for k, v in a.items()}, stop_after="preprocess")
+    return np.rint(pre["means2D"][:BAND_SPLATS]).astype(np.int64)
+
+
+def oracle_power(m2d: np.ndarray, co: np.ndarray, pix: np.ndarray) -> np.ndarray:
+    """power = -0.5 (a dx^2 + c dy^2) - b dx dy in fp32, the oracle's rounding sequence (no fused multiply-add)."""
+    f = np.float32
+    dx = (m2d[..., 0] - pix[..., 0]).astype(f)
+    dy = (m2d[..., 1] - pix[..., 1]).astype(f)
+    return (f(-0.5) * (co[..., 0] * dx * dx + co[..., 2] * dy * dy) - co[..., 1] * dx * dy).astype(f)
+
+
+def forward_power(rec: np.ndarray, pix: np.ndarray) -> np.ndarray:
+    """power in fp32 with the GPU forward's rounding sequence (gsr_blend.cu: products, then two fused multiply-adds), from
+    records [.., {x, y, a, b, c}]; each fma is evaluated exactly in float64 and rounded once."""
+    f, d = np.float32, np.float64
+    dx = (rec[..., 0] - pix[..., 0]).astype(f)
+    dy = (rec[..., 1] - pix[..., 1]).astype(f)
+    t1, t3, t2 = (rec[..., 4] * dy).astype(f), (rec[..., 2] * dx).astype(f), ((-rec[..., 3]) * dx).astype(f)
+    t4, t5 = (dy * t1).astype(f), (dy * t2).astype(f)
+    t6 = (dx.astype(d) * t3 + t4).astype(f)
+    return (t6.astype(d) * -0.5 + t5).astype(f)
+
+
+def band_pairs(rec: np.ndarray, W: int, H: int) -> int:
+    """(pixel, splat) pairs, at the pixel nearest each centre inside the image, where the backward's first evaluation of
+    opacity * exp(power) lands within its redo band |255 alpha - 1| < 8e-6 (checked with a margin: 7e-6).  rec: [P, >= 6]
+    fp32 records {x, y, a, b, c, opacity} of the rendered splats."""
+    pix = np.rint(rec[:, :2]).astype(np.float32)
+    inside = (pix[:, 0] >= 0) & (pix[:, 0] < W) & (pix[:, 1] >= 0) & (pix[:, 1] < H)
+    oG = rec[:, 5].astype(np.float64) * np.exp(forward_power(rec, pix).astype(np.float64))
+    return int((inside & (np.abs(oG * 255.0 - 1.0) < 7e-6)).sum())
+
+
+def footprint_coverage(fw: Dict, W: int, H: int) -> Dict[str, np.ndarray]:
+    """Per 8x4-pixel footprint of the blend backward (16x16 tiles, footprint f at x + 8 (f & 1), y + 4 (f >> 1)), from the oracle's
+    forward: `last`, the list position (1-based) of the furthest last contributor of its pixels; `survivors`, the list entries
+    before it that reach power <= 0 and alpha >= 1/255 at one of its pixels; `mixed`, whether its pixels inside the image have
+    different last contributors; `partial`, whether it has pixels outside the image; `terminated` and `through`, whether one of
+    its pixels stopped at T < 1e-4 (the first list entry it would blend after its last contributor takes T_final (1 - alpha) below
+    1e-4) and whether one blended to the end of its list."""
+    gx, gy = (W + 15) // 16, (H + 15) // 16
+    m2, co, nc = fw["means2D"], fw["conic_opacity"], fw["n_contrib"].astype(np.int64)
+    out = {k: [] for k in ("last", "survivors", "mixed", "partial", "terminated", "through")}
+    T_final = (np.float32(1) - fw["alpha"].reshape(H, W)).astype(np.float32)
+    fx, fy = np.arange(32) % 8, np.arange(32) // 8
+    for tile in range(gx * gy):
+        r0, r1 = (int(v) for v in fw["ranges"][tile])
+        ty, tx = divmod(tile, gx)
+        for f in range(8):
+            px, py = tx * 16 + (f & 1) * 8 + fx, ty * 16 + (f >> 1) * 4 + fy
+            inside = (px < W) & (py < H)
+            lanes = nc[py[inside], px[inside]]
+            last = int(lanes.max()) if lanes.size else 0
+            g = fw["point_list"][r0:r1].astype(np.int64)
+            pix = np.stack([px[inside], py[inside]], axis=-1).astype(np.float32)[None]
+            power = oracle_power(m2[g][:, None], co[g][:, None], pix)
+            alpha = np.minimum(np.float32(0.99), co[g][:, None, 3] * np.exp(power.astype(np.float64)).astype(np.float32))
+            hit = (power <= 0) & (alpha >= np.float32(1.0 / 255.0))
+            # per pixel, the first entry it would blend after its last contributor (index n_contrib), if any
+            after = hit & (np.arange(len(g))[:, None] >= lanes[None])
+            has = after.any(axis=0)
+            first = np.argmax(after, axis=0) if len(g) else np.zeros(len(lanes), np.int64)
+            a_next = alpha[first, np.arange(len(lanes))] if len(g) else np.ones(len(lanes), np.float32)
+            stop = has & (T_final[py[inside], px[inside]] * (np.float32(1) - a_next) < np.float32(1e-4))
+            out["terminated"].append(bool(stop.any()))
+            out["through"].append(bool((~has).any()))
+            out["last"].append(last)
+            out["survivors"].append(int(hit[:last].any(axis=1).sum()) if last else 0)
+            out["mixed"].append(bool(lanes.size and lanes.min() != lanes.max()))
+            out["partial"].append(bool((~inside).any()) and r1 > r0)
+    return {k: np.asarray(v) for k, v in out.items()}
+
+
+# The dense gradient cases (tests/test_gpu_dense_grads.py, pinned on the CPU by tests/test_dense_grads_cpu.py) and the regimes of
+# the blend backward each must reach (coverage_facts): the survivor ring (128 entries) wraps, and wraps twice; a footprint's last
+# contributor lies beyond list position 1024 (more than one 32-row ballot block) or 4096, or at 1025..1056 (+ 1024 k), where the
+# last block holds exactly 32 rows; a footprint beyond position 1024 with a pixel that terminates (T < 1e-4) next to one that
+# blends to the end of its list; footprints with pixels outside the image; (skip_band) splats in the backward's redo band.
+DENSE_CASES = {"skip_band": ("ring", "ring2", "blocks", "block_edge", "band"),
+               "dense_tile": ("ring", "ring2", "blocks", "blocks4096"), "sort_regimes": ("ring", "ring2", "blocks", "blocks4096"),
+               "coplanar": ("ring",), "config1": ("ring", "mixed"),
+               "faint_slab": ("ring", "ring2", "blocks", "mixed", "partial", "terminate_deep")}
+BAND_MIN_PAIRS = 200  # of BAND_SPLATS, each with one candidate pixel
+
+
+def dense_case(name: str, device=None) -> Dict:
+    if name == "faint_slab":
+        return faint_slab_case(device)
+    if name == "skip_band":
+        return skip_band_case(device)
+    return resolve(sort_regimes_case() if name == "sort_regimes" else case_inputs(name), device)
+
+
+def coverage_facts(a: Dict, fw: Dict, records: Optional[np.ndarray] = None) -> Dict[str, bool]:
+    """Which regimes of the blend backward the oracle's forward of a case reaches (see DENSE_CASES).  records: [P, >= 6] fp32
+    {x, y, a, b, c, opacity} of the rendered splats for the redo-band count (default: the oracle's)."""
+    c = footprint_coverage(fw, a["W"], a["H"])
+    if records is None:
+        records = np.concatenate([fw["means2D"], fw["conic_opacity"]], axis=1)[fw["radii"] > 0]
+    return {"ring": bool((c["survivors"] > 128).any()), "ring2": bool((c["survivors"] > 256).any()),
+            "blocks": bool((c["last"] > 1024).any()), "blocks4096": bool((c["last"] > 4096).any()),
+            "block_edge": bool(((c["last"] > 1024) & (((c["last"] - 1) >> 5) % 32 == 0)).any()),
+            "mixed": bool(c["mixed"].any()), "partial": bool((c["partial"] & (c["last"] > 0)).any()),
+            "terminate_deep": bool((c["terminated"] & c["through"] & (c["last"] > 1024)).any()),
+            "band": band_pairs(records, a["W"], a["H"]) >= BAND_MIN_PAIRS}
+
+
+def assert_dense_coverage(name: str, a: Dict, fw: Dict, records: Optional[np.ndarray] = None):
+    facts = coverage_facts(a, fw, records)
+    missing = [k for k in DENSE_CASES[name] if not facts[k]]
+    assert not missing, "%s does not reach %s" % (name, missing)
+
+
 def layout_args(M: Optional[int], D: int, offset: bool, device=None) -> Dict:
     """The layout case rendered from shs [P,M,3] at degree D (M None: colours precomputed from the degree-3 SH, with scales and
     rotations)."""
@@ -144,12 +339,14 @@ def row_errors(g, g64) -> np.ndarray:
     return ((g - g64).norm(dim=1)[keep] / n[keep]).numpy()
 
 
-def fp64_grads(a: Dict, fw, terms) -> Dict:
-    """{term: {name: fp64 autograd gradient}} of torch_ref.render on the oracle's decisions, for each isolated loss term.  Names
+def fp64_grads(a: Dict, fw, terms, oracle_decisions=False) -> Dict:
+    """{term: {name: fp64 autograd gradient}} of torch_ref.render on the oracle's tile lists, for each isolated loss term.  Names
     follow the oracle's dL_d* keys; dL_dmeans2D holds the pixel gradient scaled to the reference's units (0.5 W, 0.5 H).  The
-    frustum clamp is differentiated as the reference does (Gaussians near the image border differ from the true gradient)."""
+    frustum clamp is differentiated as the reference does (Gaussians near the image border differ from the true gradient).
+    oracle_decisions: the skip / terminate decisions are the oracle's fp32 ones, so that a row differs only by arithmetic (else
+    they are taken on the fp64 values)."""
     from tests import torch_ref
-    color, depth, alpha, leaves, m2d = torch_ref.render(a, fw, reference_clamp_grad=True)
+    color, depth, alpha, leaves, m2d = torch_ref.render(a, fw, reference_clamp_grad=True, oracle_decisions=oracle_decisions)
     names = {"means3D": "dL_dmeans3D", "opacities": "dL_dopacity", "shs": "dL_dsh", "scales": "dL_dscales", "rotations": "dL_drotations",
              "colors_precomp": "dL_dcolors", "cov3D_precomp": "dL_dcov3D"}
     inputs = [(k, v) for k, v in leaves.items() if v is not None] + [("means2D", m2d)]

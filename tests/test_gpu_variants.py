@@ -3,9 +3,9 @@
 Which colour + emission kernel runs depends on the SH storage: M coefficients per row, the active degree D (clamped to 3)
 and the alignment of the shs rows (16-byte aligned rows with M % 4 == 0 are staged with vector copies, 16-byte aligned
 rows of other widths through an aligned window when it fits, everything else one float at a time), and the backward's
-Gaussian kernel has a special case for M = 16.  Two more paths are selected per process: GSR_PACKED_KEYS=0 (the general
-sort and emission that scenes of more than 2^24 Gaussians use) and GSR_SH_STAGING=cpasync (LDGSTS staging instead of the
-TMA bulk copy).  This file runs each of them:
+Gaussian kernel has a special case for M = 16.  More paths are selected per process: GSR_PACKED_KEYS=0 (the general
+sort and emission that scenes of more than 2^24 Gaussians use), GSR_SH_STAGING=cpasync (LDGSTS staging instead of the
+TMA bulk copy) and GSR_BWD_OCC=8|5 (the blend backward compiled for other register budgets).  This file runs each of them:
 
   A. the layout matrix: every (M, D) a GaussianModel can store, with shs rows 16-byte aligned and 4 bytes off, against each
      other (bit identity), the CPU oracle, the compiled reference (bit identity in exact mode) and the exact-mode images;
@@ -309,7 +309,8 @@ def test_variant_cases_cover_every_tile_sort_regime(default_outputs):
     assert ((n > 0) & (n <= 2048)).any() and ((n > 2048) & (n <= 4096)).any() and (n > 4096).any()
 
 
-@pytest.mark.parametrize("env", [{"GSR_PACKED_KEYS": "0"}, {"GSR_SH_STAGING": "cpasync"}], ids=["packed_keys_off", "sh_staging_cpasync"])
+@pytest.mark.parametrize("env", [{"GSR_PACKED_KEYS": "0"}, {"GSR_SH_STAGING": "cpasync"}, {"GSR_BWD_OCC": "8"}, {"GSR_BWD_OCC": "5"}],
+                         ids=["packed_keys_off", "sh_staging_cpasync", "bwd_occ_8", "bwd_occ_5"])
 def test_process_variant_matches_the_default_path(dev, default_outputs, env, tmp_path):
     got = _run_variant(env, tmp_path)
     assert sorted(got) == sorted(default_outputs)

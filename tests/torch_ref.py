@@ -90,8 +90,24 @@ def preprocess(means3D, scales, rotations, opacities, shs, view, proj, campos, W
     return torch.stack([px, py], dim=-1), conic, rgb, depth
 
 
-def blend(means2D, conic, opac, rgb, depth, ranges, point_list, W, H, bg):
-    """Blend with the oracle's tile lists; decisions (skip / terminate) are evaluated on detached values."""
+def oracle_hits(fw, ranges, point_list, tile, xx, yy):
+    """[entries, pixels] mask of the list entries of one tile that the oracle's forward blends at each pixel: power <= 0 and
+    alpha >= 1/255 in fp32 (the oracle's rounding sequence, expf correctly rounded), up to the pixel's n_contrib."""
+    from tests.helpers import oracle_power
+    r0, r1 = int(ranges[tile, 0]), int(ranges[tile, 1])
+    g = point_list[r0:r1].numpy()
+    pix = np.stack([xx.reshape(-1).numpy(), yy.reshape(-1).numpy()], axis=-1).astype(np.float32)[None]
+    co = fw["conic_opacity"][g][:, None]
+    power = oracle_power(fw["means2D"][g][:, None], co, pix)
+    alpha = np.minimum(np.float32(0.99), co[..., 3] * np.exp(power.astype(np.float64)).astype(np.float32))
+    last = fw["n_contrib"][yy.reshape(-1).numpy(), xx.reshape(-1).numpy()].astype(np.int64)
+    pos = np.arange(1, r1 - r0 + 1)[:, None]
+    return torch.from_numpy((power <= 0) & (alpha >= np.float32(1.0 / 255.0)) & (pos <= last[None]))
+
+
+def blend(means2D, conic, opac, rgb, depth, ranges, point_list, W, H, bg, decisions=None):
+    """Blend with the oracle's tile lists; decisions (skip / terminate) are evaluated on detached values, or, with decisions (the
+    oracle's forward), taken from the oracle's fp32 evaluation and its n_contrib."""
     color = torch.zeros(3, H, W, dtype=means2D.dtype)
     dimg = torch.zeros(1, H, W, dtype=means2D.dtype)
     aimg = torch.zeros(1, H, W, dtype=means2D.dtype)
@@ -109,16 +125,24 @@ def blend(means2D, conic, opac, rgb, depth, ranges, point_list, W, H, bg):
         C = torch.zeros(n, 3, dtype=means2D.dtype)
         D = torch.zeros(n, dtype=means2D.dtype)
         done = torch.zeros(n, dtype=torch.bool)
+        hits = None if decisions is None else oracle_hits(decisions, ranges, point_list, tile, xx, yy)
         for j in range(int(ranges[tile, 0]), int(ranges[tile, 1])):
+            if hits is not None and not bool(hits[j - int(ranges[tile, 0])].any()):
+                continue  # blended nowhere in the tile: contributes nothing
+            if bool(done.all()):
+                break  # every pixel has terminated: the rest of the list contributes nothing
             g = int(point_list[j])
             dx, dy = means2D[g, 0] - pxf, means2D[g, 1] - pyf
             power = -0.5 * (conic[g, 0] * dx * dx + conic[g, 2] * dy * dy) - conic[g, 1] * dx * dy
             alpha = torch.clamp_max(opac[g] * torch.exp(power), 0.99)
             with torch.no_grad():
-                active = (~done) & (power <= 0) & (alpha >= 1.0 / 255.0)
-                term = active & (T * (1 - alpha) < 0.0001)
-                done = done | term
-                active = active & ~term
+                if hits is not None:
+                    active = hits[j - int(ranges[tile, 0])]
+                else:
+                    active = (~done) & (power <= 0) & (alpha >= 1.0 / 255.0)
+                    term = active & (T * (1 - alpha) < 0.0001)
+                    done = done | term
+                    active = active & ~term
             w = torch.where(active, alpha * T, torch.zeros_like(T))
             C = C + w[:, None] * rgb[g][None]
             D = D + w * depth[g]
@@ -130,9 +154,10 @@ def blend(means2D, conic, opac, rgb, depth, ranges, point_list, W, H, bg):
     return color, dimg, aimg
 
 
-def render(a, oracle_fw, reference_clamp_grad=False):
+def render(a, oracle_fw, reference_clamp_grad=False, oracle_decisions=False):
     """a: resolved case (tests/helpers.resolve): shs or colors_precomp, scales/rotations or cov3D_precomp.  Returns the images and
-    the fp64 leaf tensors (one per input the case provides; the absent ones are None)."""
+    the fp64 leaf tensors (one per input the case provides; the absent ones are None).  oracle_decisions: every skip / terminate
+    decision is the oracle's fp32 one (else each is taken on the fp64 values)."""
     f64 = lambda t: None if t is None else t.detach().cpu().double().clone().requires_grad_(True)  # noqa: E731
     leaves = {k: f64(a[k]) for k in ("means3D", "scales", "rotations", "opacities", "shs", "colors_precomp", "cov3D_precomp")}
     view, proj, campos = a["view"].cpu().double(), a["proj"].cpu().double(), a["campos"].cpu().double()
@@ -143,5 +168,6 @@ def render(a, oracle_fw, reference_clamp_grad=False):
     m2d.retain_grad()
     ranges = torch.from_numpy(oracle_fw["ranges"].astype(np.int64))
     plist = torch.from_numpy(oracle_fw["point_list"].astype(np.int64))
-    color, dimg, aimg = blend(m2d, conic, leaves["opacities"].reshape(-1), rgb, depth, ranges, plist, a["W"], a["H"], a["bg"].cpu().double())
+    color, dimg, aimg = blend(m2d, conic, leaves["opacities"].reshape(-1), rgb, depth, ranges, plist, a["W"], a["H"], a["bg"].cpu().double(),
+                              decisions=oracle_fw if oracle_decisions else None)
     return color, dimg, aimg, leaves, m2d
