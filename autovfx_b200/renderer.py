@@ -10,8 +10,12 @@ frame is
 
     gsr_axis_normals -> gsr_forward_multi (ONE projection/binning/sort/blend pass, 6 colour channels) -> gsr_normal_maps
 
-When gradients are required the reference structure is kept (two autograd rasterizer calls, the second one re-using the
-first one's geometry is not possible under autograd, torch ops for the normal maps), so training code sees the same graph.
+When gradients are required (training: ``train.py`` and the SuGaR trainers put ``normal`` and ``pseudo_normal`` in the loss)
+the two rasterizer calls are one autograd call, ``rasterizer.rasterize_gaussians_multi``: gsr_forward_multi for both colour
+sets, and gsr_backward_multi for both images' gradients in one blend backward (plain gsr_backward when the normal image gets
+no gradient).  The normals fed to it still come from the model's own differentiable ``get_normal``, and the normal
+normalisation and the pseudo-normal stencil are torch ops, so every parameter receives the gradient of the reference's graph
+(two passes summed), up to the order of the floating-point sums.
 
 Same argument names, return keys and error behaviour as the reference function.
 """
@@ -26,7 +30,7 @@ import torch
 from . import _lib
 from ._lib import lib as _L
 from . import rasterizer as R
-from .rasterizer import GaussianRasterizationSettings, GaussianRasterizer
+from .rasterizer import GaussianRasterizationSettings
 
 __all__ = ["render", "axis_normals", "normal_maps", "pack_frame", "fov2focal", "TURBO_LUT_BGR"]
 
@@ -255,19 +259,16 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier:
         return {"render": frame[0:4], "depth": frame[4], "normal": normal_image, "pseudo_normal": pseudo_normal,
                 "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii}
 
-    # ---- gradients required: the reference's graph, op for op, on this package's autograd rasterizer
-    rasterizer = GaussianRasterizer(raster_settings=raster_settings)
+    # ---- gradients required: one differentiable call renders both colour sets (SH colours and normals) on one projection /
+    # binning / sort / blend, and its backward takes both images' gradients in one pass; the rest is the reference's graph
     if dir_pp_normalized is None:
         dir_pp = xyz - viewpoint_camera.camera_center.repeat(pc.get_features.shape[0], 1)
         dir_pp_normalized = dir_pp / dir_pp.norm(dim=1, keepdim=True)
-    rendered_image, depth_image, alpha_image, radii = rasterizer(
-        means3D=means3D, means2D=means2D, shs=shs, colors_precomp=colors_precomp, opacities=opacity, scales=scales, rotations=rotations,
-        cov3D_precomp=cov3D_precomp)
+    normal_normed = pc.get_normal(dir_pp_normalized=dir_pp_normalized) * 0.5 + 0.5
+    rendered_image, depth_image, alpha_image, normal_image, radii = R.rasterize_gaussians_multi(
+        means3D, means2D, shs, colors_precomp, normal_normed, opacity, scales, rotations, cov3D_precomp, raster_settings)
     rendered_image = torch.cat((rendered_image, alpha_image), dim=0)
     depth_image = depth_image.squeeze(0)
-    normal_normed = pc.get_normal(dir_pp_normalized=dir_pp_normalized) * 0.5 + 0.5
-    normal_image = rasterizer(means3D=means3D, means2D=means2D, shs=None, colors_precomp=normal_normed, opacities=opacity, scales=scales,
-                              rotations=rotations, cov3D_precomp=cov3D_precomp)[0]
     normal_image = (normal_image - 0.5) * 2.
     normal_image = torch.nn.functional.normalize(normal_image.permute(1, 2, 0), p=2, dim=-1)
     c2w = viewpoint_camera.world_view_transform.inverse()

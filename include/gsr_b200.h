@@ -14,6 +14,7 @@
  * and, for the render() wrapper around the two rasterizer passes ("GR/" = sugar/gaussian_splatting/gaussian_renderer/__init__.py):
  *
  *   gsr_forward_multi replaces  both rasterizer(...) calls of one frame           GR/:134-166 (same geometry, second colour set)
+ *   gsr_backward_multi replaces both rasterizer backward passes of that frame (training with a loss on the normal image)
  *   gsr_axis_normals  replaces  pc.get_normal(dir_pp_normalized) * 0.5 + 0.5      GR/:131-132,146-147; scene/gaussian_model.py:120-128
  *   gsr_normal_maps   replaces  normal normalisation + depth pseudo normal        GR/:168-191 (depth_pcd2normal GR/:23-38)
  *   gsr_pack_frame    replaces  the per-frame 8-bit conversions before encoding   scene_representation.py:424-438, sugar/render.py:18-22
@@ -208,6 +209,16 @@ typedef struct gsr_grads {
 int gsr_backward(const gsr_frame* frame, const gsr_workspace* ws, const int32_t* radii, const float* out_alpha,
                  const float* dL_dout_color, const float* dL_dout_depth, const float* dL_dout_alpha,
                  const gsr_grads* grads, void* stream);
+
+/* Backward of a frame run through gsr_forward_multi(..., GSR_FLAG_FOR_BACKWARD) with a second colour set: gsr_backward plus
+ * the gradient of the second image.  extra_colors [P,3] is the forward's extra_colors, dL_dout_extra [3,H,W] the gradient of
+ * its out_extra, and dL_dextra [P,3] receives dL/d(extra_colors) (zero-filled by the library).  The geometry gradients in
+ * `grads` are those of the sum of both images' losses: what two gsr_backward calls of two separate passes would add up to,
+ * up to summation order.  All three extra pointers NULL is gsr_backward; only some of them NULL is GSR_ERR_INVALID. */
+int gsr_backward_multi(const gsr_frame* frame, const gsr_workspace* ws, const int32_t* radii, const float* out_alpha,
+                       const float* dL_dout_color, const float* dL_dout_depth, const float* dL_dout_alpha,
+                       const float* extra_colors, const float* dL_dout_extra, float* dL_dextra,
+                       const gsr_grads* grads, void* stream);
 
 /* present[i] = (view-space z of means3D[i] > 0.2)  — checkFrustum, rasterizer_impl.cu:54-66. */
 int gsr_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,
