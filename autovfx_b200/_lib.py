@@ -62,7 +62,7 @@ ABI_VERSION = 4
 EXPORTS = ("gsr_abi_version", "gsr_last_error", "gsr_geom_bytes", "gsr_binning_bytes", "gsr_binning_capacity", "gsr_image_bytes",
            "gsr_forward", "gsr_backward", "gsr_mark_visible", "gsr_dist2_bytes", "gsr_dist2", "gsr_get_views",
            "gsr_profile_begin", "gsr_profile_begin_strided", "gsr_profile_end", "gsr_forward_multi", "gsr_axis_normals", "gsr_normal_maps",
-           "gsr_pack_frame", "gsr_activate_gaussians", "gsr_set_option", "gsr_backward_multi")
+           "gsr_pack_frame", "gsr_activate_gaussians", "gsr_set_option", "gsr_backward_multi", "gsr_activate_gaussians_backward")
 
 
 def _load() -> C.CDLL:
@@ -106,6 +106,8 @@ def _load() -> C.CDLL:
                                    C.c_void_p, C.c_void_p]
     lib.gsr_activate_gaussians.restype = C.c_int
     lib.gsr_activate_gaussians.argtypes = [C.c_int32, C.c_int32] + [C.c_void_p] * 6 + [C.POINTER(gsr_object_xform)] + [C.c_void_p] * 6
+    lib.gsr_activate_gaussians_backward.restype = C.c_int
+    lib.gsr_activate_gaussians_backward.argtypes = [C.c_int32, C.c_int32] + [C.c_void_p] * 17
     lib.gsr_backward.restype = C.c_int
     lib.gsr_backward.argtypes = [C.POINTER(gsr_frame), C.POINTER(gsr_workspace), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p, C.POINTER(gsr_grads), C.c_void_p]

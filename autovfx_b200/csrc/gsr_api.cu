@@ -25,6 +25,10 @@ int backward_impl(const gsr_frame* f, const gsr_workspace* ws, const int32_t* ra
 int compose_impl(int N, int M, const float* xyz, const float* f_dc, const float* f_rest, const float* opacity_raw, const float* scaling_raw,
                  const float* rotation_raw, const gsr_object_xform* xform, float* means3D, float* shs, float* opacities, float* scales,
                  float* rotations, cudaStream_t st);
+int activate_backward_impl(int N, int M, const float* xyz, const float* campos, const float* opacities, const float* scales,
+                           const float* rotations, const float* rotation_raw, const float* g_o, const float* g_s, const float* g_r,
+                           const float* g_sh, const float* g_e, float* d_opacity, float* d_scaling, float* d_rotation, float* d_fdc,
+                           float* d_frest, cudaStream_t st);
 int dist2_impl(int P, const float* points, float* out, void* ws, size_t ws_bytes, cudaStream_t st);
 size_t dist2_bytes(int P);
 int profile_begin(int max_frames, int stride);
@@ -87,6 +91,17 @@ int gsr_activate_gaussians(int32_t N, int32_t M, const float* xyz, const float* 
     NvtxRange nvtx_("gsr_activate_gaussians");
     return gsr::compose_impl(N, M, xyz, f_dc, f_rest, opacity_raw, scaling_raw, rotation_raw, xform, means3D, shs, opacities, scales, rotations,
                              (cudaStream_t)stream);
+}
+
+int gsr_activate_gaussians_backward(int32_t N, int32_t M, const float* xyz, const float* campos, const float* opacities,
+                                    const float* scales, const float* rotations, const float* rotation_raw, const float* dL_dopacities,
+                                    const float* dL_dscales, const float* dL_drotations, const float* dL_dshs, const float* dL_dnormals,
+                                    float* dL_dopacity_raw, float* dL_dscaling_raw, float* dL_drotation_raw, float* dL_df_dc,
+                                    float* dL_df_rest, void* stream) {
+    NvtxRange nvtx_("gsr_activate_gaussians_backward");
+    return gsr::activate_backward_impl(N, M, xyz, campos, opacities, scales, rotations, rotation_raw, dL_dopacities, dL_dscales,
+                                       dL_drotations, dL_dshs, dL_dnormals, dL_dopacity_raw, dL_dscaling_raw, dL_drotation_raw, dL_df_dc,
+                                       dL_df_rest, (cudaStream_t)stream);
 }
 
 int gsr_backward(const gsr_frame* frame, const gsr_workspace* ws, const int32_t* radii, const float* out_alpha,

@@ -304,6 +304,52 @@ __device__ __forceinline__ uint32_t tile_foot_mask_any(float px, float py, float
     return strip_tile_mask(s, tx, ty);
 }
 
+// ---- the shading-normal decision of GaussianModel.get_normal (GM/:120-128, GU/:78-157) ------------------------------------
+// One IEEE rounding per reference torch op, in the reference's order.  Shared by k_axis_normals (the forward) and
+// k_activate_backward, which must differentiate through the very axis and flip the forward chose.
+__device__ __forceinline__ float norm3_rn(float x, float y, float z) {
+    return __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z)));
+}
+struct AxisPick {
+    int k;            // argsort(scales)[0]: the smallest scale, ties to the lowest index (GU/:137)
+    bool flip;        // flip_align_view negated the axis (GU/:151-157)
+    float qn;         // ||r||, the norm build_rotation divides by (no clamp, GU/:79)
+    float w, x, y, z; // r / ||r||
+    float a0, a1, a2; // column k of build_rotation(r), before the flip
+};
+__device__ __forceinline__ AxisPick axis_pick(float s0, float s1, float s2, float q0, float q1, float q2, float q3, float m0, float m1,
+                                              float m2, const float* campos) {
+    AxisPick p;
+    p.k = 0;
+    float sm = s0;
+    if (s1 < sm) { sm = s1; p.k = 1; }
+    if (s2 < sm) { sm = s2; p.k = 2; }
+    // build_rotation (GU/:78-99): normalise, then the k-th COLUMN of R
+    p.qn = __fsqrt_rn(__fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(q0, q0), __fmul_rn(q1, q1)), __fmul_rn(q2, q2)), __fmul_rn(q3, q3)));
+    const float r = __fdiv_rn(q0, p.qn), x = __fdiv_rn(q1, p.qn), y = __fdiv_rn(q2, p.qn), z = __fdiv_rn(q3, p.qn);
+    p.w = r; p.x = x; p.y = y; p.z = z;
+    if (p.k == 0) {
+        p.a0 = __fsub_rn(1.0f, __fmul_rn(2.0f, __fadd_rn(__fmul_rn(y, y), __fmul_rn(z, z))));
+        p.a1 = __fmul_rn(2.0f, __fadd_rn(__fmul_rn(x, y), __fmul_rn(r, z)));
+        p.a2 = __fmul_rn(2.0f, __fsub_rn(__fmul_rn(x, z), __fmul_rn(r, y)));
+    } else if (p.k == 1) {
+        p.a0 = __fmul_rn(2.0f, __fsub_rn(__fmul_rn(x, y), __fmul_rn(r, z)));
+        p.a1 = __fsub_rn(1.0f, __fmul_rn(2.0f, __fadd_rn(__fmul_rn(x, x), __fmul_rn(z, z))));
+        p.a2 = __fmul_rn(2.0f, __fadd_rn(__fmul_rn(y, z), __fmul_rn(r, x)));
+    } else {
+        p.a0 = __fmul_rn(2.0f, __fadd_rn(__fmul_rn(x, z), __fmul_rn(r, y)));
+        p.a1 = __fmul_rn(2.0f, __fsub_rn(__fmul_rn(y, z), __fmul_rn(r, x)));
+        p.a2 = __fsub_rn(1.0f, __fmul_rn(2.0f, __fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y))));
+    }
+    // dir_pp_normalized (GR/:131-132) and flip_align_view (GU/:151-157): keep the axis if it faces the camera
+    const float dx = __fsub_rn(m0, campos[0]), dy = __fsub_rn(m1, campos[1]), dz = __fsub_rn(m2, campos[2]);
+    const float dn = norm3_rn(dx, dy, dz);
+    const float vx = __fdiv_rn(dx, dn), vy = __fdiv_rn(dy, dn), vz = __fdiv_rn(dz, dn);
+    const float dot = __fadd_rn(__fadd_rn(__fmul_rn(p.a0, -vx), __fmul_rn(p.a1, -vy)), __fmul_rn(p.a2, -vz));
+    p.flip = !(dot >= 0.0f);
+    return p;
+}
+
 // SH basis constants (auxiliary.h:22-39)
 constexpr float SH_C0 = 0.28209479177387814f;
 constexpr float SH_C1 = 0.4886025119029199f;

@@ -100,4 +100,100 @@ int compose_impl(int N, int M, const float* xyz, const float* f_dc, const float*
     return check_launch("gsr_activate_gaussians", false, st);
 }
 
+// ---- backward of the activation (xform = NULL) and of the remapped shading normal (gsr_axis_normals(..., remap01 = 1)) ----------
+// Gradients with respect to the activated tensors in, gradients with respect to the raw parameters out.  With s = exp(sigma),
+// r = rho / max(||rho||, 1e-12), o = sigmoid(omega) and e = n * 0.5 + 0.5 the shading normal of the smallest axis:
+//   d sigma = g_s * s,   d omega = g_o * o (1 - o),   d f_dc | d f_rest = split of g_sh (the inverse of k_compose's cat),
+//   d rho   = the Jacobian of F.normalize applied to g_r + (the normal's gradient through build_rotation's own normalisation).
+// The axis k and the flip are piecewise constant; axis_pick recomputes the forward's decisions from the same fp32 inputs.
+struct ActivateBwdParams {
+    int N, M;
+    const float* xyz;            // [N,3] (only with g_e)
+    const float* campos;         // [3]   (only with g_e)
+    const float* opacities;      // [N]   activated
+    const float* scales;         // [N,3] activated
+    const float* rotations;      // [N,4] activated
+    const float* rotation_raw;   // [N,4]
+    const float *g_o, *g_s, *g_r;
+    const float* g_sh;           // [N,M,3] or null (colours precomputed: no SH gradient)
+    const float* g_e;            // [N,3]   or null (the normal image has no gradient)
+    float *d_opacity, *d_scaling, *d_rotation, *d_fdc, *d_frest;
+};
+
+__global__ void __launch_bounds__(256) k_activate_backward(const ActivateBwdParams p) {
+    const int n = blockIdx.x * blockDim.x + threadIdx.x;
+    if (n < p.N) {
+        const size_t n3 = 3 * (size_t)n, n4 = 4 * (size_t)n;
+        const float s0 = p.scales[n3], s1 = p.scales[n3 + 1], s2 = p.scales[n3 + 2];
+        p.d_scaling[n3] = p.g_s[n3] * s0; p.d_scaling[n3 + 1] = p.g_s[n3 + 1] * s1; p.d_scaling[n3 + 2] = p.g_s[n3 + 2] * s2;
+        const float o = p.opacities[n];
+        p.d_opacity[n] = p.g_o[n] * ((1.0f - o) * o);
+        const float r0 = p.rotations[n4], r1 = p.rotations[n4 + 1], r2 = p.rotations[n4 + 2], r3 = p.rotations[n4 + 3];
+        float b0 = p.g_r[n4], b1 = p.g_r[n4 + 1], b2 = p.g_r[n4 + 2], b3 = p.g_r[n4 + 3];  // d r
+        if (p.g_e) {
+            const AxisPick a = axis_pick(s0, s1, s2, r0, r1, r2, r3, p.xyz[n3], p.xyz[n3 + 1], p.xyz[n3 + 2], p.campos);
+            const float sg = a.flip ? -1.0f : 1.0f;
+            const float ia = 1.0f / sqrtf(a.a0 * a.a0 + a.a1 * a.a1 + a.a2 * a.a2);
+            const float m0 = sg * a.a0 * ia, m1 = sg * a.a1 * ia, m2 = sg * a.a2 * ia;  // the unit normal
+            const float e0 = 0.5f * p.g_e[n3], e1 = 0.5f * p.g_e[n3 + 1], e2 = 0.5f * p.g_e[n3 + 2];
+            const float me = m0 * e0 + m1 * e1 + m2 * e2;
+            const float c0 = sg * (e0 - m0 * me) * ia, c1 = sg * (e1 - m1 * me) * ia, c2 = sg * (e2 - m2 * me) * ia;  // d (column k)
+            const float w = a.w, x = a.x, y = a.y, z = a.z;
+            float qw, qx, qy, qz;  // d q^ = (d column / d q^)^T d column
+            if (a.k == 0) {         // (1 - 2(y^2 + z^2), 2(xy + wz), 2(xz - wy))
+                qw = 2.0f * (z * c1 - y * c2); qx = 2.0f * (y * c1 + z * c2);
+                qy = 2.0f * (x * c1 - w * c2) - 4.0f * y * c0; qz = 2.0f * (w * c1 + x * c2) - 4.0f * z * c0;
+            } else if (a.k == 1) {  // (2(xy - wz), 1 - 2(x^2 + z^2), 2(yz + wx))
+                qw = 2.0f * (x * c2 - z * c0); qx = 2.0f * (y * c0 + w * c2) - 4.0f * x * c1;
+                qy = 2.0f * (x * c0 + z * c2); qz = 2.0f * (y * c2 - w * c0) - 4.0f * z * c1;
+            } else {                // (2(xz + wy), 2(yz - wx), 1 - 2(x^2 + y^2))
+                qw = 2.0f * (y * c0 - x * c1); qx = 2.0f * (z * c0 - w * c1) - 4.0f * x * c2;
+                qy = 2.0f * (w * c0 + z * c1) - 4.0f * y * c2; qz = 2.0f * (x * c0 + y * c1);
+            }
+            const float dq = w * qw + x * qx + y * qy + z * qz, iq = 1.0f / a.qn;  // build_rotation's q / ||q||
+            b0 += (qw - w * dq) * iq; b1 += (qx - x * dq) * iq; b2 += (qy - y * dq) * iq; b3 += (qz - z * dq) * iq;
+        }
+        // F.normalize = rho / clamp_min(||rho||, 1e-12): below the clamp the denominator is a constant
+        const float p0 = p.rotation_raw[n4], p1 = p.rotation_raw[n4 + 1], p2 = p.rotation_raw[n4 + 2], p3 = p.rotation_raw[n4 + 3];
+        const float pn = __fsqrt_rn(__fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(p0, p0), __fmul_rn(p1, p1)), __fmul_rn(p2, p2)), __fmul_rn(p3, p3)));
+        if (pn >= 1e-12f) {  // the branch k_compose's fmaxf took
+            const float rb = r0 * b0 + r1 * b1 + r2 * b2 + r3 * b3, ip = 1.0f / pn;
+            b0 = (b0 - r0 * rb) * ip; b1 = (b1 - r1 * rb) * ip; b2 = (b2 - r2 * rb) * ip; b3 = (b3 - r3 * rb) * ip;
+        } else {
+            b0 = b0 / 1e-12f; b1 = b1 / 1e-12f; b2 = b2 / 1e-12f; b3 = b3 / 1e-12f;
+        }
+        p.d_rotation[n4] = b0; p.d_rotation[n4 + 1] = b1; p.d_rotation[n4 + 2] = b2; p.d_rotation[n4 + 3] = b3;
+    }
+    if (!p.g_sh) return;
+    // SH rows: g_sh[n] = cat(d f_dc[n], d f_rest[n]).  The block's 256 rows are split as one flat, coalesced range.
+    const size_t row = (size_t)3 * p.M, rest_row = row - 3;
+    const size_t first = (size_t)blockIdx.x * blockDim.x;
+    const size_t total = min((size_t)blockDim.x, (size_t)p.N - first) * row;
+    const float* src = p.g_sh + first * row;
+    for (size_t j = threadIdx.x; j < total; j += blockDim.x) {
+        const size_t r = j / row, k = j - r * row;
+        if (k < 3) p.d_fdc[(first + r) * 3 + k] = src[j];
+        else p.d_frest[(first + r) * rest_row + (k - 3)] = src[j];
+    }
+}
+
+int activate_backward_impl(int N, int M, const float* xyz, const float* campos, const float* opacities, const float* scales,
+                           const float* rotations, const float* rotation_raw, const float* g_o, const float* g_s, const float* g_r,
+                           const float* g_sh, const float* g_e, float* d_opacity, float* d_scaling, float* d_rotation, float* d_fdc,
+                           float* d_frest, cudaStream_t st) {
+    if (N < 0 || M < 1) { set_error("gsr_activate_gaussians_backward: bad sizes N=%d M=%d", N, M); return GSR_ERR_INVALID; }
+    if (N == 0) return GSR_OK;
+    if (!opacities || !scales || !rotations || !rotation_raw || !g_o || !g_s || !g_r || !d_opacity || !d_scaling || !d_rotation ||
+        (g_e && (!xyz || !campos)) || (g_sh && (!d_fdc || (M > 1 && !d_frest)))) {
+        set_error("gsr_activate_gaussians_backward: null pointer");
+        return GSR_ERR_INVALID;
+    }
+    ActivateBwdParams p{};
+    p.N = N; p.M = M; p.xyz = xyz; p.campos = campos; p.opacities = opacities; p.scales = scales; p.rotations = rotations;
+    p.rotation_raw = rotation_raw; p.g_o = g_o; p.g_s = g_s; p.g_r = g_r; p.g_sh = g_sh; p.g_e = g_e;
+    p.d_opacity = d_opacity; p.d_scaling = d_scaling; p.d_rotation = d_rotation; p.d_fdc = d_fdc; p.d_frest = d_frest;
+    k_activate_backward<<<(N + 255) / 256, 256, 0, st>>>(p);
+    return check_launch("gsr_activate_gaussians_backward", false, st);
+}
+
 }  // namespace gsr

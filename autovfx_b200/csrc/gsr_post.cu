@@ -16,46 +16,16 @@
 
 namespace gsr {
 
-__device__ __forceinline__ float norm3_rn(float x, float y, float z) {
-    return __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z)));
-}
-
 __global__ void __launch_bounds__(256) k_axis_normals(int P, const float* __restrict__ means3D, const float* __restrict__ scales,
                                                       const float* __restrict__ rotations, const float* __restrict__ campos, int remap01,
                                                       float* __restrict__ out) {
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= P) return;
-    const float s0 = scales[3 * (size_t)idx], s1 = scales[3 * (size_t)idx + 1], s2 = scales[3 * (size_t)idx + 2];
-    // argsort(scales)[0]: index of the smallest scale (GU/:137); ties resolve to the lowest index
-    int k = 0;
-    float sm = s0;
-    if (s1 < sm) { sm = s1; k = 1; }
-    if (s2 < sm) { sm = s2; k = 2; }
-    // build_rotation (GU/:78-99): normalise, then the k-th COLUMN of R
-    float q0 = rotations[4 * (size_t)idx], q1 = rotations[4 * (size_t)idx + 1], q2 = rotations[4 * (size_t)idx + 2], q3 = rotations[4 * (size_t)idx + 3];
-    const float qn = __fsqrt_rn(__fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(q0, q0), __fmul_rn(q1, q1)), __fmul_rn(q2, q2)), __fmul_rn(q3, q3)));
-    const float r = __fdiv_rn(q0, qn), x = __fdiv_rn(q1, qn), y = __fdiv_rn(q2, qn), z = __fdiv_rn(q3, qn);
-    float n0, n1, n2;
-    if (k == 0) {
-        n0 = __fsub_rn(1.0f, __fmul_rn(2.0f, __fadd_rn(__fmul_rn(y, y), __fmul_rn(z, z))));
-        n1 = __fmul_rn(2.0f, __fadd_rn(__fmul_rn(x, y), __fmul_rn(r, z)));
-        n2 = __fmul_rn(2.0f, __fsub_rn(__fmul_rn(x, z), __fmul_rn(r, y)));
-    } else if (k == 1) {
-        n0 = __fmul_rn(2.0f, __fsub_rn(__fmul_rn(x, y), __fmul_rn(r, z)));
-        n1 = __fsub_rn(1.0f, __fmul_rn(2.0f, __fadd_rn(__fmul_rn(x, x), __fmul_rn(z, z))));
-        n2 = __fmul_rn(2.0f, __fadd_rn(__fmul_rn(y, z), __fmul_rn(r, x)));
-    } else {
-        n0 = __fmul_rn(2.0f, __fadd_rn(__fmul_rn(x, z), __fmul_rn(r, y)));
-        n1 = __fmul_rn(2.0f, __fsub_rn(__fmul_rn(y, z), __fmul_rn(r, x)));
-        n2 = __fsub_rn(1.0f, __fmul_rn(2.0f, __fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y))));
-    }
-    // dir_pp_normalized (GR/:131-132) and flip_align_view (GU/:151-157): keep the axis if it faces the camera
-    const float dx = __fsub_rn(means3D[3 * (size_t)idx], campos[0]), dy = __fsub_rn(means3D[3 * (size_t)idx + 1], campos[1]),
-                dz = __fsub_rn(means3D[3 * (size_t)idx + 2], campos[2]);
-    const float dn = norm3_rn(dx, dy, dz);
-    const float vx = __fdiv_rn(dx, dn), vy = __fdiv_rn(dy, dn), vz = __fdiv_rn(dz, dn);
-    const float dot = __fadd_rn(__fadd_rn(__fmul_rn(n0, -vx), __fmul_rn(n1, -vy)), __fmul_rn(n2, -vz));
-    if (!(dot >= 0.0f)) { n0 = -n0; n1 = -n1; n2 = -n2; }
+    const AxisPick p = axis_pick(scales[3 * (size_t)idx], scales[3 * (size_t)idx + 1], scales[3 * (size_t)idx + 2], rotations[4 * (size_t)idx],
+                                 rotations[4 * (size_t)idx + 1], rotations[4 * (size_t)idx + 2], rotations[4 * (size_t)idx + 3],
+                                 means3D[3 * (size_t)idx], means3D[3 * (size_t)idx + 1], means3D[3 * (size_t)idx + 2], campos);
+    float n0 = p.a0, n1 = p.a1, n2 = p.a2;
+    if (p.flip) { n0 = -n0; n1 = -n1; n2 = -n2; }
     const float nn = norm3_rn(n0, n1, n2);
     n0 = __fdiv_rn(n0, nn); n1 = __fdiv_rn(n1, nn); n2 = __fdiv_rn(n2, nn);
     if (remap01) {  // normal * 0.5 + 0.5 (GR/:147)

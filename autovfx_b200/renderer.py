@@ -17,6 +17,10 @@ no gradient).  The normals fed to it still come from the model's own differentia
 normalisation and the pseudo-normal stencil are torch ops, so every parameter receives the gradient of the reference's graph
 (two passes summed), up to the order of the floating-point sums.
 
+``render_raw()`` takes the model's raw parameters instead (``_xyz``, ``_features_dc``, ``_features_rest``, ``_opacity``,
+``_scaling``, ``_rotation``): gsr_activate_gaussians and gsr_axis_normals replace the activations and ``get_normal``, and one
+gsr_activate_gaussians_backward launch replaces their autograd graph; the rest of the frame is render()'s.
+
 Same argument names, return keys and error behaviour as the reference function.
 """
 from __future__ import annotations
@@ -32,7 +36,7 @@ from ._lib import lib as _L
 from . import rasterizer as R
 from .rasterizer import GaussianRasterizationSettings
 
-__all__ = ["render", "axis_normals", "normal_maps", "pack_frame", "fov2focal", "TURBO_LUT_BGR"]
+__all__ = ["render", "render_raw", "axis_normals", "normal_maps", "pack_frame", "fov2focal", "TURBO_LUT_BGR"]
 
 
 def fov2focal(fov: float, pixels: float) -> float:
@@ -192,6 +196,24 @@ def _depth_pcd2normal(xyz: torch.Tensor) -> torch.Tensor:
     return torch.nn.functional.pad(n.permute(2, 0, 1), (1, 1, 1, 1), mode="constant").permute(1, 2, 0)
 
 
+def _setup(viewpoint_camera, xyz, sh_degree, pipe, bg_color, scaling_modifier):
+    # zero tensor whose gradient is the screen-space positional gradient (densification statistics, GR/:90-95)
+    screenspace_points = torch.zeros_like(xyz, dtype=xyz.dtype, requires_grad=True, device=xyz.device) + 0
+    try:
+        screenspace_points.retain_grad()
+    except Exception:  # noqa: BLE001
+        pass
+
+    tanfovx = math.tan(viewpoint_camera.FoVx * 0.5)
+    tanfovy = math.tan(viewpoint_camera.FoVy * 0.5)
+    H, W = int(viewpoint_camera.image_height), int(viewpoint_camera.image_width)
+    raster_settings = GaussianRasterizationSettings(
+        image_height=H, image_width=W, tanfovx=tanfovx, tanfovy=tanfovy, bg=bg_color, scale_modifier=scaling_modifier,
+        viewmatrix=viewpoint_camera.world_view_transform, projmatrix=viewpoint_camera.full_proj_transform,
+        sh_degree=sh_degree, campos=viewpoint_camera.camera_center, prefiltered=False, debug=pipe.debug)
+    return screenspace_points, raster_settings
+
+
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier: float = 1.0, override_color=None):
     """Render the scene.  Background tensor (bg_color) must be on GPU!  (GR/:83-218)
 
@@ -206,23 +228,9 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier:
     grad_mode = torch.is_grad_enabled() and any(
         isinstance(t, torch.Tensor) and t.requires_grad
         for t in (xyz, pc.get_opacity, pc.get_scaling, pc.get_rotation, pc.get_features, override_color))
+    screenspace_points, raster_settings = _setup(viewpoint_camera, xyz, pc.active_sh_degree, pipe, bg_color, scaling_modifier)
 
-    # zero tensor whose gradient is the screen-space positional gradient (densification statistics, GR/:90-95)
-    screenspace_points = torch.zeros_like(xyz, dtype=xyz.dtype, requires_grad=True, device=device) + 0
-    try:
-        screenspace_points.retain_grad()
-    except Exception:  # noqa: BLE001
-        pass
-
-    tanfovx = math.tan(viewpoint_camera.FoVx * 0.5)
-    tanfovy = math.tan(viewpoint_camera.FoVy * 0.5)
-    H, W = int(viewpoint_camera.image_height), int(viewpoint_camera.image_width)
-    raster_settings = GaussianRasterizationSettings(
-        image_height=H, image_width=W, tanfovx=tanfovx, tanfovy=tanfovy, bg=bg_color, scale_modifier=scaling_modifier,
-        viewmatrix=viewpoint_camera.world_view_transform, projmatrix=viewpoint_camera.full_proj_transform,
-        sh_degree=pc.active_sh_degree, campos=viewpoint_camera.camera_center, prefiltered=False, debug=pipe.debug)
-
-    means3D, means2D, opacity = xyz, screenspace_points, pc.get_opacity
+    means3D, opacity = xyz, pc.get_opacity
     scales = rotations = cov3D_precomp = None
     if pipe.compute_cov3D_python:
         cov3D_precomp = pc.get_covariance(scaling_modifier)
@@ -242,15 +250,32 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier:
     else:
         colors_precomp = override_color
 
+    if not grad_mode:
+        with torch.no_grad(), torch.cuda.device(device):
+            normal_normed = axis_normals(xyz, pc.get_scaling, pc.get_rotation, viewpoint_camera.camera_center, remap01=True)
+    else:
+        if dir_pp_normalized is None:
+            dir_pp = xyz - viewpoint_camera.camera_center.repeat(pc.get_features.shape[0], 1)
+            dir_pp_normalized = dir_pp / dir_pp.norm(dim=1, keepdim=True)
+        normal_normed = pc.get_normal(dir_pp_normalized=dir_pp_normalized) * 0.5 + 0.5
+    return _frame(viewpoint_camera, raster_settings, screenspace_points, grad_mode, means3D, shs, colors_precomp, normal_normed, opacity,
+                  scales, rotations, cov3D_precomp)
+
+
+def _frame(viewpoint_camera, raster_settings, screenspace_points, grad_mode, means3D, shs, colors_precomp, normal_normed, opacity, scales,
+           rotations, cov3D_precomp):
+    """The rasterizer call and the normal maps of render() and render_raw(), from the tensors the rasterizer takes and the
+    per-Gaussian normals remapped to [0,1]."""
+    device = means3D.device
+    H, W = int(viewpoint_camera.image_height), int(viewpoint_camera.image_width)
     fx, fy = fov2focal(viewpoint_camera.FoVx, W), fov2focal(viewpoint_camera.FoVy, H)
     cx, cy = W / 2, H / 2
 
     if not grad_mode:
-        # ---- one pass: normals kernel -> 6-channel forward -> normal maps
+        # ---- one pass: 6-channel forward -> normal maps
         with torch.no_grad(), torch.cuda.device(device):
-            normal_normed = axis_normals(xyz, pc.get_scaling, pc.get_rotation, viewpoint_camera.camera_center, remap01=True)
             frame = torch.empty((5, H, W), dtype=torch.float32, device=device)  # rgb | alpha | depth: "render" = frame[0:4] without a cat
-            radii = torch.empty((xyz.shape[0],), dtype=torch.int32, device=device)
+            radii = torch.empty((means3D.shape[0],), dtype=torch.int32, device=device)
             _c, _d, _a, normal_img, radii, _ticket = R.forward_multi(
                 means3D, shs, colors_precomp, normal_normed, opacity, scales, rotations, cov3D_precomp, raster_settings,
                 out=(frame[0:3], frame[4:5], frame[3:4], radii))
@@ -261,12 +286,8 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier:
 
     # ---- gradients required: one differentiable call renders both colour sets (SH colours and normals) on one projection /
     # binning / sort / blend, and its backward takes both images' gradients in one pass; the rest is the reference's graph
-    if dir_pp_normalized is None:
-        dir_pp = xyz - viewpoint_camera.camera_center.repeat(pc.get_features.shape[0], 1)
-        dir_pp_normalized = dir_pp / dir_pp.norm(dim=1, keepdim=True)
-    normal_normed = pc.get_normal(dir_pp_normalized=dir_pp_normalized) * 0.5 + 0.5
     rendered_image, depth_image, alpha_image, normal_image, radii = R.rasterize_gaussians_multi(
-        means3D, means2D, shs, colors_precomp, normal_normed, opacity, scales, rotations, cov3D_precomp, raster_settings)
+        means3D, screenspace_points, shs, colors_precomp, normal_normed, opacity, scales, rotations, cov3D_precomp, raster_settings)
     rendered_image = torch.cat((rendered_image, alpha_image), dim=0)
     depth_image = depth_image.squeeze(0)
     normal_image = (normal_image - 0.5) * 2.
@@ -281,3 +302,108 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier:
     pseudo_normal = _depth_pcd2normal(points3D)
     return {"render": rendered_image, "depth": depth_image, "normal": normal_image, "pseudo_normal": pseudo_normal,
             "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii}
+
+
+# ------------------------------------------------------------------------------------------ render_raw()
+_RAW_FIELDS = ("_xyz", "_features_dc", "_features_rest", "_opacity", "_scaling", "_rotation")
+
+
+def _raw_params(pc, pipe) -> Tuple[torch.Tensor, ...]:
+    """pc's raw parameters (_xyz, _features_dc, _features_rest, _opacity, _scaling, _rotation), checked."""
+    missing = [f for f in _RAW_FIELDS if not isinstance(getattr(pc, f, None), torch.Tensor)]
+    if missing:
+        raise ValueError("render_raw: the model has no raw parameter tensor %s" % ", ".join(missing))
+    for attr, fn, name in (("scaling_activation", torch.exp, "torch.exp"), ("opacity_activation", torch.sigmoid, "torch.sigmoid"),
+                           ("rotation_activation", torch.nn.functional.normalize, "torch.nn.functional.normalize")):
+        if getattr(pc, attr, None) is not fn:
+            raise ValueError("render_raw: pc.%s must be %s, the activation this path differentiates" % (attr, name))
+    for flag in ("compute_cov3D_python", "convert_SHs_python"):
+        if getattr(pipe, flag, False):
+            raise ValueError("render_raw: pipe.%s selects the torch arithmetic render_raw replaces; use render()" % flag)
+    xyz, f_dc, f_rest, opacity, scaling, rotation = (getattr(pc, f) for f in _RAW_FIELDS)
+    P = xyz.shape[0]
+    want = {"_xyz": (P, 3), "_features_dc": (P, 1, 3), "_opacity": (P, 1), "_scaling": (P, 3), "_rotation": (P, 4)}
+    for f, t in zip(_RAW_FIELDS, (xyz, f_dc, f_rest, opacity, scaling, rotation)):
+        if t.device != xyz.device or t.dtype != torch.float32:
+            raise ValueError("render_raw: pc.%s must be float32 on %s" % (f, xyz.device))
+        if f in want and tuple(t.shape) != want[f]:
+            raise ValueError("render_raw: pc.%s has shape %s, expected %s" % (f, tuple(t.shape), want[f]))
+    if f_rest.dim() != 3 or f_rest.shape[0] != P or f_rest.shape[2] != 3:
+        raise ValueError("render_raw: pc._features_rest has shape %s, expected [%d, M-1, 3]" % (tuple(f_rest.shape), P))
+    if not xyz.is_cuda:
+        raise RuntimeError("autovfx_b200.renderer: CUDA tensors required (there is no CPU path)")
+    return xyz, f_dc, f_rest, opacity, scaling, rotation
+
+
+class _ActivateRaw(torch.autograd.Function):
+    """Raw parameters -> (shs, opacities, scales, rotations, normals * 0.5 + 0.5): gsr_activate_gaussians, then gsr_axis_normals
+    on its output.  The backward is one gsr_activate_gaussians_backward launch.  _xyz and campos get no gradient here: the
+    axis and its flip are piecewise constant, so the rasterizer's dL/dmeans3D is _xyz's whole gradient."""
+
+    @staticmethod
+    def forward(ctx, xyz, f_dc, f_rest, opacity, scaling, rotation, campos):
+        device = xyz.device
+        P, M = xyz.shape[0], f_rest.shape[1] + 1
+        xyz, f_dc, f_rest, opacity, scaling, rotation = (t.detach().contiguous() for t in (xyz, f_dc, f_rest, opacity, scaling, rotation))
+        campos = _f32c(campos.detach(), device)
+        f = dict(dtype=torch.float32, device=device)
+        shs, opacities, scales, rotations = torch.empty((P, M, 3), **f), torch.empty((P, 1), **f), torch.empty((P, 3), **f), torch.empty((P, 4), **f)
+        normals = torch.empty((P, 3), **f)
+        means = torch.empty((P, 3), **f)  # the kernel's copy of the positions; the rasterizer reads _xyz itself
+        p = R._ptr
+        with torch.cuda.device(device):
+            st = _stream(device)
+            _lib.check(_L.gsr_activate_gaussians(P, M, p(xyz), p(f_dc), p(f_rest), p(opacity), p(scaling), p(rotation), None, p(means),
+                                                 p(shs), p(opacities), p(scales), p(rotations), st), "gsr_activate_gaussians")
+            _lib.check(_L.gsr_axis_normals(P, p(xyz), p(scales), p(rotations), campos.data_ptr(), 1, p(normals), st), "gsr_axis_normals")
+        ctx.save_for_backward(opacities, scales, rotations, rotation, xyz, campos)
+        ctx.M = M
+        ctx.set_materialize_grads(False)  # no SH gradient (override_color) / no normal-image gradient arrive as None
+        return shs, opacities, scales, rotations, normals
+
+    @staticmethod
+    def backward(ctx, g_shs, g_opacities, g_scales, g_rotations, g_normals):
+        opacities, scales, rotations, rotation, xyz, campos = ctx.saved_tensors
+        device, P, M = xyz.device, xyz.shape[0], ctx.M
+        f = dict(dtype=torch.float32, device=device)
+
+        def grad_in(g, like):
+            return torch.zeros_like(like) if g is None else _f32c(g, device)
+        g_opacities, g_scales, g_rotations = grad_in(g_opacities, opacities), grad_in(g_scales, scales), grad_in(g_rotations, rotations)
+        g_shs = None if g_shs is None else _f32c(g_shs, device)
+        g_normals = None if g_normals is None else _f32c(g_normals, device)
+        d_op, d_sc, d_rot = torch.empty((P, 1), **f), torch.empty((P, 3), **f), torch.empty((P, 4), **f)
+        d_dc = d_rest = None
+        if g_shs is not None:
+            d_dc, d_rest = torch.empty((P, 1, 3), **f), torch.empty((P, M - 1, 3), **f)
+        p = R._ptr
+        with torch.cuda.device(device):
+            rc = _L.gsr_activate_gaussians_backward(P, M, p(xyz), campos.data_ptr(), p(opacities), p(scales), p(rotations), p(rotation),
+                                                    p(g_opacities), p(g_scales), p(g_rotations), p(g_shs), p(g_normals), p(d_op), p(d_sc),
+                                                    p(d_rot), p(d_dc), p(d_rest), _stream(device))
+            _lib.check(rc, "gsr_activate_gaussians_backward")
+        return None, d_dc, d_rest, d_op, d_sc, d_rot, None
+
+
+def render_raw(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier: float = 1.0, override_color=None):
+    """render() from the model's RAW parameters, differentiable with respect to them: ``pc._xyz [P,3]``, ``_features_dc [P,1,3]``,
+    ``_features_rest [P,M-1,3]`` (M = 1 allowed), ``_opacity [P,1]``, ``_scaling [P,3]`` (log) and ``_rotation [P,4]``.
+
+    Same arguments, return keys and shapes as render().  The activations (exp, F.normalize, sigmoid, cat) and the shading
+    normals of ``get_normal`` are one gsr_activate_gaussians and one gsr_axis_normals launch, and their backward is one
+    gsr_activate_gaussians_backward launch, instead of the model's torch ops and their autograd graph.  The arithmetic is the
+    library's (``edit.activate``, ``axis_normals``), not the model's own torch calls, so the model must use the reference's
+    activations (``scaling_activation = torch.exp``, ``opacity_activation = torch.sigmoid``, ``rotation_activation =
+    F.normalize``) and ``pipe`` must not select ``compute_cov3D_python`` or ``convert_SHs_python``; otherwise ValueError.
+    With ``override_color`` the SH coefficients get no gradient."""
+    xyz, f_dc, f_rest, opacity_raw, scaling_raw, rotation_raw = _raw_params(pc, pipe)
+    grad_mode = torch.is_grad_enabled() and any(
+        isinstance(t, torch.Tensor) and t.requires_grad for t in (xyz, f_dc, f_rest, opacity_raw, scaling_raw, rotation_raw, override_color))
+    screenspace_points, raster_settings = _setup(viewpoint_camera, xyz, pc.active_sh_degree, pipe, bg_color, scaling_modifier)
+    with torch.set_grad_enabled(grad_mode):
+        shs, opacity, scales, rotations, normal_normed = _ActivateRaw.apply(xyz, f_dc, f_rest, opacity_raw, scaling_raw, rotation_raw,
+                                                                            viewpoint_camera.camera_center)
+    if override_color is not None:
+        shs = None
+    return _frame(viewpoint_camera, raster_settings, screenspace_points, grad_mode, xyz, shs, override_color, normal_normed, opacity,
+                  scales, rotations, None)

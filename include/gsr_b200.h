@@ -21,6 +21,7 @@
  *   gsr_activate_gaussians replaces the activations of every render call and the per-frame object edit
  *                               get_scaling/get_rotation/get_opacity/get_features   sugar/gaussian_splatting/scene/gaussian_model.py:95-115
  *                               transform_gaussians + merge_two_gaussians            gaussians_utils.py:71-125, scene_representation.py:357-371
+ *   gsr_activate_gaussians_backward replaces the autograd backward of those activations and of get_normal * 0.5 + 0.5
  *
  * Conventions (same as the reference's C++ layer):
  *   - every pointer is a DEVICE pointer to contiguous fp32 / int32 data unless it says "host";
@@ -186,6 +187,19 @@ typedef struct gsr_object_xform {
 int gsr_activate_gaussians(int32_t N, int32_t M, const float* xyz, const float* f_dc, const float* f_rest, const float* opacity_raw,
                            const float* scaling_raw, const float* rotation_raw, const gsr_object_xform* xform, float* means3D,
                            float* shs, float* opacities, float* scales, float* rotations, void* stream);
+
+/* Backward of gsr_activate_gaussians (xform NULL) together with gsr_axis_normals(xyz, scales, rotations, campos, remap01 = 1) on
+ * its outputs: gradients with respect to the activated tensors in, gradients with respect to the raw parameters out.
+ * opacities / scales / rotations are the activated values, rotation_raw the raw quaternions [N,4].  dL_dopacities [N],
+ * dL_dscales [N,3], dL_drotations [N,4] are required; dL_dshs [N,M,3] may be NULL (then dL_df_dc / dL_df_rest are not written),
+ * dL_dnormals [N,3] (the gradient of the remapped normals) may be NULL (then xyz and campos are not read).  Outputs:
+ * dL_dopacity_raw [N], dL_dscaling_raw [N,3], dL_drotation_raw [N,4], dL_df_dc [N,1,3], dL_df_rest [N,M-1,3] (unused when M == 1).
+ * The smallest axis and the flip towards campos are the forward's decisions, recomputed from the same values. */
+int gsr_activate_gaussians_backward(int32_t N, int32_t M, const float* xyz, const float* campos, const float* opacities,
+                                    const float* scales, const float* rotations, const float* rotation_raw, const float* dL_dopacities,
+                                    const float* dL_dscales, const float* dL_drotations, const float* dL_dshs, const float* dL_dnormals,
+                                    float* dL_dopacity_raw, float* dL_dscaling_raw, float* dL_drotation_raw, float* dL_df_dc,
+                                    float* dL_df_rest, void* stream);
 
 /* Gradient buffers, all caller-allocated; the library zero-fills what it accumulates into (the
  * reference's torch::zeros, rasterize_points.cu:158-168).  dL_dsh may be NULL when shs is NULL,
