@@ -15,6 +15,10 @@ int forward_impl(const gsr_frame* f, const gsr_workspace* ws, float* out_color, 
                  int32_t* radii, const float* extra_colors, float* out_extra, int flags, cudaStream_t st);
 int axis_normals_impl(int P, const float* means3D, const float* scales, const float* rotations, const float* campos, int remap01,
                       float* out, cudaStream_t st);
+int sugar_normals_impl(int P, const float* positions, const float* scales, const float* quaternions, const float* campos, float* out,
+                       cudaStream_t st);
+int sugar_normals_backward_impl(int P, const float* positions, const float* scales, const float* quaternions, const float* campos,
+                                const float* dL_dnormals, float* dL_dquaternions, cudaStream_t st);
 int normal_maps_impl(int W, int H, const float* normal_img, const float* depth, const float* c2w, float fx, float fy, float cx, float cy,
                      float* out_normal, float* out_pseudo, cudaStream_t st);
 int pack_frame_impl(int W, int H, const float* rgb, const float* alpha, const float* depth, const float* normal_hwc, float depth_scale,
@@ -71,6 +75,18 @@ int gsr_axis_normals(int32_t P, const float* means3D, const float* scales, const
                      float* out, void* stream) {
     NvtxRange nvtx_("gsr_axis_normals");
     return gsr::axis_normals_impl(P, means3D, scales, rotations, campos, remap01, out, (cudaStream_t)stream);
+}
+
+int gsr_sugar_normals(int32_t P, const float* positions, const float* scales, const float* quaternions, const float* campos, float* out,
+                      void* stream) {
+    NvtxRange nvtx_("gsr_sugar_normals");
+    return gsr::sugar_normals_impl(P, positions, scales, quaternions, campos, out, (cudaStream_t)stream);
+}
+
+int gsr_sugar_normals_backward(int32_t P, const float* positions, const float* scales, const float* quaternions, const float* campos,
+                               const float* dL_dnormals, float* dL_dquaternions, void* stream) {
+    NvtxRange nvtx_("gsr_sugar_normals_backward");
+    return gsr::sugar_normals_backward_impl(P, positions, scales, quaternions, campos, dL_dnormals, dL_dquaternions, (cudaStream_t)stream);
 }
 
 int gsr_normal_maps(int32_t W, int32_t H, const float* normal_img, const float* depth, const float* c2w, float fx, float fy, float cx,

@@ -350,6 +350,50 @@ __device__ __forceinline__ AxisPick axis_pick(float s0, float s1, float s2, floa
     return p;
 }
 
+// ---- SuGaR's shading-normal decision (sugar_model.py:801-815 get_smallest_axis, :2164-2168; GU/:151-157) -------------------------
+// Not get_normal: the rotation is pytorch3d's quaternion_to_matrix of the RAW quaternion (two_s = 2 / |q|^2, no normalisation),
+// the axis is torch.min(scaling, dim=-1)'s index (ties: the lowest index), and the view direction is F.normalize'd (1e-12 clamp).
+// One IEEE rounding per torch op, in torch's order.  Shared by k_sugar_normals and k_sugar_normals_backward.
+struct SugarAxisPick {
+    int k;            // scaling.min(dim=-1)[1]
+    bool flip;        // flip_align_view negated the axis
+    float two_s;      // 2 / (r^2 + i^2 + j^2 + k^2), as torch evaluates `2.0 / t`: reciprocal(t) * 2
+    float a0, a1, a2; // column k of quaternion_to_matrix(q), before the flip
+};
+__device__ __forceinline__ SugarAxisPick sugar_axis_pick(float s0, float s1, float s2, float r, float i, float j, float k, float m0,
+                                                         float m1, float m2, const float* campos) {
+    SugarAxisPick p;
+    p.k = 0;
+    float sm = s0;
+    if (s1 < sm) { sm = s1; p.k = 1; }
+    if (s2 < sm) { sm = s2; p.k = 2; }
+    // (q * q).sum(-1), left to right, then 2.0 / that
+    const float ss = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(r, r), __fmul_rn(i, i)), __fmul_rn(j, j)), __fmul_rn(k, k));
+    const float t = __fmul_rn(__frcp_rn(ss), 2.0f);
+    p.two_s = t;
+    // o = stack(1 - t(jj+kk), t(ij-kr), t(ik+jr), t(ij+kr), 1 - t(ii+kk), t(jk-ir), t(ik-jr), t(jk+ir), 1 - t(ii+jj)).view(3,3)
+    if (p.k == 0) {
+        p.a0 = __fsub_rn(1.0f, __fmul_rn(t, __fadd_rn(__fmul_rn(j, j), __fmul_rn(k, k))));
+        p.a1 = __fmul_rn(t, __fadd_rn(__fmul_rn(i, j), __fmul_rn(k, r)));
+        p.a2 = __fmul_rn(t, __fsub_rn(__fmul_rn(i, k), __fmul_rn(j, r)));
+    } else if (p.k == 1) {
+        p.a0 = __fmul_rn(t, __fsub_rn(__fmul_rn(i, j), __fmul_rn(k, r)));
+        p.a1 = __fsub_rn(1.0f, __fmul_rn(t, __fadd_rn(__fmul_rn(i, i), __fmul_rn(k, k))));
+        p.a2 = __fmul_rn(t, __fadd_rn(__fmul_rn(j, k), __fmul_rn(i, r)));
+    } else {
+        p.a0 = __fmul_rn(t, __fadd_rn(__fmul_rn(i, k), __fmul_rn(j, r)));
+        p.a1 = __fmul_rn(t, __fsub_rn(__fmul_rn(j, k), __fmul_rn(i, r)));
+        p.a2 = __fsub_rn(1.0f, __fmul_rn(t, __fadd_rn(__fmul_rn(i, i), __fmul_rn(j, j))));
+    }
+    // render_directions = F.normalize(positions - camera_center, dim=-1); keep the axis if dot(axis, -dir) >= 0
+    const float dx = __fsub_rn(m0, campos[0]), dy = __fsub_rn(m1, campos[1]), dz = __fsub_rn(m2, campos[2]);
+    const float dn = fmaxf(norm3_rn(dx, dy, dz), 1e-12f);
+    const float vx = __fdiv_rn(dx, dn), vy = __fdiv_rn(dy, dn), vz = __fdiv_rn(dz, dn);
+    const float dot = __fadd_rn(__fadd_rn(__fmul_rn(p.a0, -vx), __fmul_rn(p.a1, -vy)), __fmul_rn(p.a2, -vz));
+    p.flip = !(dot >= 0.0f);
+    return p;
+}
+
 // SH basis constants (auxiliary.h:22-39)
 constexpr float SH_C0 = 0.28209479177387814f;
 constexpr float SH_C1 = 0.4886025119029199f;

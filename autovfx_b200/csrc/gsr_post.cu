@@ -5,6 +5,8 @@
 //   k_axis_normals   per-Gaussian shading normal = shortest axis of the Gaussian, flipped towards the camera
 //                    (GaussianModel.get_normal, scene/gaussian_model.py:120-128; GU/:78-99,136-157), optionally remapped
 //                    to [0,1] (GR/:147) — the colors_precomp of the reference's second pass
+//   k_sugar_normals  the same for SuGaR's wrapper (sugar_scene/sugar_model.py:2164-2168): quaternion_to_matrix of the raw
+//                    quaternion, min-scale axis, flip, * 0.5 + 0.5; k_sugar_normals_backward gives its quaternion gradient
 //   k_normal_maps    rendered normal image -> unit normals [H,W,3] (GR/:168-176) and the pseudo normal from the depth map
 //                    (depth_pcd2normal + get_ray_directions, GR/:23-38,41-80,178-191)
 //   k_pack_frame     8-bit hand-off of a finished frame: RGBA (torchvision.utils.save_image rounding), normal map and
@@ -32,6 +34,62 @@ __global__ void __launch_bounds__(256) k_axis_normals(int P, const float* __rest
         n0 = __fadd_rn(__fmul_rn(n0, 0.5f), 0.5f); n1 = __fadd_rn(__fmul_rn(n1, 0.5f), 0.5f); n2 = __fadd_rn(__fmul_rn(n2, 0.5f), 0.5f);
     }
     out[3 * (size_t)idx] = n0; out[3 * (size_t)idx + 1] = n1; out[3 * (size_t)idx + 2] = n2;
+}
+
+// SuGaR's per-Gaussian shading normal (sugar_model.py:2164-2168): get_smallest_axis, flip_align_view towards camera_center,
+// division by the norm (no epsilon), then normal * 0.5 + 0.5.  positions / scales / quaternions as SuGaR's getters return them.
+__global__ void __launch_bounds__(256) k_sugar_normals(int P, const float* __restrict__ positions, const float* __restrict__ scales,
+                                                       const float* __restrict__ quaternions, const float* __restrict__ campos,
+                                                       float* __restrict__ out) {
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= P) return;
+    const size_t n3 = 3 * (size_t)idx, n4 = 4 * (size_t)idx;
+    const SugarAxisPick p = sugar_axis_pick(scales[n3], scales[n3 + 1], scales[n3 + 2], quaternions[n4], quaternions[n4 + 1],
+                                            quaternions[n4 + 2], quaternions[n4 + 3], positions[n3], positions[n3 + 1], positions[n3 + 2],
+                                            campos);
+    float n0 = p.a0, n1 = p.a1, n2 = p.a2;
+    if (p.flip) { n0 = -n0; n1 = -n1; n2 = -n2; }
+    const float nn = norm3_rn(n0, n1, n2);
+    n0 = __fdiv_rn(n0, nn); n1 = __fdiv_rn(n1, nn); n2 = __fdiv_rn(n2, nn);
+    out[n3] = __fadd_rn(__fmul_rn(n0, 0.5f), 0.5f);
+    out[n3 + 1] = __fadd_rn(__fmul_rn(n1, 0.5f), 0.5f);
+    out[n3 + 2] = __fadd_rn(__fmul_rn(n2, 0.5f), 0.5f);
+}
+
+// Its backward with respect to the raw quaternion q = (r, i, j, k).  With the column a = base + sigma * t * u(q) (base = 1 and
+// sigma = -1 on the diagonal entry, 0 and +1 elsewhere), t = 2 / |q|^2 and dt/dq = -t^2 q:
+//   c = dL/da = sign * (e - m (m.e)) / |a|,   e = 0.5 * dL/dout,   m the unit normal,
+//   dL/dq = t * sum_l sigma_l c_l du_l/dq - t^2 * (sum_l sigma_l c_l u_l) * q.
+// The axis k and the flip are piecewise constant in positions and scales, which therefore get no gradient here;
+// sugar_axis_pick recomputes the forward's decisions from the same fp32 inputs.
+__global__ void __launch_bounds__(256) k_sugar_normals_backward(int P, const float* __restrict__ positions, const float* __restrict__ scales,
+                                                                const float* __restrict__ quaternions, const float* __restrict__ campos,
+                                                                const float* __restrict__ dL_dout, float* __restrict__ dL_dq) {
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= P) return;
+    const size_t n3 = 3 * (size_t)idx, n4 = 4 * (size_t)idx;
+    const float r = quaternions[n4], i = quaternions[n4 + 1], j = quaternions[n4 + 2], k = quaternions[n4 + 3];
+    const SugarAxisPick a = sugar_axis_pick(scales[n3], scales[n3 + 1], scales[n3 + 2], r, i, j, k, positions[n3], positions[n3 + 1],
+                                            positions[n3 + 2], campos);
+    const float sg = a.flip ? -1.0f : 1.0f;
+    const float ia = 1.0f / sqrtf(a.a0 * a.a0 + a.a1 * a.a1 + a.a2 * a.a2);
+    const float m0 = sg * a.a0 * ia, m1 = sg * a.a1 * ia, m2 = sg * a.a2 * ia;
+    const float e0 = 0.5f * dL_dout[n3], e1 = 0.5f * dL_dout[n3 + 1], e2 = 0.5f * dL_dout[n3 + 2];
+    const float me = m0 * e0 + m1 * e1 + m2 * e2;
+    const float c0 = sg * (e0 - m0 * me) * ia, c1 = sg * (e1 - m1 * me) * ia, c2 = sg * (e2 - m2 * me) * ia;
+    float gr, gi, gj, gk, su;  // sum_l sigma_l c_l du_l/dq and sum_l sigma_l c_l u_l
+    if (a.k == 0) {         // u = (jj + kk, ij + kr, ik - jr)
+        gr = c1 * k - c2 * j; gi = c1 * j + c2 * k; gj = c1 * i - c2 * r - 2.0f * j * c0; gk = c1 * r + c2 * i - 2.0f * k * c0;
+        su = -c0 * (j * j + k * k) + c1 * (i * j + k * r) + c2 * (i * k - j * r);
+    } else if (a.k == 1) {  // u = (ij - kr, ii + kk, jk + ir)
+        gr = c2 * i - c0 * k; gi = c0 * j + c2 * r - 2.0f * i * c1; gj = c0 * i + c2 * k; gk = c2 * j - c0 * r - 2.0f * k * c1;
+        su = c0 * (i * j - k * r) - c1 * (i * i + k * k) + c2 * (j * k + i * r);
+    } else {                // u = (ik + jr, jk - ir, ii + jj)
+        gr = c0 * j - c1 * i; gi = c0 * k - c1 * r - 2.0f * i * c2; gj = c0 * r + c1 * k - 2.0f * j * c2; gk = c0 * i + c1 * j;
+        su = c0 * (i * k + j * r) + c1 * (j * k - i * r) - c2 * (i * i + j * j);
+    }
+    const float t = a.two_s, tts = t * t * su;
+    dL_dq[n4] = t * gr - tts * r; dL_dq[n4 + 1] = t * gi - tts * i; dL_dq[n4 + 2] = t * gj - tts * j; dL_dq[n4 + 3] = t * gk - tts * k;
 }
 
 // world-space point of pixel (x, y) at the rendered depth (GR/:41-80,185-190): directions @ c2w[:3,:3].T * depth + c2w[:3,3]
@@ -118,6 +176,25 @@ int axis_normals_impl(int P, const float* means3D, const float* scales, const fl
     if (P == 0) return GSR_OK;
     k_axis_normals<<<(P + 255) / 256, 256, 0, st>>>(P, means3D, scales, rotations, campos, remap01, out);
     return check_launch("gsr_axis_normals", false, st);
+}
+
+int sugar_normals_impl(int P, const float* positions, const float* scales, const float* quaternions, const float* campos, float* out,
+                       cudaStream_t st) {
+    if (P < 0 || (P > 0 && (!positions || !scales || !quaternions || !campos || !out))) { set_error("gsr_sugar_normals: bad arguments"); return GSR_ERR_INVALID; }
+    if (P == 0) return GSR_OK;
+    k_sugar_normals<<<(P + 255) / 256, 256, 0, st>>>(P, positions, scales, quaternions, campos, out);
+    return check_launch("gsr_sugar_normals", false, st);
+}
+
+int sugar_normals_backward_impl(int P, const float* positions, const float* scales, const float* quaternions, const float* campos,
+                                const float* dL_dnormals, float* dL_dquaternions, cudaStream_t st) {
+    if (P < 0 || (P > 0 && (!positions || !scales || !quaternions || !campos || !dL_dnormals || !dL_dquaternions))) {
+        set_error("gsr_sugar_normals_backward: bad arguments");
+        return GSR_ERR_INVALID;
+    }
+    if (P == 0) return GSR_OK;
+    k_sugar_normals_backward<<<(P + 255) / 256, 256, 0, st>>>(P, positions, scales, quaternions, campos, dL_dnormals, dL_dquaternions);
+    return check_launch("gsr_sugar_normals_backward", false, st);
 }
 
 int normal_maps_impl(int W, int H, const float* normal_img, const float* depth, const float* c2w, float fx, float fy, float cx, float cy,

@@ -21,6 +21,10 @@ normalisation and the pseudo-normal stencil are torch ops, so every parameter re
 ``_scaling``, ``_rotation``): gsr_activate_gaussians and gsr_axis_normals replace the activations and ``get_normal``, and one
 gsr_activate_gaussians_backward launch replaces their autograd graph; the rest of the frame is render()'s.
 
+``render_sugar()`` is SuGaR's wrapper (``sugar_scene/sugar_model.py:1956-2228``) with the same structure: gsr_sugar_normals (and
+gsr_sugar_normals_backward) for SuGaR's own shading normals, one rasterizer pass for both colour sets, and a single colour pass
+when the caller asks for the image alone.
+
 Same argument names, return keys and error behaviour as the reference function.
 """
 from __future__ import annotations
@@ -36,7 +40,7 @@ from ._lib import lib as _L
 from . import rasterizer as R
 from .rasterizer import GaussianRasterizationSettings
 
-__all__ = ["render", "render_raw", "axis_normals", "normal_maps", "pack_frame", "fov2focal", "TURBO_LUT_BGR"]
+__all__ = ["render", "render_raw", "render_sugar", "sugar_normals", "quaternion_to_matrix", "axis_normals", "normal_maps", "pack_frame", "fov2focal", "TURBO_LUT_BGR"]
 
 
 def fov2focal(fov: float, pixels: float) -> float:
@@ -290,18 +294,26 @@ def _frame(viewpoint_camera, raster_settings, screenspace_points, grad_mode, mea
         means3D, screenspace_points, shs, colors_precomp, normal_normed, opacity, scales, rotations, cov3D_precomp, raster_settings)
     rendered_image = torch.cat((rendered_image, alpha_image), dim=0)
     depth_image = depth_image.squeeze(0)
+    c2w = viewpoint_camera.world_view_transform.inverse()
+    normal_image, pseudo_normal = _normal_maps_torch(normal_image, depth_image, c2w, fx, fy, cx, cy)
+    return {"render": rendered_image, "depth": depth_image, "normal": normal_image, "pseudo_normal": pseudo_normal,
+            "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii}
+
+
+def _normal_maps_torch(normal_image, depth_image, c2w, fx, fy, cx, cy):
+    """Differentiable torch form of normal_maps() (GR/:168-191): the rendered normal*0.5+0.5 image [3,H,W] and the depth map
+    [H,W] -> (normal [H,W,3], pseudo_normal [H,W,3]), with ``c2w`` the 4x4 the wrapper unprojects with."""
+    device = depth_image.device
+    H, W = depth_image.shape
     normal_image = (normal_image - 0.5) * 2.
     normal_image = torch.nn.functional.normalize(normal_image.permute(1, 2, 0), p=2, dim=-1)
-    c2w = viewpoint_camera.world_view_transform.inverse()
     ys, xs = torch.meshgrid(torch.arange(H, dtype=torch.float32, device=device), torch.arange(W, dtype=torch.float32, device=device), indexing="ij")
     K = torch.tensor([fx, fy, cx, cy], dtype=torch.float32)
     directions = torch.stack([(xs - K[2] + 0.5) / K[0], (ys - K[3] + 0.5) / K[1], torch.ones_like(xs)], -1)
     rays_d = directions @ c2w[:3, :3].T
     rays_o = c2w[:3, 3].expand_as(rays_d)
     points3D = rays_o + rays_d * depth_image.unsqueeze(-1)
-    pseudo_normal = _depth_pcd2normal(points3D)
-    return {"render": rendered_image, "depth": depth_image, "normal": normal_image, "pseudo_normal": pseudo_normal,
-            "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii}
+    return normal_image, _depth_pcd2normal(points3D)
 
 
 # ------------------------------------------------------------------------------------------ render_raw()
@@ -407,3 +419,240 @@ def render_raw(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modif
         shs = None
     return _frame(viewpoint_camera, raster_settings, screenspace_points, grad_mode, xyz, shs, override_color, normal_normed, opacity,
                   scales, rotations, None)
+
+
+# ------------------------------------------------------------------------------------------ render_sugar()
+# "SS/" = sugar/sugar_scene/sugar_model.py (SuGaR.render_image_gaussian_rasterizer, SS/:1956-2228)
+def quaternion_to_matrix(quaternions: torch.Tensor) -> torch.Tensor:
+    """pytorch3d.transforms.quaternion_to_matrix, op for op: rotation matrices [...,3,3] of quaternions (real part first) that
+    are NOT normalised first; the scale enters as two_s = 2 / |q|^2.  gsr_sugar_normals evaluates the same formula."""
+    r, i, j, k = torch.unbind(quaternions, -1)
+    two_s = 2.0 / (quaternions * quaternions).sum(-1)
+    o = torch.stack((1 - two_s * (j * j + k * k), two_s * (i * j - k * r), two_s * (i * k + j * r),
+                     two_s * (i * j + k * r), 1 - two_s * (i * i + k * k), two_s * (j * k - i * r),
+                     two_s * (i * k - j * r), two_s * (j * k + i * r), 1 - two_s * (i * i + j * j)), -1)
+    return o.reshape(quaternions.shape[:-1] + (3, 3))
+
+
+def sugar_normals(positions: torch.Tensor, scales: torch.Tensor, quaternions: torch.Tensor, campos: torch.Tensor,
+                  out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """SuGaR's per-Gaussian shading normal remapped to [0,1] (SS/:2164-2168): the column of quaternion_to_matrix(quaternions)
+    that belongs to ``scales.min(dim=-1)[1]``, flipped to face ``campos``, divided by its norm, ``* 0.5 + 0.5``.  [P,3] float32.
+    Forward only; one gsr_sugar_normals launch."""
+    if not positions.is_cuda:
+        raise RuntimeError("autovfx_b200.renderer: CUDA tensors required (there is no CPU path)")
+    device = positions.device
+    with torch.cuda.device(device):
+        m, s, q, c = (_f32c(t.detach(), device) for t in (positions, scales, quaternions, campos))
+        P = m.shape[0]
+        if m.shape != (P, 3) or s.shape != (P, 3) or q.shape != (P, 4) or c.numel() != 3:
+            raise ValueError("sugar_normals: expected positions [P,3], scales [P,3], quaternions [P,4], campos [3]")
+        if out is None:
+            out = torch.empty((P, 3), dtype=torch.float32, device=device)
+        _lib.check(_L.gsr_sugar_normals(P, R._ptr(m), R._ptr(s), R._ptr(q), c.data_ptr(), R._ptr(out), _stream(device)), "gsr_sugar_normals")
+    return out
+
+
+class _SugarNormals(torch.autograd.Function):
+    """(positions, scales, quaternions, campos) -> sugar_normals(...), differentiable with respect to the quaternions: the backward is
+    one gsr_sugar_normals_backward launch.  Positions, scales and campos get no gradient: the axis (an argmin over the scales) and
+    the flip (a sign test on the view direction) are piecewise constant, and the reference's graph carries none through them."""
+
+    @staticmethod
+    def forward(ctx, positions, scales, quaternions, campos):
+        device = positions.device
+        m, s, q, c = (_f32c(t.detach(), device) for t in (positions, scales, quaternions, campos))
+        out = sugar_normals(m, s, q, c)
+        ctx.save_for_backward(m, s, q, c)
+        return out
+
+    @staticmethod
+    def backward(ctx, g_normals):
+        m, s, q, c = ctx.saved_tensors
+        device, P = m.device, m.shape[0]
+        d_q = torch.empty((P, 4), dtype=torch.float32, device=device)
+        with torch.cuda.device(device):
+            g = _f32c(g_normals, device)
+            rc = _L.gsr_sugar_normals_backward(P, R._ptr(m), R._ptr(s), R._ptr(q), c.data_ptr(), R._ptr(g), R._ptr(d_q), _stream(device))
+            _lib.check(rc, "gsr_sugar_normals_backward")
+        return None, None, d_q, None
+
+
+def _sugar_projection(znear: float, zfar: float, fovx: float, fovy: float) -> torch.Tensor:
+    """SuGaR's getProjectionMatrix (sugar/sugar_utils/graphics_utils.py): the 4x4 perspective matrix (row-major, z in [0, 1]),
+    evaluated in Python floats and stored as float32, as the reference does."""
+    top = math.tan(fovy / 2) * znear
+    right = math.tan(fovx / 2) * znear
+    bottom, left = -top, -right
+    P = torch.zeros(4, 4)
+    P[0, 0] = 2.0 * znear / (right - left)
+    P[1, 1] = 2.0 * znear / (top - bottom)
+    P[0, 2] = (right + left) / (right - left)
+    P[1, 2] = (top + bottom) / (top - bottom)
+    P[3, 2] = 1.0
+    P[2, 2] = zfar / (zfar - znear)
+    P[2, 3] = -(zfar * znear) / (zfar - znear)
+    return P
+
+
+def sugar_camera(nerf_cameras, camera_indices, fov_x: float, fov_y: float, device):
+    """The camera of SS/:2008-2035 -> (world_view_transform, full_proj_transform, camera_center [1,3], c2w [4,4] float32 numpy).
+    c2w is the camera-to-world with the OpenGL -> COLMAP axis flip; the world-to-view matrix is np.linalg.inv of it in float32
+    (getWorld2View: R^T = w2c[:3,:3], t = w2c[:3,3]); the projection is SuGaR's getProjectionMatrix with the principal point of
+    K written into its third row; the product is the reference's bmm on the device."""
+    import numpy as np
+    p3d_camera = nerf_cameras.p3d_cameras[camera_indices]
+    c2w = nerf_cameras.camera_to_worlds[camera_indices]
+    c2w = torch.cat([c2w, torch.Tensor([[0, 0, 0, 1]]).to(device)], dim=0).cpu().numpy()
+    c2w[:3, 1:3] *= -1
+    w2c = np.linalg.inv(c2w)
+    Rt = np.zeros((4, 4))
+    Rt[:3, :3] = w2c[:3, :3]  # getWorld2View(R = w2c[:3,:3]^T, t): Rt[:3,:3] = R^T
+    Rt[:3, 3] = w2c[:3, 3]
+    Rt[3, 3] = 1.0
+    world_view_transform = torch.Tensor(np.float32(Rt)).transpose(0, 1).to(device)
+    proj_transform = _sugar_projection(p3d_camera.znear.item(), p3d_camera.zfar.item(), fov_x, fov_y).transpose(0, 1).to(device)
+    proj_transform[..., 2, 0] = - p3d_camera.K[0, 0, 2]
+    proj_transform[..., 2, 1] = - p3d_camera.K[0, 1, 2]
+    full_proj_transform = (world_view_transform.unsqueeze(0).bmm(proj_transform.unsqueeze(0))).squeeze(0)
+    return world_view_transform, full_proj_transform, p3d_camera.get_camera_center(), c2w
+
+
+def render_sugar(self, nerf_cameras=None, camera_indices=0, verbose=False, bg_color=None, sh_deg=None, sh_rotations=None,
+                 compute_color_in_rasterizer=False, compute_covariance_in_rasterizer=True, return_2d_radii=False, quaternions=None,
+                 use_same_scale_in_all_directions=False, return_opacities=False, return_colors=False, positions=None, point_colors=None):
+    """SuGaR.render_image_gaussian_rasterizer (SS/:1956-2228) with the reference method's signature, arguments and return
+    values; a SuGaR model opts in with ``SuGaR.render_image_gaussian_rasterizer = render_sugar``.
+
+    ``self`` is the SuGaR model; only what the reference reads is read: points, strengths, scaling, quaternions,
+    sh_coordinates, get_points_rgb, n_points, _points.dtype, device, image_height / image_width, fov_x / fov_y, tanfovx / tanfovy,
+    nerfmodel.training_cameras.  The camera needs camera_to_worlds and p3d_cameras[i] with znear, zfar, K, get_camera_center().
+
+    The reference renders twice with the same geometry (the colours, then the shading normals as colors_precomp) and computes the
+    normals with ~15 torch ops.  Here:
+      * without a ``return_*`` flag the reference returns the image alone and discards the normals: one rasterizer pass;
+      * otherwise, without gradients: gsr_sugar_normals -> gsr_forward_multi (one pass, both colour sets) -> gsr_normal_maps;
+      * otherwise, with gradients: the same normals differentiated by gsr_sugar_normals_backward, and rasterize_gaussians_multi
+        (one forward, one backward for both images); the normal maps are torch ops, as in render().
+    The normals come from the model's own ``quaternions`` and ``scaling``, whatever ``quaternions=`` or
+    ``use_same_scale_in_all_directions`` hands the rasterizer, and face the camera from ``positions``, as in the reference.  So
+    does the reference's pseudo normal: the flipped c2w and ``fx = fov2focal(self.tanfovx, w)`` (a tangent where a field of view is
+    expected)."""
+    if nerf_cameras is None:
+        nerf_cameras = self.nerfmodel.training_cameras
+    device = self.device
+    if bg_color is None:
+        bg_color = torch.Tensor([0.0, 0.0, 0.0]).to(device)
+    if positions is None:
+        positions = self.points
+
+    world_view_transform, full_proj_transform, camera_center, c2w = sugar_camera(nerf_cameras, camera_indices, self.fov_x, self.fov_y,
+                                                                               device)
+    if verbose:
+        print("p3d camera_center", camera_center)
+        print("ns camera_center", nerf_cameras.camera_to_worlds[camera_indices][..., 3])
+    H, W = int(self.image_height), int(self.image_width)
+    raster_settings = GaussianRasterizationSettings(
+        image_height=H, image_width=W, tanfovx=self.tanfovx, tanfovy=self.tanfovy, bg=bg_color, scale_modifier=1.,
+        viewmatrix=world_view_transform, projmatrix=full_proj_transform, sh_degree=sh_deg, campos=camera_center, prefiltered=False,
+        debug=False)
+
+    if point_colors is None:
+        if not compute_color_in_rasterizer:
+            if sh_rotations is None:
+                splat_colors = self.get_points_rgb(positions=positions, camera_centers=camera_center, sh_levels=sh_deg + 1)
+            else:
+                splat_colors = self.get_points_rgb(
+                    positions=positions, camera_centers=None,
+                    directions=(torch.nn.functional.normalize(positions - camera_center, dim=-1).unsqueeze(1) @ sh_rotations)[..., 0, :],
+                    sh_levels=sh_deg + 1)
+            shs = None
+        else:
+            shs = self.sh_coordinates
+            splat_colors = None
+    else:
+        splat_colors = point_colors
+        shs = None
+
+    splat_opacities = self.strengths.view(-1, 1)
+    if quaternions is None:
+        quaternions = self.quaternions
+    if not use_same_scale_in_all_directions:
+        scales = self.scaling
+    else:
+        scales = self.scaling.mean(dim=-1, keepdim=True).expand(-1, 3)
+        scales = scales.squeeze(0)
+    if verbose:
+        print("Scales:", scales.shape, scales.min(), scales.max())
+
+    if not compute_covariance_in_rasterizer:  # SS/:2093-2112
+        cov3Dmatrix = torch.zeros((scales.shape[0], 3, 3), dtype=torch.float, device=device)
+        rotation = quaternion_to_matrix(quaternions)
+        cov3Dmatrix[:, 0, 0] = scales[:, 0] ** 2
+        cov3Dmatrix[:, 1, 1] = scales[:, 1] ** 2
+        cov3Dmatrix[:, 2, 2] = scales[:, 2] ** 2
+        cov3Dmatrix = rotation @ cov3Dmatrix @ rotation.transpose(-1, -2)
+        cov3D = torch.zeros((cov3Dmatrix.shape[0], 6), dtype=torch.float, device=device)
+        for c, (a, b) in enumerate(((0, 0), (0, 1), (0, 2), (1, 1), (1, 2), (2, 2))):
+            cov3D[:, c] = cov3Dmatrix[:, a, b]
+        quaternions = None
+        scales = None
+    else:
+        cov3D = None
+
+    # a fresh zero leaf whose gradient is the screen-space positional gradient (SS/:2117-2126)
+    screenspace_points = torch.zeros(self.n_points, 3, dtype=self._points.dtype, requires_grad=True, device=device)
+    if return_2d_radii:
+        try:
+            screenspace_points.retain_grad()
+        except Exception:  # noqa: BLE001
+            print("WARNING: return_2d_radii is True, but failed to retain grad of screenspace_points!")
+    if verbose:
+        print("points", positions.shape)
+        if not compute_color_in_rasterizer:
+            print("splat_colors", splat_colors.shape)
+        print("splat_opacities", splat_opacities.shape)
+        if not compute_covariance_in_rasterizer:
+            print("cov3D", cov3D.shape)
+            print(cov3D[0])
+        else:
+            print("quaternions", quaternions.shape)
+            print("scales", scales.shape)
+        print("screenspace_points", screenspace_points.shape)
+
+    if not (return_2d_radii or return_opacities or return_colors):
+        # the reference returns the image alone: its normal pass, normals and normal maps are not observable
+        rgb_image, _depth, alpha_image, _radii = R.GaussianRasterizer(raster_settings=raster_settings)(
+            means3D=positions, means2D=screenspace_points, shs=shs, colors_precomp=splat_colors, opacities=splat_opacities,
+            scales=scales, rotations=quaternions, cov3D_precomp=cov3D)
+        return torch.cat((rgb_image, alpha_image), dim=0).transpose(0, 1).transpose(1, 2)
+
+    fx, fy = fov2focal(self.tanfovx, W), fov2focal(self.tanfovy, H)  # SS/:2196-2197, reproduced as written
+    cx, cy = W / 2, H / 2
+    # the screen-space leaf requires grad, so the reference records a graph whenever grad mode is on
+    if not torch.is_grad_enabled():
+        with torch.cuda.device(device):
+            normal_normed = sugar_normals(positions, self.scaling, self.quaternions, camera_center)
+            frame = torch.empty((5, H, W), dtype=torch.float32, device=device)  # rgb | alpha | depth
+            radii = torch.empty((positions.shape[0],), dtype=torch.int32, device=device)
+            _c, _d, _a, normal_img, radii, _ticket = R.forward_multi(
+                positions, shs, splat_colors, normal_normed, splat_opacities, scales, quaternions, cov3D, raster_settings,
+                out=(frame[0:3], frame[4:5], frame[3:4], radii))
+            c2w_dev = torch.from_numpy(c2w).to(device)
+            normal_image, pseudo_normal = normal_maps(normal_img, frame[4], c2w_dev, fx, fy, cx, cy)
+        rendered_image, depth_image = frame[0:4], frame[4]
+    else:
+        normal_normed = _SugarNormals.apply(positions, self.scaling, self.quaternions, camera_center)
+        rgb_image, depth_image, alpha_image, normal_img, radii = R.rasterize_gaussians_multi(
+            positions, screenspace_points, shs, splat_colors, normal_normed, splat_opacities, scales, quaternions, cov3D, raster_settings)
+        rendered_image = torch.cat((rgb_image, alpha_image), dim=0)
+        depth_image = depth_image.squeeze(0)
+        normal_image, pseudo_normal = _normal_maps_torch(normal_img, depth_image, torch.FloatTensor(c2w).to(device), fx, fy, cx, cy)
+
+    outputs = {"image": rendered_image.transpose(0, 1).transpose(1, 2), "depth": depth_image, "normal": normal_image,
+               "pseudo_normal": pseudo_normal, "radii": radii, "viewspace_points": screenspace_points}
+    if return_opacities:
+        outputs["opacities"] = splat_opacities
+    if return_colors:
+        outputs["colors"] = splat_colors
+    return outputs

@@ -22,6 +22,8 @@
  *                               get_scaling/get_rotation/get_opacity/get_features   sugar/gaussian_splatting/scene/gaussian_model.py:95-115
  *                               transform_gaussians + merge_two_gaussians            gaussians_utils.py:71-125, scene_representation.py:357-371
  *   gsr_activate_gaussians_backward replaces the autograd backward of those activations and of get_normal * 0.5 + 0.5
+ *   gsr_sugar_normals replaces  SuGaR's shading normal * 0.5 + 0.5               sugar_scene/sugar_model.py:2164-2168 (get_smallest_axis :801-815)
+ *   gsr_sugar_normals_backward replaces its autograd backward (gradient with respect to the raw quaternions)
  *
  * Conventions (same as the reference's C++ layer):
  *   - every pointer is a DEVICE pointer to contiguous fp32 / int32 data unless it says "host";
@@ -152,6 +154,19 @@ int gsr_forward_multi(const gsr_frame* frame, const gsr_workspace* ws, float* ou
  * out [P,3]. */
 int gsr_axis_normals(int32_t P, const float* means3D, const float* scales, const float* rotations, const float* campos,
                      int remap01, float* out, void* stream);
+
+/* SuGaR's per-Gaussian shading normal (SuGaR.render_image_gaussian_rasterizer): column k = argmin(scales) (ties: lowest
+ * index) of quaternion_to_matrix(q) for the RAW quaternion q (2 / |q|^2, no normalisation), flipped so that
+ * dot(axis, -normalize(position - campos)) >= 0, divided by its norm (no epsilon); out [P,3] = normal * 0.5 + 0.5.
+ * positions [P,3], scales [P,3], quaternions [P,4] (real part first), campos [3].  P = 0 is a no-op. */
+int gsr_sugar_normals(int32_t P, const float* positions, const float* scales, const float* quaternions, const float* campos, float* out,
+                      void* stream);
+
+/* Backward of gsr_sugar_normals: dL_dnormals [P,3] (the gradient of normal * 0.5 + 0.5) -> dL_dquaternions [P,4].  The axis and the
+ * flip are the forward's decisions, recomputed from the same inputs; they are piecewise constant, so positions and scales get no
+ * gradient.  Every pointer is required when P > 0. */
+int gsr_sugar_normals_backward(int32_t P, const float* positions, const float* scales, const float* quaternions, const float* campos,
+                               const float* dL_dnormals, float* dL_dquaternions, void* stream);
 
 /* normal_img [3,H,W] (a rendered normal*0.5+0.5 image) -> out_normal [H,W,3] = normalize((img - 0.5) * 2);
  * depth [H,W] -> out_pseudo [H,W,3] = normalised cross product of central differences of the unprojected depth map,
