@@ -8,6 +8,8 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import torch
+
 from . import build as _build
 
 _f32p = C.c_void_p  # device pointers travel as plain integers
@@ -148,3 +150,8 @@ for _kv in filter(None, os.environ.get("GSR_OPTIONS", "").split(",")):
 def check(rc: int, what: str) -> None:
     if rc != 0:
         raise RuntimeError("%s failed (%d): %s" % (what, rc, lib.gsr_last_error().decode("utf-8", "replace")))
+
+
+def stream_ptr(device) -> C.c_void_p:
+    """PyTorch's current stream on ``device``, as the ``cudaStream_t`` argument of a library call."""
+    return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)

@@ -109,8 +109,7 @@ def activate_into(raw: Mapping[str, torch.Tensor], dst: Mapping[str, torch.Tenso
         rc = _L.gsr_activate_gaussians(N, M, raw["xyz"].data_ptr(), raw["f_dc"].data_ptr(), raw["f_rest"].data_ptr() if M > 1 else None,
                                        raw["opacity"].data_ptr(), raw["scaling"].data_ptr(), raw["rotation"].data_ptr(),
                                        C.byref(xform) if xform is not None else None, at(means, 3), at(dst["shs"], 3 * M),
-                                       at(dst["opacities"], 1), at(dst["scales"], 3), at(dst["rotations"], 4),
-                                       C.c_void_p(torch.cuda.current_stream(device).cuda_stream))
+                                       at(dst["opacities"], 1), at(dst["scales"], 3), at(dst["rotations"], 4), _lib.stream_ptr(device))
         _lib.check(rc, "gsr_activate_gaussians")
     from . import rasterizer as _R  # the arrays changed behind the version counters the geometry-reuse cache watches
     _R.invalidate_geometry_cache(device)

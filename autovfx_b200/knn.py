@@ -1,8 +1,6 @@
 """``distCUDA2`` — drop-in for ``simple_knn._C.distCUDA2`` (reference KNN/spatial.cu:15-26, KNN/ext.cpp:15-17)."""
 from __future__ import annotations
 
-import ctypes as C
-
 import torch
 
 from . import _lib
@@ -22,7 +20,6 @@ def distCUDA2(points: torch.Tensor) -> torch.Tensor:
             return means
         nbytes = _L.gsr_dist2_bytes(P)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=device)
-        rc = _L.gsr_dist2(P, pts.data_ptr(), means.data_ptr(), ws.data_ptr(), nbytes,
-                          C.c_void_p(torch.cuda.current_stream(device).cuda_stream))
+        rc = _L.gsr_dist2(P, pts.data_ptr(), means.data_ptr(), ws.data_ptr(), nbytes, _lib.stream_ptr(device))
         _lib.check(rc, "gsr_dist2")
     return means

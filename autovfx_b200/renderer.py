@@ -29,7 +29,6 @@ Same argument names, return keys and error behaviour as the reference function.
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
 from typing import Dict, Optional, Tuple
 
@@ -38,26 +37,10 @@ import torch
 from . import _lib
 from ._lib import lib as _L
 from . import rasterizer as R
-from .rasterizer import GaussianRasterizationSettings
+from .rasterizer import GaussianRasterizationSettings, _dev_f32
+from .scene import fov2focal
 
 __all__ = ["render", "render_raw", "render_sugar", "sugar_normals", "quaternion_to_matrix", "axis_normals", "normal_maps", "pack_frame", "fov2focal", "TURBO_LUT_BGR"]
-
-
-def fov2focal(fov: float, pixels: float) -> float:
-    """utils/graphics_utils.py:74-75."""
-    return pixels / (2 * math.tan(fov / 2))
-
-
-def _stream(device) -> C.c_void_p:
-    return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
-
-
-def _f32c(t: torch.Tensor, device) -> torch.Tensor:
-    if t.device != device:
-        t = t.to(device, non_blocking=True)
-    if t.dtype != torch.float32:
-        t = t.float()
-    return t.contiguous()
 
 
 # ------------------------------------------------------------------------------------------ the three post kernels
@@ -70,14 +53,14 @@ def axis_normals(means3D: torch.Tensor, scales: torch.Tensor, rotations: torch.T
         raise RuntimeError("autovfx_b200.renderer: CUDA tensors required (there is no CPU path)")
     device = means3D.device
     with torch.cuda.device(device):
-        m, s, r, c = _f32c(means3D.detach(), device), _f32c(scales.detach(), device), _f32c(rotations.detach(), device), _f32c(campos.detach(), device)
+        m, s, r, c = (_dev_f32(t.detach(), device) for t in (means3D, scales, rotations, campos))
         P = m.shape[0]
         if s.shape != (P, 3) or r.shape != (P, 4) or c.numel() != 3:
             raise ValueError("axis_normals: expected scales [P,3], rotations [P,4], campos [3]")
         if out is None:
             out = torch.empty((P, 3), dtype=torch.float32, device=device)
         rc = _L.gsr_axis_normals(P, m.data_ptr() if P else None, s.data_ptr() if P else None, r.data_ptr() if P else None, c.data_ptr(),
-                                 int(bool(remap01)), out.data_ptr() if P else None, _stream(device))
+                                 int(bool(remap01)), out.data_ptr() if P else None, _lib.stream_ptr(device))
         _lib.check(rc, "gsr_axis_normals")
     return out
 
@@ -95,16 +78,16 @@ def normal_maps(normal_img: Optional[torch.Tensor], depth: Optional[torch.Tensor
         out_n = out_p = None
         H, W = src.shape[-2], src.shape[-1]
         if normal_img is not None:
-            normal_img = _f32c(normal_img, device)
+            normal_img = _dev_f32(normal_img, device)
             out_n = out[0] if out is not None and out[0] is not None else torch.empty((H, W, 3), dtype=torch.float32, device=device)
         if depth is not None:
-            depth = _f32c(depth, device)
-            c2w = _f32c(c2w, device)
+            depth = _dev_f32(depth, device)
+            c2w = _dev_f32(c2w, device)
             if c2w.numel() < 12:
                 raise ValueError("normal_maps: c2w must hold at least 3x4 floats")
             out_p = out[1] if out is not None and out[1] is not None else torch.empty((H, W, 3), dtype=torch.float32, device=device)
         rc = _L.gsr_normal_maps(W, H, R._ptr(normal_img), R._ptr(depth), R._ptr(c2w) if depth is not None else None, fx, fy, cx, cy,
-                                R._ptr(out_n), R._ptr(out_p), _stream(device))
+                                R._ptr(out_n), R._ptr(out_p), _lib.stream_ptr(device))
         _lib.check(rc, "gsr_normal_maps")
     return out_n, out_p
 
@@ -128,10 +111,10 @@ def pack_frame(rgb: Optional[torch.Tensor] = None, alpha: Optional[torch.Tensor]
             H, W = depth.shape[-2], depth.shape[-1]
         else:
             H, W = normal_hwc.shape[0], normal_hwc.shape[1]
-        rgb = _f32c(rgb, device) if rgb is not None else None
-        alpha = _f32c(alpha, device) if alpha is not None else None
-        depth = _f32c(depth, device) if depth is not None else None
-        normal_hwc = _f32c(normal_hwc, device) if normal_hwc is not None else None
+        rgb = _dev_f32(rgb, device) if rgb is not None else None
+        alpha = _dev_f32(alpha, device) if alpha is not None else None
+        depth = _dev_f32(depth, device) if depth is not None else None
+        normal_hwc = _dev_f32(normal_hwc, device) if normal_hwc is not None else None
 
         def buf(name, shape):
             if out is not None and name in out:
@@ -144,7 +127,7 @@ def pack_frame(rgb: Optional[torch.Tensor] = None, alpha: Optional[torch.Tensor]
         if depth is not None:
             res["depth8"] = buf("depth8", (H, W))
         rc = _L.gsr_pack_frame(W, H, R._ptr(rgb), R._ptr(alpha), R._ptr(depth), R._ptr(normal_hwc), float(depth_scale),
-                               R._ptr(res.get("rgba8")), R._ptr(res.get("normal8")), R._ptr(res.get("depth8")), _stream(device))
+                               R._ptr(res.get("rgba8")), R._ptr(res.get("normal8")), R._ptr(res.get("depth8")), _lib.stream_ptr(device))
         _lib.check(rc, "gsr_pack_frame")
     return res
 
@@ -229,50 +212,60 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier:
     "visibility_filter", "radii"}."""
     xyz = pc.get_xyz
     device = xyz.device
-    grad_mode = torch.is_grad_enabled() and any(
-        isinstance(t, torch.Tensor) and t.requires_grad
-        for t in (xyz, pc.get_opacity, pc.get_scaling, pc.get_rotation, pc.get_features, override_color))
+    opacity, scaling, rotation, features = pc.get_opacity, pc.get_scaling, pc.get_rotation, pc.get_features
+    grad_mode = R._needs_backward(xyz, opacity, scaling, rotation, features, override_color)
     screenspace_points, raster_settings = _setup(viewpoint_camera, xyz, pc.active_sh_degree, pipe, bg_color, scaling_modifier)
 
-    means3D, opacity = xyz, pc.get_opacity
     scales = rotations = cov3D_precomp = None
     if pipe.compute_cov3D_python:
         cov3D_precomp = pc.get_covariance(scaling_modifier)
     else:
-        scales, rotations = pc.get_scaling, pc.get_rotation
+        scales, rotations = scaling, rotation
 
     shs = colors_precomp = None
     dir_pp_normalized = None
     if override_color is None:
         if pipe.convert_SHs_python:
-            dir_pp = xyz - viewpoint_camera.camera_center.repeat(pc.get_features.shape[0], 1)
+            dir_pp = xyz - viewpoint_camera.camera_center.repeat(features.shape[0], 1)
             dir_pp_normalized = dir_pp / dir_pp.norm(dim=1, keepdim=True)
-            shs_view = pc.get_features.transpose(1, 2).view(-1, 3, (pc.max_sh_degree + 1) ** 2)
+            shs_view = features.transpose(1, 2).view(-1, 3, (pc.max_sh_degree + 1) ** 2)
             colors_precomp = torch.clamp_min(_eval_sh_torch(pc.active_sh_degree, shs_view, dir_pp_normalized) + 0.5, 0.0)
         else:
-            shs = pc.get_features
+            shs = features
     else:
         colors_precomp = override_color
 
     if not grad_mode:
         with torch.no_grad(), torch.cuda.device(device):
-            normal_normed = axis_normals(xyz, pc.get_scaling, pc.get_rotation, viewpoint_camera.camera_center, remap01=True)
+            normal_normed = axis_normals(xyz, scaling, rotation, viewpoint_camera.camera_center, remap01=True)
     else:
         if dir_pp_normalized is None:
-            dir_pp = xyz - viewpoint_camera.camera_center.repeat(pc.get_features.shape[0], 1)
+            dir_pp = xyz - viewpoint_camera.camera_center.repeat(features.shape[0], 1)
             dir_pp_normalized = dir_pp / dir_pp.norm(dim=1, keepdim=True)
         normal_normed = pc.get_normal(dir_pp_normalized=dir_pp_normalized) * 0.5 + 0.5
-    return _frame(viewpoint_camera, raster_settings, screenspace_points, grad_mode, means3D, shs, colors_precomp, normal_normed, opacity,
-                  scales, rotations, cov3D_precomp)
+    return _render_outputs(viewpoint_camera, raster_settings, screenspace_points, grad_mode, xyz, shs, colors_precomp, normal_normed,
+                           opacity, scales, rotations, cov3D_precomp)
 
 
-def _frame(viewpoint_camera, raster_settings, screenspace_points, grad_mode, means3D, shs, colors_precomp, normal_normed, opacity, scales,
-           rotations, cov3D_precomp):
-    """The rasterizer call and the normal maps of render() and render_raw(), from the tensors the rasterizer takes and the
-    per-Gaussian normals remapped to [0,1]."""
-    device = means3D.device
+def _render_outputs(viewpoint_camera, raster_settings, screenspace_points, grad_mode, *inputs):
+    """_frame() with render()'s camera (GR/:168-191) and return keys; shared by render() and render_raw()."""
     H, W = int(viewpoint_camera.image_height), int(viewpoint_camera.image_width)
-    fx, fy = fov2focal(viewpoint_camera.FoVx, W), fov2focal(viewpoint_camera.FoVy, H)
+    w2c = viewpoint_camera.world_view_transform
+    c2w = w2c.inverse if grad_mode else (lambda: torch.linalg.inv_ex(w2c.float())[0])  # GR/:185; inv_ex: no error-check sync
+    image, depth, normal, pseudo_normal, radii = _frame(raster_settings, screenspace_points, grad_mode, *inputs, c2w,
+                                                        fov2focal(viewpoint_camera.FoVx, W), fov2focal(viewpoint_camera.FoVy, H))
+    return {"render": image, "depth": depth, "normal": normal, "pseudo_normal": pseudo_normal, "viewspace_points": screenspace_points,
+            "visibility_filter": radii > 0, "radii": radii}
+
+
+def _frame(raster_settings, screenspace_points, grad_mode, means3D, shs, colors_precomp, normal_normed, opacity, scales, rotations,
+           cov3D_precomp, c2w, fx, fy):
+    """The rasterizer call and the normal maps of every wrapper, from the tensors the rasterizer takes, the per-Gaussian normals
+    remapped to [0,1] and the pseudo normal's camera: ``c2w()`` returns the 4x4 it unprojects with (called after the rasterizer,
+    where the reference computes it), ``fx`` / ``fy`` are the focal lengths.  Returns (rgb|alpha [4,H,W], depth [H,W],
+    normal [H,W,3], pseudo_normal [H,W,3], radii)."""
+    device = means3D.device
+    H, W = int(raster_settings.image_height), int(raster_settings.image_width)
     cx, cy = W / 2, H / 2
 
     if not grad_mode:
@@ -283,10 +276,8 @@ def _frame(viewpoint_camera, raster_settings, screenspace_points, grad_mode, mea
             _c, _d, _a, normal_img, radii, _ticket = R.forward_multi(
                 means3D, shs, colors_precomp, normal_normed, opacity, scales, rotations, cov3D_precomp, raster_settings,
                 out=(frame[0:3], frame[4:5], frame[3:4], radii))
-            c2w = torch.linalg.inv_ex(viewpoint_camera.world_view_transform.float())[0]  # no error-check sync; GR/:185
-            normal_image, pseudo_normal = normal_maps(normal_img, frame[4], c2w, fx, fy, cx, cy)
-        return {"render": frame[0:4], "depth": frame[4], "normal": normal_image, "pseudo_normal": pseudo_normal,
-                "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii}
+            normal_image, pseudo_normal = normal_maps(normal_img, frame[4], c2w(), fx, fy, cx, cy)
+        return frame[0:4], frame[4], normal_image, pseudo_normal, radii
 
     # ---- gradients required: one differentiable call renders both colour sets (SH colours and normals) on one projection /
     # binning / sort / blend, and its backward takes both images' gradients in one pass; the rest is the reference's graph
@@ -294,10 +285,8 @@ def _frame(viewpoint_camera, raster_settings, screenspace_points, grad_mode, mea
         means3D, screenspace_points, shs, colors_precomp, normal_normed, opacity, scales, rotations, cov3D_precomp, raster_settings)
     rendered_image = torch.cat((rendered_image, alpha_image), dim=0)
     depth_image = depth_image.squeeze(0)
-    c2w = viewpoint_camera.world_view_transform.inverse()
-    normal_image, pseudo_normal = _normal_maps_torch(normal_image, depth_image, c2w, fx, fy, cx, cy)
-    return {"render": rendered_image, "depth": depth_image, "normal": normal_image, "pseudo_normal": pseudo_normal,
-            "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii}
+    normal_image, pseudo_normal = _normal_maps_torch(normal_image, depth_image, c2w(), fx, fy, cx, cy)
+    return rendered_image, depth_image, normal_image, pseudo_normal, radii
 
 
 def _normal_maps_torch(normal_image, depth_image, c2w, fx, fy, cx, cy):
@@ -357,14 +346,14 @@ class _ActivateRaw(torch.autograd.Function):
         device = xyz.device
         P, M = xyz.shape[0], f_rest.shape[1] + 1
         xyz, f_dc, f_rest, opacity, scaling, rotation = (t.detach().contiguous() for t in (xyz, f_dc, f_rest, opacity, scaling, rotation))
-        campos = _f32c(campos.detach(), device)
+        campos = _dev_f32(campos.detach(), device)
         f = dict(dtype=torch.float32, device=device)
         shs, opacities, scales, rotations = torch.empty((P, M, 3), **f), torch.empty((P, 1), **f), torch.empty((P, 3), **f), torch.empty((P, 4), **f)
         normals = torch.empty((P, 3), **f)
         means = torch.empty((P, 3), **f)  # the kernel's copy of the positions; the rasterizer reads _xyz itself
         p = R._ptr
         with torch.cuda.device(device):
-            st = _stream(device)
+            st = _lib.stream_ptr(device)
             _lib.check(_L.gsr_activate_gaussians(P, M, p(xyz), p(f_dc), p(f_rest), p(opacity), p(scaling), p(rotation), None, p(means),
                                                  p(shs), p(opacities), p(scales), p(rotations), st), "gsr_activate_gaussians")
             _lib.check(_L.gsr_axis_normals(P, p(xyz), p(scales), p(rotations), campos.data_ptr(), 1, p(normals), st), "gsr_axis_normals")
@@ -380,10 +369,10 @@ class _ActivateRaw(torch.autograd.Function):
         f = dict(dtype=torch.float32, device=device)
 
         def grad_in(g, like):
-            return torch.zeros_like(like) if g is None else _f32c(g, device)
+            return torch.zeros_like(like) if g is None else _dev_f32(g, device)
         g_opacities, g_scales, g_rotations = grad_in(g_opacities, opacities), grad_in(g_scales, scales), grad_in(g_rotations, rotations)
-        g_shs = None if g_shs is None else _f32c(g_shs, device)
-        g_normals = None if g_normals is None else _f32c(g_normals, device)
+        g_shs = None if g_shs is None else _dev_f32(g_shs, device)
+        g_normals = None if g_normals is None else _dev_f32(g_normals, device)
         d_op, d_sc, d_rot = torch.empty((P, 1), **f), torch.empty((P, 3), **f), torch.empty((P, 4), **f)
         d_dc = d_rest = None
         if g_shs is not None:
@@ -392,7 +381,7 @@ class _ActivateRaw(torch.autograd.Function):
         with torch.cuda.device(device):
             rc = _L.gsr_activate_gaussians_backward(P, M, p(xyz), campos.data_ptr(), p(opacities), p(scales), p(rotations), p(rotation),
                                                     p(g_opacities), p(g_scales), p(g_rotations), p(g_shs), p(g_normals), p(d_op), p(d_sc),
-                                                    p(d_rot), p(d_dc), p(d_rest), _stream(device))
+                                                    p(d_rot), p(d_dc), p(d_rest), _lib.stream_ptr(device))
             _lib.check(rc, "gsr_activate_gaussians_backward")
         return None, d_dc, d_rest, d_op, d_sc, d_rot, None
 
@@ -409,16 +398,15 @@ def render_raw(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modif
     F.normalize``) and ``pipe`` must not select ``compute_cov3D_python`` or ``convert_SHs_python``; otherwise ValueError.
     With ``override_color`` the SH coefficients get no gradient."""
     xyz, f_dc, f_rest, opacity_raw, scaling_raw, rotation_raw = _raw_params(pc, pipe)
-    grad_mode = torch.is_grad_enabled() and any(
-        isinstance(t, torch.Tensor) and t.requires_grad for t in (xyz, f_dc, f_rest, opacity_raw, scaling_raw, rotation_raw, override_color))
+    grad_mode = R._needs_backward(xyz, f_dc, f_rest, opacity_raw, scaling_raw, rotation_raw, override_color)
     screenspace_points, raster_settings = _setup(viewpoint_camera, xyz, pc.active_sh_degree, pipe, bg_color, scaling_modifier)
     with torch.set_grad_enabled(grad_mode):
         shs, opacity, scales, rotations, normal_normed = _ActivateRaw.apply(xyz, f_dc, f_rest, opacity_raw, scaling_raw, rotation_raw,
                                                                             viewpoint_camera.camera_center)
     if override_color is not None:
         shs = None
-    return _frame(viewpoint_camera, raster_settings, screenspace_points, grad_mode, xyz, shs, override_color, normal_normed, opacity,
-                  scales, rotations, None)
+    return _render_outputs(viewpoint_camera, raster_settings, screenspace_points, grad_mode, xyz, shs, override_color, normal_normed,
+                           opacity, scales, rotations, None)
 
 
 # ------------------------------------------------------------------------------------------ render_sugar()
@@ -443,13 +431,14 @@ def sugar_normals(positions: torch.Tensor, scales: torch.Tensor, quaternions: to
         raise RuntimeError("autovfx_b200.renderer: CUDA tensors required (there is no CPU path)")
     device = positions.device
     with torch.cuda.device(device):
-        m, s, q, c = (_f32c(t.detach(), device) for t in (positions, scales, quaternions, campos))
+        m, s, q, c = (_dev_f32(t.detach(), device) for t in (positions, scales, quaternions, campos))
         P = m.shape[0]
         if m.shape != (P, 3) or s.shape != (P, 3) or q.shape != (P, 4) or c.numel() != 3:
             raise ValueError("sugar_normals: expected positions [P,3], scales [P,3], quaternions [P,4], campos [3]")
         if out is None:
             out = torch.empty((P, 3), dtype=torch.float32, device=device)
-        _lib.check(_L.gsr_sugar_normals(P, R._ptr(m), R._ptr(s), R._ptr(q), c.data_ptr(), R._ptr(out), _stream(device)), "gsr_sugar_normals")
+        _lib.check(_L.gsr_sugar_normals(P, R._ptr(m), R._ptr(s), R._ptr(q), c.data_ptr(), R._ptr(out), _lib.stream_ptr(device)),
+                   "gsr_sugar_normals")
     return out
 
 
@@ -461,7 +450,7 @@ class _SugarNormals(torch.autograd.Function):
     @staticmethod
     def forward(ctx, positions, scales, quaternions, campos):
         device = positions.device
-        m, s, q, c = (_f32c(t.detach(), device) for t in (positions, scales, quaternions, campos))
+        m, s, q, c = (_dev_f32(t.detach(), device) for t in (positions, scales, quaternions, campos))
         out = sugar_normals(m, s, q, c)
         ctx.save_for_backward(m, s, q, c)
         return out
@@ -472,8 +461,9 @@ class _SugarNormals(torch.autograd.Function):
         device, P = m.device, m.shape[0]
         d_q = torch.empty((P, 4), dtype=torch.float32, device=device)
         with torch.cuda.device(device):
-            g = _f32c(g_normals, device)
-            rc = _L.gsr_sugar_normals_backward(P, R._ptr(m), R._ptr(s), R._ptr(q), c.data_ptr(), R._ptr(g), R._ptr(d_q), _stream(device))
+            g = _dev_f32(g_normals, device)
+            rc = _L.gsr_sugar_normals_backward(P, R._ptr(m), R._ptr(s), R._ptr(q), c.data_ptr(), R._ptr(g), R._ptr(d_q),
+                                               _lib.stream_ptr(device))
             _lib.check(rc, "gsr_sugar_normals_backward")
         return None, None, d_q, None
 
@@ -627,28 +617,13 @@ def render_sugar(self, nerf_cameras=None, camera_indices=0, verbose=False, bg_co
             scales=scales, rotations=quaternions, cov3D_precomp=cov3D)
         return torch.cat((rgb_image, alpha_image), dim=0).transpose(0, 1).transpose(1, 2)
 
-    fx, fy = fov2focal(self.tanfovx, W), fov2focal(self.tanfovy, H)  # SS/:2196-2197, reproduced as written
-    cx, cy = W / 2, H / 2
     # the screen-space leaf requires grad, so the reference records a graph whenever grad mode is on
-    if not torch.is_grad_enabled():
-        with torch.cuda.device(device):
-            normal_normed = sugar_normals(positions, self.scaling, self.quaternions, camera_center)
-            frame = torch.empty((5, H, W), dtype=torch.float32, device=device)  # rgb | alpha | depth
-            radii = torch.empty((positions.shape[0],), dtype=torch.int32, device=device)
-            _c, _d, _a, normal_img, radii, _ticket = R.forward_multi(
-                positions, shs, splat_colors, normal_normed, splat_opacities, scales, quaternions, cov3D, raster_settings,
-                out=(frame[0:3], frame[4:5], frame[3:4], radii))
-            c2w_dev = torch.from_numpy(c2w).to(device)
-            normal_image, pseudo_normal = normal_maps(normal_img, frame[4], c2w_dev, fx, fy, cx, cy)
-        rendered_image, depth_image = frame[0:4], frame[4]
-    else:
-        normal_normed = _SugarNormals.apply(positions, self.scaling, self.quaternions, camera_center)
-        rgb_image, depth_image, alpha_image, normal_img, radii = R.rasterize_gaussians_multi(
-            positions, screenspace_points, shs, splat_colors, normal_normed, splat_opacities, scales, quaternions, cov3D, raster_settings)
-        rendered_image = torch.cat((rgb_image, alpha_image), dim=0)
-        depth_image = depth_image.squeeze(0)
-        normal_image, pseudo_normal = _normal_maps_torch(normal_img, depth_image, torch.FloatTensor(c2w).to(device), fx, fy, cx, cy)
-
+    grad_mode = torch.is_grad_enabled()
+    normal_normed = (_SugarNormals.apply if grad_mode else sugar_normals)(positions, self.scaling, self.quaternions, camera_center)
+    rendered_image, depth_image, normal_image, pseudo_normal, radii = _frame(
+        raster_settings, screenspace_points, grad_mode, positions, shs, splat_colors, normal_normed, splat_opacities, scales, quaternions,
+        cov3D, lambda: torch.from_numpy(c2w).to(device, torch.float32),
+        fov2focal(self.tanfovx, W), fov2focal(self.tanfovy, H))  # SS/:2196-2197, reproduced as written
     outputs = {"image": rendered_image.transpose(0, 1).transpose(1, 2), "depth": depth_image, "normal": normal_image,
                "pseudo_normal": pseudo_normal, "radii": radii, "viewspace_points": screenspace_points}
     if return_opacities:
