@@ -65,7 +65,7 @@ EXPORTS = ("gsr_abi_version", "gsr_last_error", "gsr_geom_bytes", "gsr_binning_b
            "gsr_forward", "gsr_backward", "gsr_mark_visible", "gsr_dist2_bytes", "gsr_dist2", "gsr_get_views",
            "gsr_profile_begin", "gsr_profile_begin_strided", "gsr_profile_end", "gsr_forward_multi", "gsr_axis_normals", "gsr_normal_maps",
            "gsr_pack_frame", "gsr_activate_gaussians", "gsr_set_option", "gsr_backward_multi", "gsr_activate_gaussians_backward",
-           "gsr_sugar_normals", "gsr_sugar_normals_backward")
+           "gsr_sugar_normals", "gsr_sugar_normals_backward", "gsr_sugar_colors", "gsr_sugar_colors_backward")
 
 
 def _load() -> C.CDLL:
@@ -105,6 +105,10 @@ def _load() -> C.CDLL:
     lib.gsr_sugar_normals.argtypes = [C.c_int32] + [C.c_void_p] * 6
     lib.gsr_sugar_normals_backward.restype = C.c_int
     lib.gsr_sugar_normals_backward.argtypes = [C.c_int32] + [C.c_void_p] * 7
+    lib.gsr_sugar_colors.restype = C.c_int
+    lib.gsr_sugar_colors.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 9
+    lib.gsr_sugar_colors_backward.restype = C.c_int
+    lib.gsr_sugar_colors_backward.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 13
     lib.gsr_normal_maps.restype = C.c_int
     lib.gsr_normal_maps.argtypes = [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_float,
                                     C.c_void_p, C.c_void_p, C.c_void_p]

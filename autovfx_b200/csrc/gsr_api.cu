@@ -19,6 +19,12 @@ int sugar_normals_impl(int P, const float* positions, const float* scales, const
                        cudaStream_t st);
 int sugar_normals_backward_impl(int P, const float* positions, const float* scales, const float* quaternions, const float* campos,
                                 const float* dL_dnormals, float* dL_dquaternions, cudaStream_t st);
+int sugar_colors_impl(int P, int M, int deg, const float* positions, const float* campos, const float* directions, const float* sh_dc,
+                      const float* sh_rest, const float* densities, float* out_colors, float* out_opacities, cudaStream_t st);
+int sugar_colors_backward_impl(int P, int M, int deg, const float* positions, const float* campos, const float* directions,
+                               const float* sh_dc, const float* sh_rest, const float* densities, const float* dL_dcolors,
+                               const float* dL_dopacities, float* dL_dsh_dc, float* dL_dsh_rest, float* dL_dpositions, float* dL_ddensities,
+                               cudaStream_t st);
 int normal_maps_impl(int W, int H, const float* normal_img, const float* depth, const float* c2w, float fx, float fy, float cx, float cy,
                      float* out_normal, float* out_pseudo, cudaStream_t st);
 int pack_frame_impl(int W, int H, const float* rgb, const float* alpha, const float* depth, const float* normal_hwc, float depth_scale,
@@ -87,6 +93,22 @@ int gsr_sugar_normals_backward(int32_t P, const float* positions, const float* s
                                const float* dL_dnormals, float* dL_dquaternions, void* stream) {
     NvtxRange nvtx_("gsr_sugar_normals_backward");
     return gsr::sugar_normals_backward_impl(P, positions, scales, quaternions, campos, dL_dnormals, dL_dquaternions, (cudaStream_t)stream);
+}
+
+int gsr_sugar_colors(int32_t P, int32_t M, int32_t deg, const float* positions, const float* campos, const float* directions,
+                     const float* sh_dc, const float* sh_rest, const float* densities, float* out_colors, float* out_opacities, void* stream) {
+    NvtxRange nvtx_("gsr_sugar_colors");
+    return gsr::sugar_colors_impl(P, M, deg, positions, campos, directions, sh_dc, sh_rest, densities, out_colors, out_opacities,
+                                  (cudaStream_t)stream);
+}
+
+int gsr_sugar_colors_backward(int32_t P, int32_t M, int32_t deg, const float* positions, const float* campos, const float* directions,
+                              const float* sh_dc, const float* sh_rest, const float* densities, const float* dL_dcolors,
+                              const float* dL_dopacities, float* dL_dsh_dc, float* dL_dsh_rest, float* dL_dpositions, float* dL_ddensities,
+                              void* stream) {
+    NvtxRange nvtx_("gsr_sugar_colors_backward");
+    return gsr::sugar_colors_backward_impl(P, M, deg, positions, campos, directions, sh_dc, sh_rest, densities, dL_dcolors, dL_dopacities,
+                                           dL_dsh_dc, dL_dsh_rest, dL_dpositions, dL_ddensities, (cudaStream_t)stream);
 }
 
 int gsr_normal_maps(int32_t W, int32_t H, const float* normal_img, const float* depth, const float* c2w, float fx, float fy, float cx,

@@ -68,7 +68,7 @@ __global__ void __launch_bounds__(256) k_compose(const ComposeParams p) {
         const float qn = fmaxf(__fsqrt_rn(__fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(q0, q0), __fmul_rn(q1, q1)), __fmul_rn(q2, q2)), __fmul_rn(q3, q3))), 1e-12f);
         p.rotations[4 * (size_t)n] = __fdiv_rn(q0, qn); p.rotations[4 * (size_t)n + 1] = __fdiv_rn(q1, qn);
         p.rotations[4 * (size_t)n + 2] = __fdiv_rn(q2, qn); p.rotations[4 * (size_t)n + 3] = __fdiv_rn(q3, qn);
-        p.opacities[n] = __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-p.opacity_raw[n])));
+        p.opacities[n] = sigmoid_rn(p.opacity_raw[n]);
     }
     // SH rows: shs[n] = cat(f_dc[n], f_rest[n]) (GM/:107-110).  The block's 256 rows are copied as one flat, coalesced range.
     const size_t row = (size_t)3 * p.M, rest_row = row - 3;

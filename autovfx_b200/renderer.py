@@ -23,7 +23,9 @@ gsr_activate_gaussians_backward launch replaces their autograd graph; the rest o
 
 ``render_sugar()`` is SuGaR's wrapper (``sugar_scene/sugar_model.py:1956-2228``) with the same structure: gsr_sugar_normals (and
 gsr_sugar_normals_backward) for SuGaR's own shading normals, one rasterizer pass for both colour sets, and a single colour pass
-when the caller asks for the image alone.
+when the caller asks for the image alone.  ``render_sugar_raw()`` is render_sugar() with SuGaR's colours (get_points_rgb, eval_sh
+up to degree 4) and opacities (strengths) computed from the model's raw SH leaves and densities by gsr_sugar_colors, and their
+backward by one gsr_sugar_colors_backward launch.
 
 Same argument names, return keys and error behaviour as the reference function.
 """
@@ -40,7 +42,7 @@ from . import rasterizer as R
 from .rasterizer import GaussianRasterizationSettings, _dev_f32
 from .scene import fov2focal
 
-__all__ = ["render", "render_raw", "render_sugar", "sugar_normals", "quaternion_to_matrix", "axis_normals", "normal_maps", "pack_frame", "fov2focal", "TURBO_LUT_BGR"]
+__all__ = ["render", "render_raw", "render_sugar", "render_sugar_raw", "sugar_normals", "quaternion_to_matrix", "axis_normals", "normal_maps", "pack_frame", "fov2focal", "TURBO_LUT_BGR"]
 
 
 # ------------------------------------------------------------------------------------------ the three post kernels
@@ -528,6 +530,16 @@ def render_sugar(self, nerf_cameras=None, camera_indices=0, verbose=False, bg_co
     ``use_same_scale_in_all_directions`` hands the rasterizer, and face the camera from ``positions``, as in the reference.  So
     does the reference's pseudo normal: the flipped c2w and ``fx = fov2focal(self.tanfovx, w)`` (a tangent where a field of view is
     expected)."""
+    return _render_sugar(self, None, nerf_cameras, camera_indices, verbose, bg_color, sh_deg, sh_rotations, compute_color_in_rasterizer,
+                         compute_covariance_in_rasterizer, return_2d_radii, quaternions, use_same_scale_in_all_directions, return_opacities,
+                         return_colors, positions, point_colors)
+
+
+def _render_sugar(self, raw, nerf_cameras, camera_indices, verbose, bg_color, sh_deg, sh_rotations, compute_color_in_rasterizer,
+                  compute_covariance_in_rasterizer, return_2d_radii, quaternions, use_same_scale_in_all_directions, return_opacities,
+                  return_colors, positions, point_colors):
+    """render_sugar()'s body.  ``raw`` None: the colours and opacities come from the model's get_points_rgb / strengths; otherwise
+    it is the checked (sh_dc, sh_rest, densities) of render_sugar_raw() and they come from _SugarColors."""
     if nerf_cameras is None:
         nerf_cameras = self.nerfmodel.training_cameras
     device = self.device
@@ -547,24 +559,28 @@ def render_sugar(self, nerf_cameras=None, camera_indices=0, verbose=False, bg_co
         viewmatrix=world_view_transform, projmatrix=full_proj_transform, sh_degree=sh_deg, campos=camera_center, prefiltered=False,
         debug=False)
 
-    if point_colors is None:
-        if not compute_color_in_rasterizer:
-            if sh_rotations is None:
-                splat_colors = self.get_points_rgb(positions=positions, camera_centers=camera_center, sh_levels=sh_deg + 1)
-            else:
-                splat_colors = self.get_points_rgb(
-                    positions=positions, camera_centers=None,
-                    directions=(torch.nn.functional.normalize(positions - camera_center, dim=-1).unsqueeze(1) @ sh_rotations)[..., 0, :],
-                    sh_levels=sh_deg + 1)
-            shs = None
-        else:
-            shs = self.sh_coordinates
-            splat_colors = None
+    if raw is not None:
+        shs, splat_colors, splat_opacities = _sugar_raw_colors(self, raw, positions, camera_center, sh_deg, sh_rotations,
+                                                               compute_color_in_rasterizer, point_colors)
     else:
-        splat_colors = point_colors
-        shs = None
+        if point_colors is None:
+            if not compute_color_in_rasterizer:
+                if sh_rotations is None:
+                    splat_colors = self.get_points_rgb(positions=positions, camera_centers=camera_center, sh_levels=sh_deg + 1)
+                else:
+                    splat_colors = self.get_points_rgb(
+                        positions=positions, camera_centers=None,
+                        directions=(torch.nn.functional.normalize(positions - camera_center, dim=-1).unsqueeze(1) @ sh_rotations)[..., 0, :],
+                        sh_levels=sh_deg + 1)
+                shs = None
+            else:
+                shs = self.sh_coordinates
+                splat_colors = None
+        else:
+            splat_colors = point_colors
+            shs = None
 
-    splat_opacities = self.strengths.view(-1, 1)
+        splat_opacities = self.strengths.view(-1, 1)
     if quaternions is None:
         quaternions = self.quaternions
     if not use_same_scale_in_all_directions:
@@ -631,3 +647,148 @@ def render_sugar(self, nerf_cameras=None, camera_indices=0, verbose=False, bg_co
     if return_colors:
         outputs["colors"] = splat_colors
     return outputs
+
+
+# ------------------------------------------------------------------------------------------ render_sugar_raw()
+_SUGAR_RAW_FIELDS = ("_sh_coordinates_dc", "_sh_coordinates_rest", "all_densities")
+
+
+def _sugar_raw_leaves(self, sh_deg, with_colors: bool) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """The SuGaR model's raw SH leaves and densities (_sh_coordinates_dc [P,1,3], _sh_coordinates_rest [P,M-1,3], all_densities
+    with P elements), checked, and with ``with_colors`` the degree eval_sh will be called with."""
+    dev = torch.device(self.device)
+    leaves = []
+    for f in _SUGAR_RAW_FIELDS:
+        t = getattr(self, f, None)
+        if not isinstance(t, torch.Tensor):
+            raise ValueError("render_sugar_raw: the model has no tensor %s" % f)
+        if t.dtype != torch.float32:
+            raise ValueError("render_sugar_raw: self.%s must be float32, not %s" % (f, t.dtype))
+        if t.device.type != dev.type or (dev.index is not None and t.device.index != dev.index):
+            raise ValueError("render_sugar_raw: self.%s is on %s, the model on %s" % (f, t.device, dev))
+        leaves.append(t)
+    sh_dc, sh_rest, dens = leaves
+    P = sh_dc.shape[0]
+    if tuple(sh_dc.shape) != (P, 1, 3):
+        raise ValueError("render_sugar_raw: self._sh_coordinates_dc has shape %s, expected [P, 1, 3]" % (tuple(sh_dc.shape),))
+    if sh_rest.dim() != 3 or sh_rest.shape[0] != P or sh_rest.shape[2] != 3:
+        raise ValueError("render_sugar_raw: self._sh_coordinates_rest has shape %s, expected [%d, M-1, 3]" % (tuple(sh_rest.shape), P))
+    if dens.numel() != P:
+        raise ValueError("render_sugar_raw: self.all_densities has %d elements, expected %d" % (dens.numel(), P))
+    if getattr(self, "return_one_densities", False):
+        raise ValueError("render_sugar_raw: self.return_one_densities is set; its strengths are ones, not the sigmoid this path "
+                         "differentiates; use render_sugar")
+    if with_colors:  # the asserts of SuGaR's eval_sh
+        M = sh_rest.shape[1] + 1
+        if isinstance(sh_deg, bool) or not isinstance(sh_deg, int) or not 0 <= sh_deg <= 4:
+            raise ValueError("render_sugar_raw: sh_deg must be an integer in 0..4 (SuGaR's eval_sh), got %r" % (sh_deg,))
+        if (sh_deg + 1) ** 2 > M:
+            raise ValueError("render_sugar_raw: sh_deg %d needs %d SH coefficients per channel, the model stores M = %d"
+                             % (sh_deg, (sh_deg + 1) ** 2, M))
+    if not sh_dc.is_cuda:
+        raise RuntimeError("autovfx_b200.renderer: CUDA tensors required (there is no CPU path)")
+    return sh_dc, sh_rest, dens
+
+
+class _SugarColors(torch.autograd.Function):
+    """(src, campos, sh_dc, sh_rest, densities, deg, directions_mode) -> (colors [P,3], opacities [P,1]) of SuGaR's get_points_rgb and
+    strengths: one gsr_sugar_colors launch, and one gsr_sugar_colors_backward launch for the backward.  src is the positions
+    (camera-centre mode, with campos) or the view directions (directions_mode).  src = None gives the opacities alone; then the SH
+    leaves are not read and get no gradient."""
+
+    @staticmethod
+    def forward(ctx, src, campos, sh_dc, sh_rest, densities, deg, directions_mode):
+        device = densities.device
+        P, M = sh_dc.shape[0], sh_rest.shape[1] + 1
+        f = dict(dtype=torch.float32, device=device)
+        dens = densities.detach().contiguous()
+        opac = torch.empty((P, 1), **f)
+        ctx.with_colors, ctx.deg, ctx.M, ctx.directions_mode = src is not None, int(deg), M, bool(directions_mode)
+        ctx.set_materialize_grads(False)
+        p = R._ptr
+        if src is None:
+            with torch.cuda.device(device):
+                _lib.check(_L.gsr_sugar_colors(P, M, 0, None, None, None, None, None, p(dens), None, p(opac), _lib.stream_ptr(device)),
+                           "gsr_sugar_colors")
+            ctx.save_for_backward(dens)
+            return opac
+        src_ = _dev_f32(src.detach(), device)
+        if tuple(src_.shape) != (P, 3):
+            raise ValueError("render_sugar_raw: %s has shape %s, expected [%d, 3]" % ("directions" if directions_mode else "positions",
+                                                                                   tuple(src_.shape), P))
+        c = None if directions_mode else _dev_f32(campos.detach(), device).reshape(-1)
+        dc, rest = sh_dc.detach().contiguous(), sh_rest.detach().contiguous()
+        colors = torch.empty((P, 3), **f)
+        with torch.cuda.device(device):
+            pos, dirs = (None, p(src_)) if directions_mode else (p(src_), None)
+            _lib.check(_L.gsr_sugar_colors(P, M, ctx.deg, pos, None if c is None else c.data_ptr(), dirs, p(dc), p(rest), p(dens), p(colors),
+                                           p(opac), _lib.stream_ptr(device)), "gsr_sugar_colors")
+        ctx.save_for_backward(dens, src_, dc, rest, *(() if c is None else (c,)))
+        return colors, opac
+
+    @staticmethod
+    def backward(ctx, *grads):
+        device = ctx.saved_tensors[0].device
+        p = R._ptr
+        if not ctx.with_colors:
+            (dens,), (g_op,) = ctx.saved_tensors, grads
+            if g_op is None:
+                return None, None, None, None, None, None, None
+            g_op = _dev_f32(g_op, device)
+            d_dens = torch.empty_like(dens)
+            with torch.cuda.device(device):
+                _lib.check(_L.gsr_sugar_colors_backward(dens.numel(), ctx.M, 0, None, None, None, None, None, p(dens), None, p(g_op), None,
+                                                        None, None, p(d_dens), _lib.stream_ptr(device)), "gsr_sugar_colors_backward")
+            return None, None, None, None, d_dens, None, None
+        dens, src, dc, rest = ctx.saved_tensors[:4]
+        c = None if ctx.directions_mode else ctx.saved_tensors[4]
+        g_col, g_op = grads
+        g_col = None if g_col is None else _dev_f32(g_col, device)
+        g_op = None if g_op is None else _dev_f32(g_op, device)
+        d_src = d_dc = d_rest = d_dens = None
+        if g_col is not None:
+            d_src, d_dc, d_rest = torch.empty_like(src), torch.empty_like(dc), torch.empty_like(rest)
+        if g_op is not None:
+            d_dens = torch.empty_like(dens)
+        if g_col is not None or g_op is not None:
+            pos, dirs = (None, p(src)) if ctx.directions_mode else (p(src), None)
+            with torch.cuda.device(device):
+                _lib.check(_L.gsr_sugar_colors_backward(dc.shape[0], ctx.M, ctx.deg, pos, None if c is None else c.data_ptr(), dirs, p(dc),
+                                                        p(rest), p(dens), p(g_col), p(g_op), p(d_dc), p(d_rest), p(d_src), p(d_dens),
+                                                        _lib.stream_ptr(device)), "gsr_sugar_colors_backward")
+        return d_src, None, d_dc, d_rest, d_dens, None, None
+
+
+def _sugar_raw_colors(self, raw, positions, camera_center, sh_deg, sh_rotations, compute_color_in_rasterizer, point_colors):
+    """(shs, splat_colors, splat_opacities) of SS/:2063-2080 from the raw leaves through _SugarColors."""
+    sh_dc, sh_rest, dens = raw
+    if point_colors is not None or compute_color_in_rasterizer:  # the opacities alone
+        opacities = _SugarColors.apply(None, None, sh_dc, sh_rest, dens, 0, False)
+        return (self.sh_coordinates if point_colors is None else None), point_colors, opacities
+    if sh_rotations is None:
+        colors, opacities = _SugarColors.apply(positions, camera_center, sh_dc, sh_rest, dens, sh_deg, False)
+    else:
+        directions = (torch.nn.functional.normalize(positions - camera_center, dim=-1).unsqueeze(1) @ sh_rotations)[..., 0, :]
+        colors, opacities = _SugarColors.apply(directions, None, sh_dc, sh_rest, dens, sh_deg, True)
+    return None, colors, opacities
+
+
+def render_sugar_raw(self, nerf_cameras=None, camera_indices=0, verbose=False, bg_color=None, sh_deg=None, sh_rotations=None,
+                     compute_color_in_rasterizer=False, compute_covariance_in_rasterizer=True, return_2d_radii=False, quaternions=None,
+                     use_same_scale_in_all_directions=False, return_opacities=False, return_colors=False, positions=None, point_colors=None):
+    """render_sugar() with SuGaR's colours and opacities computed in CUDA from the model's raw leaves; a SuGaR model opts in with
+    ``SuGaR.render_image_gaussian_rasterizer = render_sugar_raw``.  Same signature, return values, shapes and strides.
+
+    ``get_points_rgb`` (SuGaR's eval_sh, degrees 0-4, ``+ 0.5``, ``clamp_min(0)``) and ``strengths`` (``sigmoid(all_densities)``)
+    are one gsr_sugar_colors launch, and their backward one gsr_sugar_colors_backward launch, instead of the model's torch graph.
+    The raw leaves read are ``_sh_coordinates_dc`` [P,1,3], ``_sh_coordinates_rest`` [P,M-1,3] (M = 1 allowed) and
+    ``all_densities``; everything else (points, scaling, quaternions, sh_coordinates, the camera) comes through the getters
+    render_sugar reads, so a mesh-bound model works as an unbound one.  Branches: ``point_colors`` and
+    ``compute_color_in_rasterizer=True`` take the opacities alone (the SH leaves get no gradient from them); ``sh_rotations``
+    passes the rotated directions, built in torch as the reference builds them; ``positions=`` receives the direction gradient.
+    ValueError: a missing, non-float32 or misplaced leaf, a leaf of the wrong shape, ``return_one_densities`` set, or, when the
+    colours are evaluated, ``sh_deg`` outside 0..4 or needing more than M coefficients (the reference's asserts)."""
+    raw = _sugar_raw_leaves(self, sh_deg, point_colors is None and not compute_color_in_rasterizer)
+    return _render_sugar(self, raw, nerf_cameras, camera_indices, verbose, bg_color, sh_deg, sh_rotations, compute_color_in_rasterizer,
+                         compute_covariance_in_rasterizer, return_2d_radii, quaternions, use_same_scale_in_all_directions, return_opacities,
+                         return_colors, positions, point_colors)

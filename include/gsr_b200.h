@@ -24,6 +24,9 @@
  *   gsr_activate_gaussians_backward replaces the autograd backward of those activations and of get_normal * 0.5 + 0.5
  *   gsr_sugar_normals replaces  SuGaR's shading normal * 0.5 + 0.5               sugar_scene/sugar_model.py:2164-2168 (get_smallest_axis :801-815)
  *   gsr_sugar_normals_backward replaces its autograd backward (gradient with respect to the raw quaternions)
+ *   gsr_sugar_colors  replaces  SuGaR.get_points_rgb (eval_sh, degrees 0-4) and   sugar_model.py:711-755, :394-398
+ *                               SuGaR.strengths = sigmoid(all_densities)           (sugar_utils/spherical_harmonics.py:117-172)
+ *   gsr_sugar_colors_backward replaces their autograd backward
  *
  * Conventions (same as the reference's C++ layer):
  *   - every pointer is a DEVICE pointer to contiguous fp32 / int32 data unless it says "host";
@@ -167,6 +170,27 @@ int gsr_sugar_normals(int32_t P, const float* positions, const float* scales, co
  * gradient.  Every pointer is required when P > 0. */
 int gsr_sugar_normals_backward(int32_t P, const float* positions, const float* scales, const float* quaternions, const float* campos,
                                const float* dL_dnormals, float* dL_dquaternions, void* stream);
+
+/* SuGaR's per-Gaussian colours and opacities (SuGaR.get_points_rgb with its eval_sh, degrees 0..4, and SuGaR.strengths):
+ *   out_colors [P,3]  = clamp_min(eval_sh(deg, cat(sh_dc, sh_rest)[:, :(deg+1)^2], dirs) + 0.5, 0)
+ *   out_opacities [P] = sigmoid(densities)
+ * dirs = F.normalize(positions - campos) (1e-12 clamp) when directions == NULL, otherwise directions [P,3] as given (not
+ * normalised).  sh_dc [P,1,3], sh_rest [P,M-1,3] (may be NULL when M == 1), densities [P], positions [P,3], campos [3].  One
+ * IEEE rounding per torch op in the order SuGaR's Python writes them.  out_colors == NULL skips the colours (no SH, position or
+ * direction is read); out_opacities == NULL skips the opacities (densities is not read).  deg outside 0..4 or
+ * M < (deg+1)^2 is GSR_ERR_INVALID.  P = 0 is a no-op. */
+int gsr_sugar_colors(int32_t P, int32_t M, int32_t deg, const float* positions, const float* campos, const float* directions,
+                     const float* sh_dc, const float* sh_rest, const float* densities, float* out_colors, float* out_opacities, void* stream);
+
+/* Backward of gsr_sugar_colors (same P, M, deg and inputs): dL_dcolors [P,3] and / or dL_dopacities [P] in (either may be NULL).
+ * With dL_dcolors: dL_dsh_dc [P,1,3], dL_dsh_rest [P,M-1,3] (coefficients beyond the active degree get zeros) and dL_dpositions
+ * [P,3] (the gradient of `directions` when directions != NULL) are written in full.  With dL_dopacities: dL_ddensities [P] =
+ * g * o (1 - o).  The clamp decisions (gradient where the pre-clamp colour is >= 0) and the normalisation branch (below 1e-12
+ * the denominator is the constant 1e-12) are recomputed from the inputs; nothing is kept between the two calls. */
+int gsr_sugar_colors_backward(int32_t P, int32_t M, int32_t deg, const float* positions, const float* campos, const float* directions,
+                              const float* sh_dc, const float* sh_rest, const float* densities, const float* dL_dcolors,
+                              const float* dL_dopacities, float* dL_dsh_dc, float* dL_dsh_rest, float* dL_dpositions, float* dL_ddensities,
+                              void* stream);
 
 /* normal_img [3,H,W] (a rendered normal*0.5+0.5 image) -> out_normal [H,W,3] = normalize((img - 0.5) * 2);
  * depth [H,W] -> out_pseudo [H,W,3] = normalised cross product of central differences of the unprojected depth map,

@@ -1,14 +1,19 @@
 """SuGaR coarse-training step throughput: SuGaR's render_image_gaussian_rasterizer as the reference writes it (two GaussianRasterizer
-calls on the drop-in, the normals as torch ops: tests/sugar_ref.sugar_render_two_pass) against renderer.render_sugar.
+calls on the drop-in, the normals as torch ops: tests/sugar_ref.sugar_render_two_pass) against renderer.render_sugar and
+renderer.render_sugar_raw (SuGaR's colours and opacities from the raw leaves in CUDA).
 
 One step is a regularised step of sugar/sugar_trainers/coarse_density.py: render one trajectory camera with
 compute_color_in_rasterizer=False, return_2d_radii=True, return_opacities=True; loss = L1 on the image + L1 between "normal" and
 "pseudo_normal".detach() + the opacity entropy term; then the SDF branch's depth render with gradients (point_colors = view-space
-depth, bg = its maximum, channel 0 of the image only) added to the loss; loss.backward().  The two arms alternate step by step in
+depth, bg = its maximum, channel 0 of the image only) added to the loss; loss.backward().  The three arms alternate step by step in
 one process, each step timed with CUDA events after warm-up.  --profile instead counts the kernels of one step per arm with
-torch.profiler; --frames times the no-grad frame call of sugar/render.py (return_2d_radii, the normal maps) in frames/s.
+torch.profiler, and those of the model's colour graph alone (get_points_rgb once and strengths twice, forward and backward: what
+render_sugar_raw replaces in a step); --frames times the no-grad frame call of sugar/render.py (return_2d_radii, the normal maps) in
+frames/s.  --sh-degree 4 runs SuGaR's own storage, M = 25, at degree 4 (the model's get_points_rgb then evaluates SuGaR's degree-4
+eval_sh: tests/sugar_colors_ref.py).
 
     python tools/bench_train_sugar.py --steps 20 --warmup 3 [--gaussians 3000000] [--width 1920 --height 1080] [--profile] [--frames]
+                                      [--sh-degree 4]
 """
 from __future__ import annotations
 
@@ -39,15 +44,24 @@ def main():
     ap.add_argument("--height", type=int, default=1080)
     ap.add_argument("--profile", action="store_true", help="count the kernels of one step per arm instead of timing")
     ap.add_argument("--frames", action="store_true", help="time the no-grad frame call instead of the training step")
+    ap.add_argument("--sh-degree", type=int, default=3, choices=(3, 4), help="3: M = 16; 4: M = 25 (SuGaR's storage)")
     args = ap.parse_args()
     dev = torch.device("cuda:0")
+    deg = args.sh_degree
     g = {k: v.to(dev) for k, v in scene.config3_scene(P=args.gaussians).items()}  # SH degree 3: M = 16
+    if deg == 4:  # nine more coefficients per channel, drawn like the degree-3 ones
+        extra = torch.randn(args.gaussians, 9, 3, generator=torch.Generator().manual_seed(1)).to(dev) * 0.1
+        g["shs"] = torch.cat([g["shs"], extra], 1).contiguous()
     traj = scene.trajectory_dict(radius=4.0, num_views=300, theta=30.0, w=args.width, h=args.height, fov_x_deg=60.0)
     eyes = [np.asarray(f["transform_matrix"], dtype=np.float64)[:3, 3] for f in traj["frames"]]
     cams = SR.Cameras(eyes, device=dev)
-    model = SR.SugarModel(g, cams, args.width, args.height, math.radians(60.0))
+    if deg == 3:
+        model = SR.SugarModel(g, cams, args.width, args.height, math.radians(60.0))
+    else:
+        from tests import sugar_colors_ref as SC
+        model = SC.SugarModel4(g, cams, args.width, args.height, math.radians(60.0))
     params = list(model.leaves.values())
-    arms = {"render_sugar": renderer.render_sugar, "two_pass": SR.sugar_render_two_pass}
+    arms = {"render_sugar": renderer.render_sugar, "two_pass": SR.sugar_render_two_pass, "render_sugar_raw": renderer.render_sugar_raw}
     gen = torch.Generator().manual_seed(0)
     gt = torch.rand(args.height, args.width, 3, generator=gen).to(dev)
 
@@ -56,7 +70,7 @@ def main():
         for p in params:
             p.grad = None
         ci = i % len(cams.p3d_cameras)
-        out = fn(model, nerf_cameras=cams, camera_indices=ci, sh_deg=3, compute_color_in_rasterizer=False, return_2d_radii=True,
+        out = fn(model, nerf_cameras=cams, camera_indices=ci, sh_deg=deg, compute_color_in_rasterizer=False, return_2d_radii=True,
                  return_opacities=True)
         img = out["image"][..., :3]
         loss = (img - gt).abs().mean()
@@ -74,7 +88,7 @@ def main():
 
     def frame(arm, i):
         with torch.no_grad():
-            arms[arm](model, nerf_cameras=cams, camera_indices=i % len(cams.p3d_cameras), sh_deg=3, return_2d_radii=True)
+            arms[arm](model, nerf_cameras=cams, camera_indices=i % len(cams.p3d_cameras), sh_deg=deg, return_2d_radii=True)
 
     work = frame if args.frames else step
     for i in range(args.warmup):
@@ -82,7 +96,8 @@ def main():
             work(arm, i)
     torch.cuda.synchronize()
     res = {"workload": ("no-grad frame" if args.frames else "SuGaR coarse-density step with the SDF depth render") +
-           ", %.1fM Gaussians SH-deg 3 (M=16), %dx%d, 300-camera trajectory" % (args.gaussians / 1e6, args.width, args.height),
+           ", %.1fM Gaussians SH-deg %d (M=%d), %dx%d, 300-camera trajectory" % (args.gaussians / 1e6, deg, (deg + 1) ** 2, args.width,
+                                                                                  args.height),
            "card": card()}
     try:
         res["card"]["clocks_mhz"] = {"sm": torch.cuda.clock_rate()}
@@ -90,13 +105,32 @@ def main():
         pass
     if args.profile:
         from torch.profiler import ProfilerActivity, profile
-        for arm in arms:
+
+        def kernels_of(fn):
             with profile(activities=[ProfilerActivity.CUDA]) as prof:
-                work(arm, args.warmup)
+                fn()
                 torch.cuda.synchronize()
-            kernels = [e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA and "memcpy" not in e.name.lower()
-                       and "memset" not in e.name.lower()]
+            return [e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA and "memcpy" not in e.name.lower()
+                    and "memset" not in e.name.lower()]
+        for arm in arms:
+            kernels = kernels_of(lambda: work(arm, args.warmup))
             res[arm] = {"kernels_per_step": len(kernels), "kernel_ms": sum(e.device_time for e in kernels) / 1000.0}
+            if arm == "render_sugar_raw":
+                res[arm]["colour_kernels"] = sorted({e.name for e in kernels if "sugar_colors" in e.name})
+        if not args.frames:  # the model's colour graph of one step, forward and backward, with its gradient seeds made beforehand
+            camera_center = cams.p3d_cameras[args.warmup % len(cams.p3d_cameras)].get_camera_center()
+            seeds = (torch.ones(args.gaussians, 3, device=dev), torch.ones(args.gaussians, 1, device=dev),
+                     torch.ones(args.gaussians, 1, device=dev))
+
+            def colour_graph():
+                for p in params:
+                    p.grad = None
+                colors = model.get_points_rgb(positions=model.points, camera_centers=camera_center, sh_levels=deg + 1)
+                torch.autograd.backward((colors, model.strengths.view(-1, 1), model.strengths.view(-1, 1)), seeds)
+            colour_graph()
+            kernels = kernels_of(colour_graph)
+            res["colour_graph"] = {"kernels": len(kernels), "kernel_ms": sum(e.device_time for e in kernels) / 1000.0,
+                                   "share_of_render_sugar_step": len(kernels) / res["render_sugar"]["kernels_per_step"]}
         print(json.dumps(res))
         return
     ms = {a: [] for a in arms}
@@ -115,6 +149,7 @@ def main():
         res[arm] = {unit + "_median": float(np.median(rate)), unit + "_p10": float(np.percentile(rate, 10)),
                     unit + "_p90": float(np.percentile(rate, 90)), "ms_median": float(np.median(v))}
     res["speedup_median"] = res["render_sugar"][unit + "_median"] / res["two_pass"][unit + "_median"]
+    res["raw_over_render_sugar_median"] = res["render_sugar_raw"][unit + "_median"] / res["render_sugar"][unit + "_median"]
     print(json.dumps(res))
 
 
