@@ -41,6 +41,9 @@ int activate_backward_impl(int N, int M, const float* xyz, const float* campos, 
                            float* d_frest, cudaStream_t st);
 int dist2_impl(int P, const float* points, float* out, void* ws, size_t ws_bytes, cudaStream_t st);
 size_t dist2_bytes(int P);
+int knn_impl(int P1, int P2, int K, const float* queries, const float* points, float* out_d, int64_t* out_i, void* ws, size_t ws_bytes,
+             cudaStream_t st);
+size_t knn_bytes(int P1, int P2);
 int profile_begin(int max_frames, int stride);
 int set_option(const char* name, int value);
 int profile_end(float* ms, int* frames);
@@ -171,6 +174,16 @@ size_t gsr_dist2_bytes(int32_t P) { return gsr::dist2_bytes(P); }
 int gsr_dist2(int32_t P, const float* points, float* mean_dists, void* workspace, size_t workspace_bytes, void* stream) {
     NvtxRange nvtx_("gsr_dist2");
     return gsr::dist2_impl(P, points, mean_dists, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+size_t gsr_knn_bytes(int32_t P1, int32_t P2, int32_t K) {
+    (void)K;  // the workspace does not depend on K
+    return gsr::knn_bytes(P1, P2);
+}
+int gsr_knn(int32_t P1, int32_t P2, int32_t K, const float* queries, const float* points, float* out_dists, int64_t* out_idx,
+            void* workspace, size_t workspace_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_knn");
+    return gsr::knn_impl(P1, P2, K, queries, points, out_dists, out_idx, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 int gsr_profile_begin(int max_frames) { return gsr::profile_begin(max_frames, 1); }

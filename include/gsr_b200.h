@@ -10,6 +10,7 @@
  *                               (Rasterizer::backward, rasterizer_impl.cu:343-446)
  *   gsr_mark_visible  replaces  _C.mark_visible                  DGR/rasterize_points.cu:211-230
  *   gsr_dist2         replaces  simple_knn._C.distCUDA2          KNN/spatial.cu:15-26 (SimpleKNN::knn, KNN/simple_knn.cu:185-220)
+ *   gsr_knn           replaces  pytorch3d.ops.knn_points in SuGaR  sugar_scene/sugar_model.py:47, :233, :899, :914, :1213 (N = 1, D = 3)
  *
  * and, for the render() wrapper around the two rasterizer passes ("GR/" = sugar/gaussian_splatting/gaussian_renderer/__init__.py):
  *
@@ -281,6 +282,16 @@ int gsr_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, c
 size_t gsr_dist2_bytes(int32_t P);
 int gsr_dist2(int32_t P, const float* points, float* mean_dists, void* workspace, size_t workspace_bytes,
               void* stream);
+
+/* Exact K nearest neighbours (pytorch3d.ops.knn_points for one cloud pair in 3-D): for each of the P1 queries [P1,3], the K
+ * nearest of the P2 points [P2,3], ascending, as squared distances out_dists [P1,K] and indices into points out_idx [P1,K].
+ * queries == NULL: the queries are the points themselves (P1 == P2).  d = (dx*dx + dy*dy) + dz*dz, dx = point.x - query.x,
+ * each operation rounded once (no FMA).  Ties in d go to the lower index; the query itself is not excluded.
+ * 1 <= K <= 32 and K <= P2, otherwise GSR_ERR_INVALID.  P1 = 0 launches nothing.  `workspace` needs gsr_knn_bytes(P1, P2, K)
+ * bytes (with queries == NULL, gsr_knn_bytes(0, P2, K) suffices). */
+size_t gsr_knn_bytes(int32_t P1, int32_t P2, int32_t K);
+int gsr_knn(int32_t P1, int32_t P2, int32_t K, const float* queries, const float* points, float* out_dists, int64_t* out_idx,
+            void* workspace, size_t workspace_bytes, void* stream);
 
 /* Device pointers into the workspaces of the last layout (P, capacity, W, H) — for parity tests that
  * compare per-stage buffers with the reference (SURVEY §4).  Pure pointer arithmetic, no CUDA calls. */
