@@ -27,7 +27,7 @@ struct GeomLayout {
         size_t o = 0;
         records = o; o = align_up(o + 48 * P, 256);
         ranks = o;   o = align_up(o + 32 * P, 256);  // 8 x u32 in-tile ranks for Gaussians touching <= 8 tiles
-        vis_list = o; o = align_up(o + 4 * P, 256);  // ids of the visible Gaussians (k_project -> k_color_emit)
+        vis_list = o; o = align_up(o + 4 * P, 256);  // ids of the visible Gaussians (k_project -> k_emit)
         cov3D = o;   o = align_up(o + 24 * P, 256);
         clamped = o; o = align_up(o + P, 256);
         total = o + 256;

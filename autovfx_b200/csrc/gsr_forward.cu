@@ -1,4 +1,4 @@
-// gsr_b200 forward pass: projection -> tile histogram/scan -> colour + instance emission -> per-tile depth sort -> blend.
+// gsr_b200 forward pass: projection + colour -> tile histogram/scan -> instance emission -> per-tile depth sort -> blend.
 //
 // Replaces CudaRasterizer::Rasterizer::forward (DGR/cuda_rasterizer/rasterizer_impl.cu:197-339) and the
 // kernels it drives (forward.cu:155-256 preprocessCUDA, rasterizer_impl.cu:70-138 duplicateWithKeys /
@@ -6,10 +6,10 @@
 //
 // Pipeline (results are identical, see DESIGN.md):
 //   k_project     every Gaussian: near cull, conservative screen test, EWA projection, radius, tile rectangle, ranked per-tile
-//                 tickets, the geometry part of the record, the compact list of visible Gaussians;
+//                 tickets, SH -> RGB from a TMA-staged row, the whole record, the compact list of visible Gaussians;
 //   k_tile_scan   exclusive scan over the tiles: ranges, R and the overflow flag stay on the device (no host round trip);
-//   k_color_emit  every VISIBLE Gaussian: SH -> RGB from a TMA-staged row, one (depth bits, id, footprint mask) pair per
-//                 (Gaussian, tile) scattered to ranges[tile].x + rank;
+//   k_emit        every VISIBLE Gaussian: one (depth bits, id, footprint mask) pair per (Gaussian, tile) scattered to
+//                 ranges[tile].x + rank;
 //   k_sort_tiles  one CTA per tile sorts its bucket by (depth bits, id) — exactly the order of the reference's stable radix sort
 //                 of (tile | depth) keys, because the reference emits every (tile, Gaussian) pair once in ascending Gaussian id
 //                 (rasterizer_impl.cu:98-108) — and transposes the footprint masks into the ballot matrix;
@@ -43,7 +43,7 @@ int check_launch(const char* what, bool debug, cudaStream_t stream) {
 }
 
 // =====================================================================================================
-// Kernel 1: projection of every Gaussian (k_project); its colour is evaluated later, only for the visible ones (k_color_emit)
+// Kernel 1: projection and colour of every Gaussian (k_project)
 // =====================================================================================================
 struct PreParams {
     int P, D, M, W, H, gx, gy;
@@ -62,6 +62,7 @@ struct PreParams {
 };
 
 constexpr int PRE_THREADS = 128;
+constexpr int EMIT_MINB = 8;  // resident CTAs per SM k_emit is compiled for
 
 __host__ __device__ constexpr int sh_nf(int deg) { return 3 * (deg + 1) * (deg + 1); }
 __host__ __device__ constexpr int sh_nv(int deg, bool win) { return (sh_nf(deg) + 3) / 4 + (win ? 1 : 0); }  // float4 per staged row
@@ -76,6 +77,8 @@ __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(gmem));
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
+// orders this thread's earlier generic-proxy accesses to shared memory before later async-proxy (TMA) writes to it
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 
 // TMA bulk copy (cp.async.bulk, SASS UBLKCP) of one contiguous row global -> shared, completion on an mbarrier
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -187,28 +190,46 @@ __device__ __forceinline__ void cov3d_ref_rounding(float sx, float sy, float sz,
     c3[5] = __fmaf_rn(M22, M22, __fmaf_rn(M20, M20, __fmul_rn(M21, M21)));
 }
 
-// Kernel 1 of 5 (colour-agnostic; DEG / VEC / BULK / WIN only matter to k_color_emit below).
+// Kernel 1 of 5.
 // Phase 1, one thread per Gaussian: load the 44 bytes of geometry, near cull, and a cheap CONSERVATIVE screen test — an upper
 // bound of the splat radius (trace and norm bounds, see radius_bound) against the image rectangle; a Gaussian it rejects has an
 // empty tile rectangle in the reference too (forward.cu:236), so it gets radius 0 without the projection math.  The survivors of
-// the CTA are compacted through shared memory.  Phase 2, one thread per survivor (whole warps retire early): 3D covariance, EWA
-// projection, conic, radius, tile rectangle (forward.cu:155-256 minus the colour), the per-tile histogram with ranked tickets,
-// and the compact list of visible Gaussians the colour + emission kernel walks.  The 192-byte SH row is not touched here.
+// the CTA are compacted through shared memory.  Phase 2, one thread per survivor (whole warps retire early): the survivor's SH
+// row is requested first, so that its latency overlaps the 3D covariance, EWA projection, conic, radius, tile rectangle
+// (forward.cu:155-256) and the per-tile histogram with ranked tickets; then SH -> RGB (forward.cu:20-71), the whole 48-byte
+// record in one go, and the compact list of visible Gaussians the emission kernel walks.
+// DEG = -1: colours are precomputed.  VEC: SH rows are 16-byte aligned (M % 4 == 0) -> 16-byte staging, either one TMA bulk
+// copy per Gaussian issued by its own lane (BULK) or coalesced cp.async by the whole warp; otherwise scalar loads.  WIN (with
+// VEC and BULK): rows are only 4-byte aligned (M = 25, the SuGaR storage: 300-byte rows) — each lane bulk-copies the 16-byte
+// aligned window that contains its coefficients (one extra float4) and evaluates from its row's offset inside the window.
 struct ProjCand {  // one phase-1 survivor
     float mx, my, mz, opacity;
     float a0, a1, a2, a3, a4, a5, a6;  // scale.xyz + rotation.rxyz, or cov3D[0..5]
     int idx;
 };
 
-template <int MINB, bool TIGHT>
-__global__ void __launch_bounds__(PRE_THREADS, MINB) k_project(const PreParams p) {
+template <int DEG, bool VEC, bool BULK, bool WIN, bool TIGHT>
+__global__ void __launch_bounds__(PRE_THREADS, 8) k_project(const PreParams p) {
+    constexpr int DG = DEG < 0 ? 0 : DEG;
+    constexpr int NF = sh_nf(DG);
+    constexpr int STRIDE = sh_stride(DG, VEC, WIN);
+    constexpr int WSTAGE = DEG < 0 ? 0 : 32 * STRIDE;  // floats per warp: the SH rows of its 32 survivors
+    constexpr size_t CAND_BYTES = sizeof(ProjCand) * PRE_THREADS, STAGE_BYTES = sizeof(float) * (PRE_THREADS / 32) * WSTAGE;
     __shared__ CamConsts cam;
     __shared__ float s_w2;                       // upper bound of the squared spectral norm of the view matrix's 3x3 part
-    __shared__ ProjCand s_cand[PRE_THREADS];
+    // the survivors, then (once every thread holds its own) the SH staging rows: one area keeps 8 CTAs per SM at degree 3
+    __shared__ __align__(16) unsigned char s_buf[CAND_BYTES > STAGE_BYTES ? CAND_BYTES : STAGE_BYTES];
+    __shared__ __align__(8) unsigned long long stage_bar[PRE_THREADS / 32];
     __shared__ int s_wcnt[PRE_THREADS / 32];
+    ProjCand* s_cand = reinterpret_cast<ProjCand*>(s_buf);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     if (tid < 16) cam.view[tid] = p.view[tid];
     else if (tid < 32) cam.proj[tid - 16] = p.proj[tid - 16];
+    else if (tid < 35) cam.campos[tid - 32] = p.campos[tid - 32];
+    if (DEG >= 0 && VEC && BULK && lane == 0) {
+        mbar_init((uint32_t)__cvta_generic_to_shared(&stage_bar[warp]), 1u);
+        mbar_fence_init();
+    }
     __syncthreads();
     if (tid == 0) {
         // rigid view matrices have orthonormal rows: then the norm is 1; anything else falls back to the Frobenius norm
@@ -283,12 +304,54 @@ __global__ void __launch_bounds__(PRE_THREADS, MINB) k_project(const PreParams p
     }
     if (cand) s_cand[base + __popc(cm & ((1u << lane) - 1u))] = me;
     __syncthreads();
-    if (warp * 32 >= ncand) return;  // whole warp without work
 
     // ---- phase 2 ----
     const bool valid = tid < ncand;
     const ProjCand c = s_cand[valid ? tid : 0];
     const int idx = c.idx;
+    if (WSTAGE > 0) {  // the staging rows overwrite s_cand
+        fence_proxy_async_smem();
+        __syncthreads();
+    }
+    if (warp * 32 >= ncand) return;  // whole warp without work
+
+    // request the SH rows of the warp's survivors now; they are waited for after the projection and the tickets
+    const unsigned cmask = __ballot_sync(GSR_FULL, valid);
+    float* wstage = reinterpret_cast<float*>(s_buf) + warp * WSTAGE;
+    const uint32_t bar = (uint32_t)__cvta_generic_to_shared(&stage_bar[warp]);
+    int win_off = 0;  // floats between the start of the staged window and the row's first coefficient (WIN only)
+    if constexpr (DEG >= 0) {
+        const size_t row_floats = (size_t)p.M * 3;
+        if (VEC && BULK) {
+            constexpr int NV = sh_nv(DG, WIN);
+            if (lane == 0) mbar_arrive_expect_tx(bar, (uint32_t)__popc(cmask) * NV * 16u);
+            if (valid) {
+                const float* src = p.shs + (size_t)idx * row_floats;
+                if (WIN) {
+                    win_off = (int)(((uintptr_t)src & 15u) >> 2);
+                    src -= win_off;
+                }
+                bulk_g2s((uint32_t)__cvta_generic_to_shared(wstage + lane * STRIDE), src, NV * 16u, bar);
+            }
+        } else if (VEC) {
+            constexpr int NV = (NF + 3) / 4;
+#pragma unroll
+            for (int it = 0; it < NV; it++) {
+                const int item = it * 32 + lane;
+                const int gl = item / NV, part = item - gl * NV;
+                const uint32_t gid = __shfl_sync(GSR_FULL, (uint32_t)idx, gl);
+                if ((cmask >> gl) & 1u) cp_async16(wstage + gl * STRIDE + part * 4, p.shs + (size_t)gid * row_floats + part * 4);
+            }
+        } else {
+#pragma unroll 4
+            for (int it = 0; it < NF; it++) {
+                const int item = it * 32 + lane;
+                const int gl = item / NF, part = item - gl * NF;
+                const uint32_t gid = __shfl_sync(GSR_FULL, (uint32_t)idx, gl);
+                if ((cmask >> gl) & 1u) wstage[gl * STRIDE + part] = p.shs[(size_t)gid * row_floats + part];
+            }
+        }
+    }
     bool vis = false;
     int radius = 0, x0 = 0, y0 = 0, x1 = 0, y1 = 0;
     float px = 0, py = 0, depth = 0, con_a = 0, con_b = 0, con_c = 0;
@@ -344,7 +407,7 @@ __global__ void __launch_bounds__(PRE_THREADS, MINB) k_project(const PreParams p
     if (!vis) { x0 = y0 = x1 = y1 = 0; }
 
     // Per-tile histogram.  Gaussians touching <= 8 tiles take a ranked ticket per tile (atomic with return) in COLUMN-major
-    // order — the order k_color_emit walks them — and store the ranks, so the emission needs no atomics.  Larger rectangles
+    // order — the order k_emit walks them — and store the ranks, so the emission needs no atomics.  Larger rectangles
     // are counted separately, warp-cooperatively.  With p.tight a tile of the reference's rectangle only receives an instance
     // if the splat can reach alpha >= 1/255 at one of its pixel centres (opt-in: lists differ from the reference's, images do not).
     const float tau = footprint_tau(opacity);
@@ -379,13 +442,30 @@ __global__ void __launch_bounds__(PRE_THREADS, MINB) k_project(const PreParams p
         }
     }
 
+    // ---- colour ----
+    float rgb[3] = {0, 0, 0};
+    unsigned clamp_bits = 0;
+    if constexpr (DEG < 0) {
+        if (vis) {
+            rgb[0] = p.colors_precomp[3 * (size_t)idx];
+            rgb[1] = p.colors_precomp[3 * (size_t)idx + 1];
+            rgb[2] = p.colors_precomp[3 * (size_t)idx + 2];
+        }
+    } else {
+        if (VEC && BULK) mbar_wait(bar, 0u);
+        else if (VEC) cp_async_wait_all();
+        __syncwarp();
+        if (vis) sh_eval<DG>(wstage + lane * STRIDE + win_off, make_float3(c.mx, c.my, c.mz), cam.campos, rgb, clamp_bits);
+    }
+
     if (valid) {
         p.radii[idx] = radius;
         if (vis) {
             float4* rec = p.records + 3 * (size_t)idx;
             rec[0] = make_float4(px, py, con_a, con_b);
             rec[1] = make_float4(con_c, opacity, depth, __int_as_float(radius));
-            rec[2] = make_float4(c.mx, c.my, c.mz, 0.0f);  // the mean, for k_color_emit's view direction (it overwrites the quad with the colour)
+            rec[2] = make_float4(rgb[0], rgb[1], rgb[2], log2f(opacity));  // .w: log2(opacity) for the default blend
+            if (p.for_backward) p.clamped[idx] = (uint8_t)clamp_bits;
             if (rect_n <= 8) {
                 uint4* rr = reinterpret_cast<uint4*>(p.ranks + 8 * (size_t)idx);
                 rr[0] = make_uint4(rk[0], rk[1], rk[2], rk[3]);
@@ -497,23 +577,16 @@ __global__ void __launch_bounds__(1024) k_tile_scan(const uint32_t* __restrict__
 }
 
 // =====================================================================================================
-// Kernel 3 of 5: colour + instance emission, one thread per VISIBLE Gaussian (the compact list k_project wrote), every
-// lane busy.  (a) SH -> RGB (forward.cu:20-71) from the Gaussian's SH row, staged by ONE TMA bulk copy issued by its own
-// lane; (b) the work of duplicateWithKeys (rasterizer_impl.cu:70-111): one (depth bits, id) pair per (Gaussian, tile)
-// scattered to ranges[tile].x + rank — the ranks were drawn by k_project, so no atomics for rectangles of <= 8 tiles;
-// (c) PACKED (P <= 2^24): the pair's low word is (id << 8 | mask), mask = which of the tile's eight 8x4 warp footprints the
-// splat can touch (strip intervals, computed once per tile column of the rectangle), so k_sort_tiles needs no gather.
-// The kernel streams 192 B of SH per thread and has issue slots to spare for (c).
-// DEG = -1: colours are precomputed.  VEC: SH rows are 16-byte aligned (M % 4 == 0) -> 16-byte staging, either one TMA
-// bulk copy per Gaussian (BULK) or coalesced cp.async by the whole warp.  WIN (with VEC and BULK): rows are only 4-byte
-// aligned (M = 25, the SuGaR storage: 300-byte rows) — each lane bulk-copies the 16-byte aligned window that contains its
-// coefficients (one extra float4) and evaluates from its row's offset inside the window.
+// Kernel 3 of 5: instance emission, one thread per VISIBLE Gaussian (the compact list k_project wrote), every lane busy.
+// (a) the work of duplicateWithKeys (rasterizer_impl.cu:70-111): one (depth bits, id) pair per (Gaussian, tile) scattered to
+// ranges[tile].x + rank — the ranks were drawn by k_project, so no atomics for rectangles of <= 8 tiles; (b) PACKED
+// (P <= 2^24): the pair's low word is (id << 8 | mask), mask = which of the tile's eight 8x4 warp footprints the splat can
+// touch (strip intervals, computed once per tile column of the rectangle), so k_sort_tiles needs no gather.  Only the first
+// 32 bytes of the record (geometry, opacity, depth, radius) are read.
 // =====================================================================================================
 struct EmitParams {
-    int P, M, gx, gy, for_backward;
-    const float *shs, *colors_precomp, *campos;
-    float4* records;
-    uint8_t* clamped;
+    int P, gx, gy;
+    const float4* records;
     const uint32_t* ranks;
     const uint32_t* vis_list;
     const uint2* ranges;
@@ -522,112 +595,38 @@ struct EmitParams {
     const gsr_counters* counters;
 };
 
-template <int DEG, bool VEC, bool BULK, bool WIN, bool TIGHT, bool PACKED>
-__global__ void __launch_bounds__(PRE_THREADS, 8) k_color_emit(const EmitParams p) {
-    constexpr int DG = DEG < 0 ? 0 : DEG;
-    constexpr int NF = sh_nf(DG);
-    constexpr int STRIDE = sh_stride(DG, VEC, WIN);
-    __shared__ float campos[3];
-    // per warp: the SH staging rows of its 32 Gaussians, later reused as the emission's owner table (16 words per Gaussian)
-    constexpr int WSTAGE = (DEG < 0 || 32 * STRIDE < 16 * 32) ? 16 * 32 : 32 * STRIDE;
-    __shared__ __align__(16) float stage[(PRE_THREADS / 32) * WSTAGE];
-    __shared__ __align__(8) unsigned long long stage_bar[PRE_THREADS / 32];
+template <bool TIGHT, bool PACKED>
+__global__ void __launch_bounds__(PRE_THREADS, EMIT_MINB) k_emit(const EmitParams p) {
+    __shared__ __align__(16) float s_own[(PRE_THREADS / 32) * 16 * 32];  // per warp: the owner table, 16 words per Gaussian
 
     const uint32_t nvis = p.counters->num_visible;
     if (blockIdx.x * PRE_THREADS >= nvis) return;  // the grid is sized for P; blocks past the visible list leave at once
+    if (p.counters->overflow) return;              // set by k_tile_scan: the binning buffer is too small for this frame
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (BULK && lane == 0) {
-        mbar_init((uint32_t)__cvta_generic_to_shared(&stage_bar[warp]), 1u);
-        mbar_fence_init();
-    }
-    if (tid < 3) campos[tid] = p.campos[tid];
-    __syncthreads();
 
     const uint32_t k = blockIdx.x * PRE_THREADS + tid;
     const bool vis = k < nvis;
     const uint32_t idx = vis ? p.vis_list[k] : 0u;
-    // the whole 48-byte record (two 32-byte sectors whichever part is read): geometry, radius, and the mean k_project parked in the colour quad
-    float4 r0 = make_float4(0, 0, 0, 0), r1 = r0, r2 = r0;
+    float4 r0 = make_float4(0, 0, 0, 0), r1 = r0;
     int radius = 0;
     if (vis) {
         r0 = p.records[3 * (size_t)idx];
         r1 = p.records[3 * (size_t)idx + 1];
-        r2 = p.records[3 * (size_t)idx + 2];
         radius = __float_as_int(r1.w);
     }
     const float tau = footprint_tau(r1.y);  // = the value k_project used for its tight-tile decisions (same function of the same opacity)
 
-    // ---- colour ----
-    float rgb[3] = {0, 0, 0};
-    unsigned clamp_bits = 0;
-    float* wstage = stage + warp * WSTAGE;
-    if constexpr (DEG < 0) {
-        if (vis) {
-            rgb[0] = p.colors_precomp[3 * (size_t)idx];
-            rgb[1] = p.colors_precomp[3 * (size_t)idx + 1];
-            rgb[2] = p.colors_precomp[3 * (size_t)idx + 2];
-        }
-    } else {
-        const float3 mean = {r2.x, r2.y, r2.z};
-        const unsigned vismask = __ballot_sync(GSR_FULL, vis);
-        const size_t row_floats = (size_t)p.M * 3;
-        int win_off = 0;  // floats between the start of the staged window and the row's first coefficient (WIN only)
-        if (VEC && BULK) {
-            constexpr int NV = sh_nv(DG, WIN);
-            const uint32_t bar = (uint32_t)__cvta_generic_to_shared(&stage_bar[warp]);
-            if (vismask) {
-                if (lane == 0) mbar_arrive_expect_tx(bar, (uint32_t)__popc(vismask) * NV * 16u);
-                if (vis) {
-                    const float* src = p.shs + (size_t)idx * row_floats;
-                    if (WIN) {
-                        win_off = (int)(((uintptr_t)src & 15u) >> 2);
-                        src -= win_off;
-                    }
-                    bulk_g2s((uint32_t)__cvta_generic_to_shared(wstage + lane * STRIDE), src, NV * 16u, bar);
-                }
-                mbar_wait(bar, 0u);
-            }
-        } else if (VEC) {
-            constexpr int NV = (NF + 3) / 4;
-#pragma unroll
-            for (int it = 0; it < NV; it++) {
-                const int item = it * 32 + lane;
-                const int gl = item / NV, part = item - gl * NV;
-                const uint32_t gid = __shfl_sync(GSR_FULL, idx, gl);
-                if ((vismask >> gl) & 1u) cp_async16(wstage + gl * STRIDE + part * 4, p.shs + (size_t)gid * row_floats + part * 4);
-            }
-            cp_async_wait_all();
-        } else {
-#pragma unroll 4
-            for (int it = 0; it < NF; it++) {
-                const int item = it * 32 + lane;
-                const int gl = item / NF, part = item - gl * NF;
-                const uint32_t gid = __shfl_sync(GSR_FULL, idx, gl);
-                if ((vismask >> gl) & 1u) wstage[gl * STRIDE + part] = p.shs[(size_t)gid * row_floats + part];
-            }
-        }
-        __syncwarp();
-        if (vis) sh_eval<DG>(wstage + lane * STRIDE + win_off, mean, campos, rgb, clamp_bits);
-    }
-    if (vis) {
-        p.records[3 * (size_t)idx + 2] = make_float4(rgb[0], rgb[1], rgb[2], log2f(r1.y));  // .w: log2(opacity) for the default blend
-        if (p.for_backward) p.clamped[idx] = (uint8_t)clamp_bits;
-    }
-
-    // ---- emission ----
     // The (Gaussian, tile column) pairs of the warp's 32 Gaussians are FLATTENED into one work list and dealt to the lanes round
     // robin, so a lane whose Gaussian covers one tile does not idle while its neighbour walks a 3x3 rectangle: every owner parks
     // its rectangle, strip context and key words in shared memory, a warp scan of the per-Gaussian item counts gives each item
     // its owner (binary search over 32 prefix sums), and the item's lane evaluates the two strips of its column once and walks
     // the column's (at most 8) tiles.  Columns taller than 8 tiles (rectangles of > 8 tiles only) are split into chunks of 8 rows.
-    if (p.counters->overflow) return;  // set by k_tile_scan: the binning buffer is too small for this frame
     int x0 = 0, y0 = 0, x1 = 0, y1 = 0;
     if (vis) tile_rect(r0.x, r0.y, radius, p.gx, p.gy, x0, y0, x1, y1);
     const int w = x1 - x0, h = y1 - y0, cnt = w * h;
     const int cpc = (h + 7) >> 3;  // chunks per column
     const int n_items = w * cpc;
-    float* own = wstage;  // the SH staging area is free after sh_eval
-    __syncwarp();
+    float* own = s_own + warp * 16 * 32;
     {
         StripCtx sc = {};
         if (PACKED && cnt > 0) {
@@ -1018,7 +1017,7 @@ __device__ void sort_bucket_small(const unsigned long long* __restrict__ g, uint
 
 // ---- footprint ballot matrix ------------------------------------------------------------------------------------
 // After the sort every entry of the tile carries an 8-bit mask: which of the tile's eight 8x4-pixel warp footprints the splat
-// can touch (PACKED: the low byte of the key, computed by k_color_emit; otherwise the record is gathered and the mask computed
+// can touch (PACKED: the low byte of the key, computed by k_emit; otherwise the record is gathered and the mask computed
 // here).  The masks of 32 consecutive list entries are transposed by eight ballots into one ROW of the ballot matrix:
 // bal[row][f] = bit i set iff entry 32 row + i touches footprint f.  The blend warp that owns footprint f reads column f — one
 // word per 32 entries — and expands it into the positions of its survivors on the fly, so the blend has no per-entry cull
@@ -1223,19 +1222,19 @@ static int sh_bulk_mode() {  // GSR_SH_STAGING=cpasync selects the LDGSTS path, 
     }
     return mode;
 }
-template <int DEG, bool TIGHT, bool PACKED>
-static void launch_ce_v(bool vec, bool win, const EmitParams& ep, cudaStream_t st) {
-    const int grid = (ep.P + PRE_THREADS - 1) / PRE_THREADS;  // sized for P; blocks past the visible list exit at once
-    if (DEG < 0) k_color_emit<-1, false, false, false, TIGHT, PACKED><<<grid, PRE_THREADS, 0, st>>>(ep);
-    else if (win && sh_bulk_mode()) k_color_emit<DEG, true, true, true, TIGHT, PACKED><<<grid, PRE_THREADS, 0, st>>>(ep);
-    else if (vec && sh_bulk_mode()) k_color_emit<DEG, true, true, false, TIGHT, PACKED><<<grid, PRE_THREADS, 0, st>>>(ep);
-    else if (vec) k_color_emit<DEG, true, false, false, TIGHT, PACKED><<<grid, PRE_THREADS, 0, st>>>(ep);
-    else k_color_emit<DEG, false, false, false, TIGHT, PACKED><<<grid, PRE_THREADS, 0, st>>>(ep);
+template <int DEG, bool TIGHT>
+static void launch_project_v(bool vec, bool win, const PreParams& pp, cudaStream_t st) {
+    const int grid = (pp.P + PRE_THREADS - 1) / PRE_THREADS;
+    if constexpr (DEG < 0) k_project<-1, false, false, false, TIGHT><<<grid, PRE_THREADS, 0, st>>>(pp);
+    else if (win && sh_bulk_mode()) k_project<DEG, true, true, true, TIGHT><<<grid, PRE_THREADS, 0, st>>>(pp);
+    else if (vec && sh_bulk_mode()) k_project<DEG, true, true, false, TIGHT><<<grid, PRE_THREADS, 0, st>>>(pp);
+    else if (vec) k_project<DEG, true, false, false, TIGHT><<<grid, PRE_THREADS, 0, st>>>(pp);
+    else k_project<DEG, false, false, false, TIGHT><<<grid, PRE_THREADS, 0, st>>>(pp);
 }
 template <int DEG>
-static void launch_color_emit(bool vec, bool win, bool tight, bool packed, const EmitParams& ep, cudaStream_t st) {
-    if (tight) { if (packed) launch_ce_v<DEG, true, true>(vec, win, ep, st); else launch_ce_v<DEG, true, false>(vec, win, ep, st); }
-    else       { if (packed) launch_ce_v<DEG, false, true>(vec, win, ep, st); else launch_ce_v<DEG, false, false>(vec, win, ep, st); }
+static void launch_project(bool vec, bool win, bool tight, const PreParams& pp, cudaStream_t st) {
+    if (tight) launch_project_v<DEG, true>(vec, win, pp, st);
+    else launch_project_v<DEG, false>(vec, win, pp, st);
 }
 
 static void launch_blend(const BlendArgs& a, cudaStream_t st) { launch_blend_lists(a, st); }
@@ -1341,13 +1340,18 @@ int forward_impl(const gsr_frame* f, const gsr_workspace* ws, float* out_color, 
     uint2* ranges = (uint2*)(img + il.ranges);
     int rc = GSR_OK;
     if (!resume) {
-        static int minb = -1;  // GSR_PROJ_MINB=8|10|12: resident CTAs per SM the kernel is compiled for (experiment knob)
-        if (minb < 0) { const char* e = getenv("GSR_PROJ_MINB"); minb = e ? atoi(e) : 8; }
-        const int grid = (f->P + PRE_THREADS - 1) / PRE_THREADS;
-        if (pp.tight) k_project<8, true><<<grid, PRE_THREADS, 0, st>>>(pp);
-        else if (minb == 12) k_project<12, false><<<grid, PRE_THREADS, 0, st>>>(pp);
-        else if (minb == 10) k_project<10, false><<<grid, PRE_THREADS, 0, st>>>(pp);
-        else k_project<8, false><<<grid, PRE_THREADS, 0, st>>>(pp);
+        if (f->colors_precomp) launch_project<-1>(false, false, pp.tight, pp, st);
+        else {
+            const bool vec = (f->M % 4 == 0) && (((uintptr_t)f->shs & 15) == 0);
+            // 4-byte aligned rows (e.g. M = 25): the aligned window of sh_nv(D, true) float4 must fit inside every row
+            const bool win = !vec && (((uintptr_t)f->shs & 15) == 0) && (size_t)f->M * 12 >= (size_t)sh_nv(D, true) * 16;
+            switch (D) {
+                case 0: launch_project<0>(vec, win, pp.tight, pp, st); break;
+                case 1: launch_project<1>(vec, win, pp.tight, pp, st); break;
+                case 2: launch_project<2>(vec, win, pp.tight, pp, st); break;
+                default: launch_project<3>(vec, win, pp.tight, pp, st); break;
+            }
+        }
         prof_mark(1, st);
         if ((rc = check_launch("gsr_forward/project", debug, st))) return rc;
 
@@ -1363,24 +1367,16 @@ int forward_impl(const gsr_frame* f, const gsr_workspace* ws, float* out_color, 
     if (packed_ok < 0) { const char* e = getenv("GSR_PACKED_KEYS"); packed_ok = (e && e[0] == '0') ? 0 : 1; }
     const bool packed = packed_ok && f->P <= (1 << 24);
     EmitParams ep;
-    ep.P = f->P; ep.M = f->M; ep.gx = il.gx; ep.gy = il.gy; ep.for_backward = pp.for_backward;
-    ep.shs = f->shs; ep.colors_precomp = f->colors_precomp; ep.campos = f->campos;
-    ep.records = pp.records; ep.clamped = pp.clamped; ep.ranks = pp.ranks; ep.vis_list = pp.vis_list;
+    ep.P = f->P; ep.gx = il.gx; ep.gy = il.gy;
+    ep.records = pp.records; ep.ranks = pp.ranks; ep.vis_list = pp.vis_list;
     ep.ranges = ranges; ep.tile_fill = (uint32_t*)(img + il.tile_fill); ep.pairs = (uint2*)(bin + bl.pairs); ep.counters = counters;
-    if (f->colors_precomp) launch_color_emit<-1>(false, false, pp.tight, packed, ep, st);
-    else {
-        const bool vec = (f->M % 4 == 0) && (((uintptr_t)f->shs & 15) == 0);
-        // 4-byte aligned rows (e.g. M = 25): the aligned window of sh_nv(D, true) float4 must fit inside every row
-        const bool win = !vec && (((uintptr_t)f->shs & 15) == 0) && (size_t)f->M * 12 >= (size_t)sh_nv(D, true) * 16;
-        switch (D) {
-            case 0: launch_color_emit<0>(vec, win, pp.tight, packed, ep, st); break;
-            case 1: launch_color_emit<1>(vec, win, pp.tight, packed, ep, st); break;
-            case 2: launch_color_emit<2>(vec, win, pp.tight, packed, ep, st); break;
-            default: launch_color_emit<3>(vec, win, pp.tight, packed, ep, st); break;
-        }
+    {
+        const int grid = (f->P + PRE_THREADS - 1) / PRE_THREADS;  // sized for P; blocks past the visible list exit at once
+        if (pp.tight) { if (packed) k_emit<true, true><<<grid, PRE_THREADS, 0, st>>>(ep); else k_emit<true, false><<<grid, PRE_THREADS, 0, st>>>(ep); }
+        else          { if (packed) k_emit<false, true><<<grid, PRE_THREADS, 0, st>>>(ep); else k_emit<false, false><<<grid, PRE_THREADS, 0, st>>>(ep); }
     }
     prof_mark(3, st);
-    if ((rc = check_launch("gsr_forward/color_emit", debug, st))) return rc;
+    if ((rc = check_launch("gsr_forward/emit", debug, st))) return rc;
 
     const int keep_pairs = (flags & GSR_FLAG_SORTED_KEYS) ? 1 : 0;
     uint32_t* n_contrib = (flags & GSR_FLAG_FOR_BACKWARD) ? (uint32_t*)(img + il.n_contrib) : nullptr;

@@ -103,7 +103,7 @@ def main():
     ms = e0.elapsed_time(e1) / K
     res = {"tag": args.tag, "env": {k: os.environ.get(k) for k in ("GSR_BLEND", "GSR_BLEND_WARPS") if os.environ.get(k)},
            "exact": args.exact, "tight": args.tight, "streams": NS, "ms_per_frame": round(ms, 4), "fps": round(1000.0 / ms, 1),
-           "kernel_ms": {k: round(float(ms_k[i]), 4) for i, k in enumerate(["project", "tile_scan", "color_emit", "sort_tiles", "blend"])},
+           "kernel_ms": {k: round(float(ms_k[i]), 4) for i, k in enumerate(["project", "tile_scan", "emit", "sort_tiles", "blend"])},
            "avg_R": sum(s["num_rendered"] for s in st) / K, "avg_foot": sum(s["foot_total"] for s in st) / K,
            "avg_redos": sum(s["exact_redos"] for s in st) / K, "overflow": sum(s["overflow"] for s in st)}
     if args.backward:

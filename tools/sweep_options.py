@@ -115,7 +115,7 @@ def main():
                     ms_k, nfr = (C.c_float * 5)(), C.c_int(0)
                     _lib.check(_lib.lib.gsr_profile_end(ms_k, C.byref(nfr)), "profile_end")
                     if best is None or ms < best:
-                        kms = {k_: round(float(ms_k[i_]), 4) for i_, k_ in enumerate(["project", "tile_scan", "color_emit", "sort_tiles", "blend"])}
+                        kms = {k_: round(float(ms_k[i_]), 4) for i_, k_ in enumerate(["project", "tile_scan", "emit", "sort_tiles", "blend"])}
                 ovf = sum(t_.stats()["overflow"] for t_ in tk)
                 best = ms if best is None else min(best, ms)
             res = {"config": cname, "streams": NS, "kernel_ms": kms, "ms_per_frame": round(best, 4), "fps": round(1000.0 / best, 1), "bit_equal": same,
