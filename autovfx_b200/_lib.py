@@ -65,7 +65,8 @@ EXPORTS = ("gsr_abi_version", "gsr_last_error", "gsr_geom_bytes", "gsr_binning_b
            "gsr_forward", "gsr_backward", "gsr_mark_visible", "gsr_dist2_bytes", "gsr_dist2", "gsr_get_views",
            "gsr_profile_begin", "gsr_profile_begin_strided", "gsr_profile_end", "gsr_forward_multi", "gsr_axis_normals", "gsr_normal_maps",
            "gsr_pack_frame", "gsr_activate_gaussians", "gsr_set_option", "gsr_backward_multi", "gsr_activate_gaussians_backward",
-           "gsr_sugar_normals", "gsr_sugar_normals_backward", "gsr_sugar_colors", "gsr_sugar_colors_backward", "gsr_knn_bytes", "gsr_knn")
+           "gsr_sugar_normals", "gsr_sugar_normals_backward", "gsr_sugar_colors", "gsr_sugar_colors_backward", "gsr_knn_bytes", "gsr_knn",
+           "gsr_sugar_field_bytes", "gsr_sugar_field", "gsr_sugar_field_backward")
 
 
 def _load() -> C.CDLL:
@@ -86,7 +87,8 @@ def _load() -> C.CDLL:
     if lib.gsr_abi_version() != ABI_VERSION:
         raise ImportError("autovfx_b200: ABI mismatch, rebuild with `python -m autovfx_b200.build --force`")
     lib.gsr_last_error.restype = C.c_char_p
-    for n in ("gsr_geom_bytes", "gsr_image_bytes", "gsr_binning_bytes", "gsr_binning_capacity", "gsr_dist2_bytes", "gsr_knn_bytes"):
+    for n in ("gsr_geom_bytes", "gsr_image_bytes", "gsr_binning_bytes", "gsr_binning_capacity", "gsr_dist2_bytes", "gsr_knn_bytes",
+              "gsr_sugar_field_bytes"):
         getattr(lib, n).restype = C.c_size_t
     lib.gsr_geom_bytes.argtypes = [C.c_int32]
     lib.gsr_image_bytes.argtypes = [C.c_int32, C.c_int32]
@@ -132,6 +134,12 @@ def _load() -> C.CDLL:
     lib.gsr_knn_bytes.argtypes = [C.c_int32] * 3
     lib.gsr_knn.restype = C.c_int
     lib.gsr_knn.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 5 + [C.c_size_t, C.c_void_p]
+    lib.gsr_sugar_field_bytes.argtypes = [C.c_int32]
+    lib.gsr_sugar_field.restype = C.c_int
+    lib.gsr_sugar_field.argtypes = [C.c_int32] * 4 + [C.c_void_p] * 7 + [C.c_float] * 3 + [C.c_void_p] * 5 + [C.c_size_t, C.c_void_p]
+    lib.gsr_sugar_field_backward.restype = C.c_int
+    lib.gsr_sugar_field_backward.argtypes = ([C.c_int32] * 4 + [C.c_void_p] * 7 + [C.c_float] * 3 + [C.c_void_p] * 10 +
+                                             [C.c_size_t, C.c_void_p])
     lib.gsr_get_views.restype = C.c_int
     lib.gsr_get_views.argtypes = [C.POINTER(gsr_workspace), C.c_int32, C.c_int32, C.c_int32, C.POINTER(gsr_views)]
     lib.gsr_profile_begin.restype = C.c_int

@@ -44,6 +44,16 @@ size_t dist2_bytes(int P);
 int knn_impl(int P1, int P2, int K, const float* queries, const float* points, float* out_d, int64_t* out_i, void* ws, size_t ws_bytes,
              cudaStream_t st);
 size_t knn_bytes(int P1, int P2);
+size_t sugar_field_bytes(int P);
+int sugar_field_impl(int N, int K, int P, int R, const float* x, const int64_t* rows, const int64_t* row_idx, const float* points,
+                     const float* scaling, const float* quaternions, const float* strengths, float density_factor,
+                     float opacity_min_clamp, float sdf_offset, float* out_density, float* out_opac, float* out_beta, float* out_sdf,
+                     void* ws, size_t ws_bytes, cudaStream_t st);
+int sugar_field_backward_impl(int N, int K, int P, int R, const float* x, const int64_t* rows, const int64_t* row_idx,
+                              const float* points, const float* scaling, const float* quaternions, const float* strengths,
+                              float density_factor, float opacity_min_clamp, float sdf_offset, const float* g_density, const float* g_opac,
+                              const float* g_beta, const float* g_sdf, float* dx, float* d_points, float* d_scaling, float* d_quaternions,
+                              float* d_strengths, void* ws, size_t ws_bytes, cudaStream_t st);
 int profile_begin(int max_frames, int stride);
 int set_option(const char* name, int value);
 int profile_end(float* ms, int* frames);
@@ -184,6 +194,27 @@ int gsr_knn(int32_t P1, int32_t P2, int32_t K, const float* queries, const float
             void* workspace, size_t workspace_bytes, void* stream) {
     NvtxRange nvtx_("gsr_knn");
     return gsr::knn_impl(P1, P2, K, queries, points, out_dists, out_idx, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+size_t gsr_sugar_field_bytes(int32_t P) { return gsr::sugar_field_bytes(P); }
+int gsr_sugar_field(int32_t N, int32_t K, int32_t P, int32_t R, const float* x, const int64_t* rows, const int64_t* row_idx,
+                    const float* points, const float* scaling, const float* quaternions, const float* strengths, float density_factor,
+                    float opacity_min_clamp, float sdf_offset, float* out_density, float* out_opacities, float* out_beta, float* out_sdf,
+                    void* workspace, size_t workspace_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_sugar_field");
+    return gsr::sugar_field_impl(N, K, P, R, x, rows, row_idx, points, scaling, quaternions, strengths, density_factor, opacity_min_clamp,
+                                 sdf_offset, out_density, out_opacities, out_beta, out_sdf, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int gsr_sugar_field_backward(int32_t N, int32_t K, int32_t P, int32_t R, const float* x, const int64_t* rows, const int64_t* row_idx,
+                             const float* points, const float* scaling, const float* quaternions, const float* strengths,
+                             float density_factor, float opacity_min_clamp, float sdf_offset, const float* dL_ddensity,
+                             const float* dL_dopacities, const float* dL_dbeta, const float* dL_dsdf, float* dL_dx, float* dL_dpoints,
+                             float* dL_dscaling, float* dL_dquaternions, float* dL_dstrengths, void* workspace, size_t workspace_bytes,
+                             void* stream) {
+    NvtxRange nvtx_("gsr_sugar_field_backward");
+    return gsr::sugar_field_backward_impl(N, K, P, R, x, rows, row_idx, points, scaling, quaternions, strengths, density_factor,
+                                          opacity_min_clamp, sdf_offset, dL_ddensity, dL_dopacities, dL_dbeta, dL_dsdf, dL_dx, dL_dpoints,
+                                          dL_dscaling, dL_dquaternions, dL_dstrengths, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 int gsr_profile_begin(int max_frames) { return gsr::profile_begin(max_frames, 1); }

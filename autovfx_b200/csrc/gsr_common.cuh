@@ -402,6 +402,38 @@ __device__ __forceinline__ SugarAxisPick sugar_axis_pick(float s0, float s1, flo
     return p;
 }
 
+// The whole of pytorch3d's quaternion_to_matrix(q) for a raw q = (r, i, j, k), row-major R[3 * row + col], with sugar_axis_pick's
+// roundings; t = two_s = 2 / |q|^2 as torch evaluates it.
+__device__ __forceinline__ void quat_to_matrix_rn(float r, float i, float j, float k, float (&R)[9], float& t) {
+    const float ss = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(r, r), __fmul_rn(i, i)), __fmul_rn(j, j)), __fmul_rn(k, k));
+    t = __fmul_rn(__frcp_rn(ss), 2.0f);
+    R[0] = __fsub_rn(1.0f, __fmul_rn(t, __fadd_rn(__fmul_rn(j, j), __fmul_rn(k, k))));
+    R[1] = __fmul_rn(t, __fsub_rn(__fmul_rn(i, j), __fmul_rn(k, r)));
+    R[2] = __fmul_rn(t, __fadd_rn(__fmul_rn(i, k), __fmul_rn(j, r)));
+    R[3] = __fmul_rn(t, __fadd_rn(__fmul_rn(i, j), __fmul_rn(k, r)));
+    R[4] = __fsub_rn(1.0f, __fmul_rn(t, __fadd_rn(__fmul_rn(i, i), __fmul_rn(k, k))));
+    R[5] = __fmul_rn(t, __fsub_rn(__fmul_rn(j, k), __fmul_rn(i, r)));
+    R[6] = __fmul_rn(t, __fsub_rn(__fmul_rn(i, k), __fmul_rn(j, r)));
+    R[7] = __fmul_rn(t, __fadd_rn(__fmul_rn(j, k), __fmul_rn(i, r)));
+    R[8] = __fsub_rn(1.0f, __fmul_rn(t, __fadd_rn(__fmul_rn(i, i), __fmul_rn(j, j))));
+}
+// Its vector-Jacobian product for dL/dR = G (row-major): with R = base + t u(q) and dt/dq = -t^2 q,
+//   dL/dq = t * sum_ab G_ab du_ab/dq - t^2 * (sum_ab G_ab u_ab) * q.
+// k_sugar_normals_backward is the special case of one non-zero column.
+__device__ __forceinline__ void quat_to_matrix_vjp(float r, float i, float j, float k, float t, const float (&G)[9], float (&dq)[4]) {
+    const float s01 = G[1] + G[3], s02 = G[2] + G[6], s12 = G[5] + G[7];  // symmetric parts
+    const float a10 = G[3] - G[1], a02 = G[2] - G[6], a21 = G[7] - G[5];  // antisymmetric parts
+    const float gr = k * a10 + j * a02 + i * a21;
+    const float gi = j * s01 + k * s02 + r * a21 - 2.0f * i * (G[4] + G[8]);
+    const float gj = i * s01 + k * s12 + r * a02 - 2.0f * j * (G[0] + G[8]);
+    const float gk = i * s02 + j * s12 + r * a10 - 2.0f * k * (G[0] + G[4]);
+    const float su = -G[0] * (j * j + k * k) - G[4] * (i * i + k * k) - G[8] * (i * i + j * j) + G[1] * (i * j - k * r) +
+                     G[2] * (i * k + j * r) + G[3] * (i * j + k * r) + G[5] * (j * k - i * r) + G[6] * (i * k - j * r) +
+                     G[7] * (j * k + i * r);
+    const float tts = t * t * su;
+    dq[0] = t * gr - tts * r; dq[1] = t * gi - tts * i; dq[2] = t * gj - tts * j; dq[3] = t * gk - tts * k;
+}
+
 // SH basis constants (auxiliary.h:22-39; degree 4: SuGaR's sugar_utils/spherical_harmonics.py:23-33)
 constexpr float SH_C0 = 0.28209479177387814f;
 constexpr float SH_C1 = 0.4886025119029199f;

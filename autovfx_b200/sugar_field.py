@@ -1,0 +1,222 @@
+"""SuGaR's SDF-regularisation field in CUDA: drop-ins for ``SuGaR.get_field_values`` and ``SuGaR.compute_density``
+("SS/" = sugar/sugar_scene/sugar_model.py:1118-1187 and :1216-1239, with get_covariance :602-608 and get_beta 'average'
+:1063-1066), forward and backward through ``gsr_sugar_field`` / ``gsr_sugar_field_backward``.
+
+Opt in on the class (both take the methods' exact signatures and return what they return)::
+
+    from autovfx_b200.sugar_field import get_field_values, compute_density
+    SuGaR.get_field_values = get_field_values
+    SuGaR.compute_density = compute_density
+
+The model is read through its getters (``points``, ``scaling``, ``quaternions``, ``strengths``, ``knn_idx``, ``beta_mode``), so
+autograd carries the gradients of x and of the getters' outputs back to the raw parameters.  No [N,K,3,3] tensor is built: the
+kernels gather one 64-byte record per (sample, neighbour) pair and recompute everything in the backward.
+"""
+from __future__ import annotations
+
+import numpy as np
+import torch
+
+from . import _lib
+
+__all__ = ["get_field_values", "compute_density", "FIELD_MAX_K"]
+
+FIELD_MAX_K = 32
+
+
+def _lib_handle():
+    return _lib.lib
+
+
+def _ptr(t):
+    return None if t is None else t.data_ptr()
+
+
+def _check_tensor(who, name, t, shape, dtype):
+    """shape: a tuple of ints or None (any size) per dimension."""
+    if not isinstance(t, torch.Tensor):
+        raise ValueError("%s: %s must be a torch.Tensor, got %s" % (who, name, type(t).__name__))
+    if t.dtype != dtype:
+        raise ValueError("%s: %s must be %s, got %s" % (who, name, dtype, t.dtype))
+    if t.dim() != len(shape) or any(s is not None and s != d for s, d in zip(shape, t.shape)):
+        want = "[" + ", ".join("*" if s is None else str(s) for s in shape) + "]"
+        raise ValueError("%s: %s must have shape %s, got %s" % (who, name, want, tuple(t.shape)))
+
+
+def _model_tensors(who, self):
+    points, scaling, quaternions, strengths = self.points, self.scaling, self.quaternions, self.strengths
+    _check_tensor(who, "self.points", points, (None, 3), torch.float32)
+    P = points.shape[0]
+    _check_tensor(who, "self.scaling", scaling, (P, 3), torch.float32)
+    _check_tensor(who, "self.quaternions", quaternions, (P, 4), torch.float32)
+    if not isinstance(strengths, torch.Tensor) or strengths.shape not in ((P, 1), (P,)):
+        raise ValueError("%s: self.strengths must have shape [%d, 1], got %s" % (who, P, getattr(strengths, "shape", None)))
+    _check_tensor(who, "self.strengths", strengths, tuple(strengths.shape), torch.float32)
+    return points, scaling, quaternions, strengths.reshape(P)
+
+
+def _require_cuda(who, *ts):
+    dev = ts[0].device
+    for t in ts:
+        if t is not None and not t.is_cuda:
+            raise RuntimeError("autovfx_b200.%s: every tensor must be a CUDA tensor (there is no CPU path)" % who)
+    for t in ts:
+        if t is not None and t.device != dev:
+            raise ValueError("%s: tensors on %s and %s" % (who, dev, t.device))
+
+
+class _Cfg:
+    __slots__ = ("N", "K", "P", "R", "df", "omc", "offset", "opac", "beta", "sdf")
+
+    def __init__(self, N, K, P, R, df, omc, offset, opac, beta, sdf):
+        self.N, self.K, self.P, self.R = N, K, P, R
+        self.df, self.omc, self.offset = df, omc, offset
+        self.opac, self.beta, self.sdf = opac, beta, sdf
+
+
+def _forward(cfg, x, rows, row_idx, points, scaling, quaternions, strengths):
+    dev = x.device
+    N, K = cfg.N, cfg.K
+    density = torch.empty(N, dtype=torch.float32, device=dev)
+    opac = torch.empty((N, K), dtype=torch.float32, device=dev) if cfg.opac else None
+    beta = torch.empty(N, dtype=torch.float32, device=dev) if cfg.beta else None
+    sdf = torch.empty(N, dtype=torch.float32, device=dev) if cfg.sdf else None
+    if N > 0:
+        L = _lib_handle()
+        nbytes = L.gsr_sugar_field_bytes(cfg.P)
+        ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
+        rc = L.gsr_sugar_field(N, K, cfg.P, cfg.R, x.data_ptr(), rows.data_ptr(), _ptr(row_idx), points.data_ptr(), scaling.data_ptr(),
+                               quaternions.data_ptr(), strengths.data_ptr(), cfg.df, cfg.omc, cfg.offset, density.data_ptr(),
+                               _ptr(opac), _ptr(beta), _ptr(sdf), ws.data_ptr(), nbytes, _lib.stream_ptr(dev))
+        _lib.check(rc, "gsr_sugar_field")
+    return density, opac, beta, sdf
+
+
+class _SugarField(torch.autograd.Function):
+    """Outputs: density, then neighbour opacities, beta and sdf when the configuration asks for them."""
+
+    @staticmethod
+    def forward(ctx, x, points, scaling, quaternions, strengths, rows, row_idx, cfg):
+        ctx.set_materialize_grads(False)
+        ctx.cfg = cfg
+        ctx.save_for_backward(x, points, scaling, quaternions, strengths, rows, row_idx)
+        density, opac, beta, sdf = _forward(cfg, x, rows, row_idx, points, scaling, quaternions, strengths)
+        return tuple(t for t in (density, opac, beta, sdf) if t is not None)
+
+    @staticmethod
+    def backward(ctx, *grads):
+        cfg = ctx.cfg
+        x, points, scaling, quaternions, strengths, rows, row_idx = ctx.saved_tensors
+        it = iter(grads)
+        g_density = next(it)
+        g_opac = next(it) if cfg.opac else None
+        g_beta = next(it) if cfg.beta else None
+        g_sdf = next(it) if cfg.sdf else None
+        g = [None if t is None else t.contiguous() for t in (g_density, g_opac, g_beta, g_sdf)]
+        dev = x.device
+        P, N = cfg.P, cfg.N
+        dx = torch.zeros_like(x) if ctx.needs_input_grad[0] else None
+        d_points = torch.zeros_like(points)
+        d_scaling = torch.zeros_like(scaling)
+        d_quaternions = torch.zeros_like(quaternions)
+        d_strengths = torch.zeros_like(strengths)
+        if N > 0 and any(t is not None for t in g):
+            L = _lib_handle()
+            nbytes = 2 * L.gsr_sugar_field_bytes(P)
+            ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
+            rc = L.gsr_sugar_field_backward(N, cfg.K, P, cfg.R, x.data_ptr(), rows.data_ptr(), _ptr(row_idx), points.data_ptr(),
+                                            scaling.data_ptr(), quaternions.data_ptr(), strengths.data_ptr(), cfg.df, cfg.omc,
+                                            cfg.offset, *[_ptr(t) for t in g], _ptr(dx), d_points.data_ptr(), d_scaling.data_ptr(),
+                                            d_quaternions.data_ptr(), d_strengths.data_ptr(), ws.data_ptr(), nbytes,
+                                            _lib.stream_ptr(dev))
+            _lib.check(rc, "gsr_sugar_field_backward")
+        need = ctx.needs_input_grad
+        return (dx, d_points if need[1] else None, d_scaling if need[2] else None, d_quaternions if need[3] else None,
+                d_strengths if need[4] else None, None, None, None)
+
+
+def _field(who, self, x, rows, row_idx, density_factor, opacity_min_clamp, offset, opac, beta, sdf):
+    """Validated inputs -> (density, opac or None, beta or None, sdf or None)."""
+    points, scaling, quaternions, strengths = _model_tensors(who, self)
+    _check_tensor(who, "x", x, (None, 3), torch.float32)
+    N, P = x.shape[0], points.shape[0]
+    _check_tensor(who, "closest_gaussians_idx" if row_idx is None else "self.knn_idx", rows, (None, None), torch.int64)
+    R, K = rows.shape
+    if not 1 <= K <= FIELD_MAX_K:
+        raise ValueError("%s: K = %d neighbours per sample must be in 1..%d" % (who, K, FIELD_MAX_K))
+    if row_idx is None and R != N:
+        raise ValueError("%s: closest_gaussians_idx has %d rows for %d samples" % (who, R, N))
+    for name, v in (("density_factor", density_factor), ("opacity_min_clamp", opacity_min_clamp)):
+        if isinstance(v, bool) or not isinstance(v, (int, float)):
+            raise ValueError("%s: %s must be a Python number, got %r" % (who, name, v))
+    _require_cuda(who, x, rows, row_idx, points, scaling, quaternions, strengths)
+    cfg = _Cfg(N, K, P, R, float(density_factor), float(opacity_min_clamp), offset, opac, beta, sdf)
+    rows = rows.contiguous()
+    row_idx = None if row_idx is None else row_idx.contiguous()
+    ins = [t.contiguous() for t in (x, points, scaling, quaternions, strengths)]
+    with torch.cuda.device(x.device):
+        if torch.is_grad_enabled() and any(t.requires_grad for t in ins):
+            outs = iter(_SugarField.apply(*ins, rows, row_idx, cfg))
+            return tuple(next(outs) if want else None for want in (True, opac, beta, sdf))
+        return _forward(cfg, ins[0], rows, row_idx, *ins[1:])
+
+
+def get_field_values(self, x, gaussian_idx=None, closest_gaussians_idx=None, gaussian_strengths=None, gaussian_centers=None,
+                     gaussian_inv_scaled_rotation=None, return_sdf=True, density_threshold=1., density_factor=1.,
+                     return_sdf_grad=False, sdf_grad_max_value=10., opacity_min_clamp=1e-16, return_closest_gaussian_opacities=False,
+                     return_beta=False):
+    """SuGaR.get_field_values (SS/:1118-1187) in CUDA.  Returns SuGaR's dict: 'density' (the sum before the d >= 1
+    normalisation), then 'closest_gaussian_opacities' [N,K], 'beta' and 'sdf' as requested.  The neighbours are
+    closest_gaussians_idx [N,K] or, when it is None, self.knn_idx[gaussian_idx] (read in place, never gathered).
+
+    Raises ValueError, naming the argument, for what no SuGaR caller uses: return_sdf_grad=True, the gaussian_strengths /
+    gaussian_centers / gaussian_inv_scaled_rotation overrides, a beta_mode other than 'average' when beta or the sdf is asked for,
+    both indices None, bad shapes or dtypes, K outside 1..32.  CPU tensors raise RuntimeError (there is no CPU path)."""
+    who = "get_field_values"
+    if return_sdf_grad:
+        raise ValueError("get_field_values: return_sdf_grad=True is not supported (no SuGaR trainer asks for sdf_grad)")
+    for name, v in (("gaussian_strengths", gaussian_strengths), ("gaussian_centers", gaussian_centers),
+                    ("gaussian_inv_scaled_rotation", gaussian_inv_scaled_rotation)):
+        if v is not None:
+            raise ValueError("get_field_values: the %s override is not supported (pass None: the model's getters are used)" % name)
+    want_beta = bool(return_sdf or return_beta)
+    if want_beta:
+        mode = self.beta_mode
+        if mode in ("learnable", "weighted_average"):
+            raise ValueError("get_field_values: beta_mode = %r is not supported (only 'average')" % (mode,))
+        if mode != "average":
+            raise ValueError("Unknown beta_mode.")
+    if closest_gaussians_idx is not None:
+        rows, row_idx = closest_gaussians_idx, None
+    elif gaussian_idx is not None:
+        rows = self.knn_idx
+        _check_tensor(who, "self.knn_idx", rows, (None, None), torch.int64)
+        _check_tensor(who, "gaussian_idx", gaussian_idx, (None,), torch.int64)
+        row_idx = gaussian_idx
+        if isinstance(x, torch.Tensor) and x.dim() == 2 and gaussian_idx.shape[0] != x.shape[0]:
+            raise ValueError("get_field_values: gaussian_idx has %d entries for %d samples" % (gaussian_idx.shape[0], x.shape[0]))
+    else:
+        raise ValueError("get_field_values: gaussian_idx and closest_gaussians_idx are both None")
+    offset = float(np.float32(np.sqrt(-2. * np.log(min(density_threshold, 1.))))) if return_sdf else 0.0
+    density, opac, beta, sdf = _field(who, self, x, rows, row_idx, density_factor, opacity_min_clamp, offset,
+                                      bool(return_closest_gaussian_opacities), want_beta, bool(return_sdf))
+    fields = {"density": density}
+    if return_closest_gaussian_opacities:
+        fields["closest_gaussian_opacities"] = opac
+    if return_beta:
+        fields["beta"] = beta
+    if return_sdf:
+        fields["sdf"] = sdf
+    return fields
+
+
+def compute_density(self, x, closest_gaussians_idx=None, density_factor=1., return_closest_gaussian_opacities=False):
+    """SuGaR.compute_density (SS/:1216-1239) in CUDA: densities [N] (and the neighbour opacities [N,K]).  Without indices it
+    calls self.get_gaussians_closest_to_samples(x), so the model's knn_points binding applies."""
+    if closest_gaussians_idx is None:
+        closest_gaussians_idx = self.get_gaussians_closest_to_samples(x)
+    density, opac, _, _ = _field("compute_density", self, x, closest_gaussians_idx, None, density_factor, 1e-16, 0.0,
+                                 bool(return_closest_gaussian_opacities), False, False)
+    if return_closest_gaussian_opacities:
+        return density, opac
+    return density

@@ -11,6 +11,8 @@
  *   gsr_mark_visible  replaces  _C.mark_visible                  DGR/rasterize_points.cu:211-230
  *   gsr_dist2         replaces  simple_knn._C.distCUDA2          KNN/spatial.cu:15-26 (SimpleKNN::knn, KNN/simple_knn.cu:185-220)
  *   gsr_knn           replaces  pytorch3d.ops.knn_points in SuGaR  sugar_scene/sugar_model.py:47, :233, :899, :914, :1213 (N = 1, D = 3)
+ *   gsr_sugar_field   replaces  SuGaR.get_field_values / compute_density  sugar_scene/sugar_model.py:1118-1187, :1216-1239
+ *                               (get_covariance :602-608, get_beta 'average' :1063-1066); gsr_sugar_field_backward their autograd
  *
  * and, for the render() wrapper around the two rasterizer passes ("GR/" = sugar/gaussian_splatting/gaussian_renderer/__init__.py):
  *
@@ -292,6 +294,37 @@ int gsr_dist2(int32_t P, const float* points, float* mean_dists, void* workspace
 size_t gsr_knn_bytes(int32_t P1, int32_t P2, int32_t K);
 int gsr_knn(int32_t P1, int32_t P2, int32_t K, const float* queries, const float* points, float* out_dists, int64_t* out_idx,
             void* workspace, size_t workspace_bytes, void* stream);
+
+/* SuGaR's SDF-regularisation field (SuGaR.get_field_values with beta_mode 'average', SuGaR.compute_density) at N samples x [N,3]
+ * over K neighbours each (1 <= K <= 32) among P Gaussians given by SuGaR's getters: points [P,3], scaling [P,3], quaternions [P,4]
+ * (as the getter returns them; quaternion_to_matrix divides by |q|^2), strengths [P].  Sample n uses the Gaussians
+ * rows[row_idx[n], 0..K-1] of the int64 table rows [R,K] (row_idx NULL: rows[n], R == N).  Per pair, with
+ * A = quaternion_to_matrix(q) * (1 / clamp(s, 1e-8)) column-wise and w = A^T (x - centre):
+ *   out_opacities [N,K] = (density_factor * strength) * exp(-0.5 * clamp((w0^2 + w1^2) + w2^2, 0, 1e8))
+ *   out_density   [N]   = the sum over the K pairs
+ *   out_beta      [N]   = the mean over the K pairs of the Gaussian's min scale
+ *   out_sdf       [N]   = beta * (sqrt(-2 log(clamp(d_hat, opacity_min_clamp))) - sdf_offset), d_hat = d / (d + 1e-12) where
+ *                         d >= 1, else d; sdf_offset = sqrt(-2 log(min(density_threshold, 1))) as float
+ * Any output may be NULL (not requested).  N = 0 is a no-op.  Negative sizes, K outside 1..32, row_idx NULL with R != N, or a
+ * missing input when N > 0 are GSR_ERR_INVALID; `workspace` (16-byte aligned) needs gsr_sugar_field_bytes(P) bytes for the
+ * forward, twice that for the backward, else GSR_ERR_WORKSPACE.  A row or Gaussian index outside its array is never read: the
+ * sample's outputs are NaN. */
+size_t gsr_sugar_field_bytes(int32_t P);
+int gsr_sugar_field(int32_t N, int32_t K, int32_t P, int32_t R, const float* x, const int64_t* rows, const int64_t* row_idx,
+                    const float* points, const float* scaling, const float* quaternions, const float* strengths, float density_factor,
+                    float opacity_min_clamp, float sdf_offset, float* out_density, float* out_opacities, float* out_beta, float* out_sdf,
+                    void* workspace, size_t workspace_bytes, void* stream);
+
+/* Backward of gsr_sugar_field (same sizes, inputs and constants; it recomputes the forward): the gradients of the four outputs in
+ * (any may be NULL; dL_dsdf and dL_dbeta need no forward output), torch's backward formulas out: dL_dx [N,3] (may be NULL) and
+ * dL_dpoints [P,3], dL_dscaling [P,3], dL_dquaternions [P,4], dL_dstrengths [P] (required, written in full).  Where torch's
+ * gradient is not finite (d >= 1 with an sdf gradient: sqrt'(0)), this one is not either. */
+int gsr_sugar_field_backward(int32_t N, int32_t K, int32_t P, int32_t R, const float* x, const int64_t* rows, const int64_t* row_idx,
+                             const float* points, const float* scaling, const float* quaternions, const float* strengths,
+                             float density_factor, float opacity_min_clamp, float sdf_offset, const float* dL_ddensity,
+                             const float* dL_dopacities, const float* dL_dbeta, const float* dL_dsdf, float* dL_dx, float* dL_dpoints,
+                             float* dL_dscaling, float* dL_dquaternions, float* dL_dstrengths, void* workspace, size_t workspace_bytes,
+                             void* stream);
 
 /* Device pointers into the workspaces of the last layout (P, capacity, W, H) — for parity tests that
  * compare per-stage buffers with the reference (SURVEY §4).  Pure pointer arithmetic, no CUDA calls. */
