@@ -54,6 +54,14 @@ int sugar_field_backward_impl(int N, int K, int P, int R, const float* x, const 
                               float density_factor, float opacity_min_clamp, float sdf_offset, const float* g_density, const float* g_opac,
                               const float* g_beta, const float* g_sdf, float* dx, float* d_points, float* d_scaling, float* d_quaternions,
                               float* d_strengths, void* ws, size_t ws_bytes, cudaStream_t st);
+size_t sugar_sdf_normal_bytes(int P);
+int sugar_sdf_normal_impl(int N, int K, int P, const float* x, const int64_t* gidx, const int64_t* knn, const float* points,
+                          const float* scaling, const float* quaternions, const float* opac, float* out_loss, float* out_est, void* ws,
+                          size_t ws_bytes, cudaStream_t st);
+int sugar_sdf_normal_backward_impl(int N, int K, int P, const float* x, const int64_t* gidx, const int64_t* knn, const float* points,
+                                   const float* scaling, const float* quaternions, const float* opac, const float* g_loss,
+                                   const float* g_est, float* dx, float* d_points, float* d_quaternions, void* ws, size_t ws_bytes,
+                                   cudaStream_t st);
 int profile_begin(int max_frames, int stride);
 int set_option(const char* name, int value);
 int profile_end(float* ms, int* frames);
@@ -215,6 +223,23 @@ int gsr_sugar_field_backward(int32_t N, int32_t K, int32_t P, int32_t R, const f
     return gsr::sugar_field_backward_impl(N, K, P, R, x, rows, row_idx, points, scaling, quaternions, strengths, density_factor,
                                           opacity_min_clamp, sdf_offset, dL_ddensity, dL_dopacities, dL_dbeta, dL_dsdf, dL_dx, dL_dpoints,
                                           dL_dscaling, dL_dquaternions, dL_dstrengths, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+size_t gsr_sugar_sdf_normal_bytes(int32_t P) { return gsr::sugar_sdf_normal_bytes(P); }
+int gsr_sugar_sdf_normal(int32_t N, int32_t K, int32_t P, const float* x, const int64_t* gidx, const int64_t* knn_idx,
+                         const float* points, const float* scaling, const float* quaternions, const float* opacities, float* out_loss,
+                         float* out_estimate, void* workspace, size_t workspace_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_sugar_sdf_normal");
+    return gsr::sugar_sdf_normal_impl(N, K, P, x, gidx, knn_idx, points, scaling, quaternions, opacities, out_loss, out_estimate,
+                                      workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int gsr_sugar_sdf_normal_backward(int32_t N, int32_t K, int32_t P, const float* x, const int64_t* gidx, const int64_t* knn_idx,
+                                  const float* points, const float* scaling, const float* quaternions, const float* opacities,
+                                  const float* dL_dloss, const float* dL_destimate, float* dL_dx, float* dL_dpoints,
+                                  float* dL_dquaternions, void* workspace, size_t workspace_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_sugar_sdf_normal_backward");
+    return gsr::sugar_sdf_normal_backward_impl(N, K, P, x, gidx, knn_idx, points, scaling, quaternions, opacities, dL_dloss, dL_destimate,
+                                               dL_dx, dL_dpoints, dL_dquaternions, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 int gsr_profile_begin(int max_frames) { return gsr::profile_begin(max_frames, 1); }

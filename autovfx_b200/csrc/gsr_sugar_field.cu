@@ -323,4 +323,289 @@ int sugar_field_backward_impl(int N, int K, int P, int R, const float* x, const 
     return check_launch("gsr_sugar_field_backward", false, st);
 }
 
+// ================================================================================================================================
+// The better-normal regulariser and the projection estimate of the coarse trainers ("CD/" = sugar/sugar_trainers/coarse_density.py
+// :704-707 and :756-780; coarse_sdf.py :735-759 is the same code), over the same samples and knn_idx rows as the field.  n_g is
+// column k_g of quaternion_to_matrix(q_g), k_g the lowest index of min(s_g) (get_normals -> get_smallest_axis, SS/:801-839).
+//
+//   k_normal_prepare  one thread per Gaussian: a 32-byte record {p.xyz, c = clamp(min s, 1e-6)^2 | n.xyz, 0}, two aligned
+//                     16-byte loads per pair
+//   k_normal<W>       one segment of W = pow2 >= K lanes per sample, lane = neighbour j of knn_idx[i], i = sdf_gaussian_idx[n]:
+//                     sigma_j = sign(n_j . n_i), w_j = (o_nj |(x - p_j) . sigma_j n_j|) / c_j, w_hat = w / clamp(sum w, 1e-6),
+//                     r = n_i - sum_j w_hat_j sigma_j n_j, loss = (r0^2 + r1^2) + r2^2; and the estimate (x - p_i) . n_i
+//   k_normal_backward<W>  recomputes the forward; dL/dx per sample without atomics, the normal (and, for the estimate, centre)
+//                     gradients of every pair into a per-Gaussian 32-byte scratch with 16-byte RED.ADDs.  sigma, the weights,
+//                     their sum, o and c are detached, as the trainer (sdf_better_normal_gradient_through_normal_only) has them
+//   k_normal_chain    one thread per Gaussian: the normal gradient -> dL/dquaternions through column k_g of quaternion_to_matrix;
+//                     dL/dpoints
+//
+// Dots are pinned as (a0 b0 + a1 b1) + a2 b2 and the K-sums are seg_sum's fixed butterfly; every other op is one IEEE rounding.
+__global__ void __launch_bounds__(256) k_normal_prepare(int P, const float* __restrict__ points, const float* __restrict__ scaling,
+                                                        const float* __restrict__ quaternions, float4* __restrict__ rec) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= P) return;
+    const size_t p3 = 3 * (size_t)p, p4 = 4 * (size_t)p;
+    float R[9], t;
+    quat_to_matrix_rn(quaternions[p4], quaternions[p4 + 1], quaternions[p4 + 2], quaternions[p4 + 3], R, t);
+    int km = 0;
+    float sm = scaling[p3];
+    if (scaling[p3 + 1] < sm) { sm = scaling[p3 + 1]; km = 1; }
+    if (scaling[p3 + 2] < sm) { sm = scaling[p3 + 2]; km = 2; }
+    const float cm = sm < 1e-6f ? 1e-6f : sm;  // clamp(min=1e-6), NaN passes
+    rec[2 * (size_t)p] = make_float4(points[p3], points[p3 + 1], points[p3 + 2], __fmul_rn(cm, cm));
+    rec[2 * (size_t)p + 1] = make_float4(R[km], R[3 + km], R[6 + km], 0.0f);
+}
+
+struct NormalIn {
+    int N, K, P;
+    const float* x;          // [N,3] sdf_samples
+    const int64_t* gidx;     // [N]   sdf_gaussian_idx
+    const int64_t* knn;      // [P,K] knn_idx (loss only)
+    const float* opac;       // [N,K] closest_gaussian_opacities (loss only)
+    const float4* rec;       // [P] x 2 float4
+};
+
+__device__ __forceinline__ float dot3_rn(float a0, float a1, float a2, float b0, float b1, float b2) {
+    return __fadd_rn(__fadd_rn(__fmul_rn(a0, b0), __fmul_rn(a1, b1)), __fmul_rn(a2, b2));
+}
+
+// The sample's own Gaussian i, read by every lane of the segment.
+struct NormalSample {
+    bool ok;          // i inside [0, P)
+    int64_t i;
+    float x0, x1, x2;
+    float4 pc, nz;    // (p_i, c_i), (n_i, 0)
+};
+
+__device__ __forceinline__ void normal_sample(const NormalIn& a, int64_t n, NormalSample& s) {
+    s.i = a.gidx[n];
+    s.ok = s.i >= 0 && s.i < a.P;
+    s.x0 = a.x[3 * n]; s.x1 = a.x[3 * n + 1]; s.x2 = a.x[3 * n + 2];
+    const float nan = __int_as_float(0x7fc00000);
+    s.pc = s.nz = make_float4(nan, nan, nan, nan);
+    if (s.ok) { s.pc = __ldg(a.rec + 2 * s.i); s.nz = __ldg(a.rec + 2 * s.i + 1); }
+}
+
+// One (sample, neighbour) pair of the loss: sigma_j, n'_j = sigma_j n_j and the raw weight w_j.  An index outside its array is
+// never read and gives w = NaN, which the segment sum spreads over the sample.
+struct NormalPair {
+    bool ok;
+    int64_t j;
+    float sg, m0, m1, m2, w;
+};
+
+__device__ __forceinline__ void normal_pair(const NormalIn& a, int64_t n, int k, const NormalSample& s, NormalPair& f) {
+    f.j = s.ok ? a.knn[s.i * a.K + k] : -1;
+    f.ok = s.ok && f.j >= 0 && f.j < a.P;
+    if (!f.ok) {
+        f.sg = f.m0 = f.m1 = f.m2 = f.w = __int_as_float(0x7fc00000);
+        return;
+    }
+    const float4 pc = __ldg(a.rec + 2 * f.j), nz = __ldg(a.rec + 2 * f.j + 1);
+    const float dt = dot3_rn(nz.x, nz.y, nz.z, s.nz.x, s.nz.y, s.nz.z);
+    f.sg = (float)((0.0f < dt) - (dt < 0.0f));  // torch.sign: sign(0) = 0 drops the neighbour
+    f.m0 = __fmul_rn(nz.x, f.sg); f.m1 = __fmul_rn(nz.y, f.sg); f.m2 = __fmul_rn(nz.z, f.sg);
+    const float d = fabsf(dot3_rn(__fsub_rn(s.x0, pc.x), __fsub_rn(s.x1, pc.y), __fsub_rn(s.x2, pc.z), f.m0, f.m1, f.m2));
+    f.w = __fdiv_rn(__fmul_rn(a.opac[n * a.K + k], d), pc.w);
+}
+
+// The loss's segment reductions: w_hat of this lane and T = sum_j w_hat_j n'_j (every lane gets T).
+template <int W>
+__device__ __forceinline__ float normal_sums(const NormalPair& f, float& T0, float& T1, float& T2) {
+    const float S = seg_sum<W>(f.w);
+    const float wh = __fdiv_rn(f.w, S < 1e-6f ? 1e-6f : S);  // clamp(min=1e-6), NaN passes
+    T0 = seg_sum<W>(__fmul_rn(wh, f.m0));
+    T1 = seg_sum<W>(__fmul_rn(wh, f.m1));
+    T2 = seg_sum<W>(__fmul_rn(wh, f.m2));
+    return wh;
+}
+
+template <int W>
+__global__ void __launch_bounds__(256) k_normal(NormalIn a, float* __restrict__ out_loss, float* __restrict__ out_est) {
+    const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t n = (int64_t)(t / W);
+    const int k = (int)(t % W);
+    const bool active = n < a.N && k < a.K;  // every lane takes part in the shuffles
+    NormalSample s;
+    if (active) normal_sample(a, n, s);
+    if (out_loss) {
+        NormalPair f;
+        f.w = f.m0 = f.m1 = f.m2 = 0.0f;
+        if (active) normal_pair(a, n, k, s, f);
+        float T0, T1, T2;
+        normal_sums<W>(f, T0, T1, T2);
+        if (active && k == 0) {
+            const float r0 = __fsub_rn(s.nz.x, T0), r1 = __fsub_rn(s.nz.y, T1), r2 = __fsub_rn(s.nz.z, T2);
+            out_loss[n] = dot3_rn(r0, r1, r2, r0, r1, r2);
+        }
+    }
+    if (out_est && active && k == 0)
+        out_est[n] = dot3_rn(__fsub_rn(s.x0, s.pc.x), __fsub_rn(s.x1, s.pc.y), __fsub_rn(s.x2, s.pc.z), s.nz.x, s.nz.y, s.nz.z);
+}
+
+struct NormalGrad {
+    const float* g_loss;  // [N] dL/dloss
+    const float* g_est;   // [N] dL/destimate
+    float* dx;            // [N,3]
+    float4* grec;         // [P] x 2 float4: (dp.xyz, 0), (dn.xyz, 0)
+};
+
+template <int W>
+__global__ void __launch_bounds__(256) k_normal_backward(NormalIn a, NormalGrad b) {
+    const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t n = (int64_t)(t / W);
+    const int k = (int)(t % W);
+    const bool active = n < a.N && k < a.K;
+    NormalSample s;
+    s.ok = true;
+    if (active) normal_sample(a, n, s);
+    float dn0 = 0.0f, dn1 = 0.0f, dn2 = 0.0f;  // dL/dn_i of this sample (lane 0)
+    bool bad = active && !s.ok;
+    if (b.g_loss) {
+        NormalPair f;
+        f.w = f.m0 = f.m1 = f.m2 = 0.0f;
+        f.ok = true;
+        if (active) normal_pair(a, n, k, s, f);
+        float T0, T1, T2;
+        const float wh = normal_sums<W>(f, T0, T1, T2);
+        if (seg_sum<W>(f.ok ? 0.0f : 1.0f) != 0.0f) bad = active;
+        if (active && !bad) {
+            // loss = sum_c r_c^2: dr = g * (2 r); r = n_i - T: dn_i = dr, dT = -dr; T = sum_j w_hat_j (sigma_j n_j)
+            const float gl = b.g_loss[n];
+            dn0 = __fmul_rn(gl, __fmul_rn(2.0f, __fsub_rn(s.nz.x, T0)));
+            dn1 = __fmul_rn(gl, __fmul_rn(2.0f, __fsub_rn(s.nz.y, T1)));
+            dn2 = __fmul_rn(gl, __fmul_rn(2.0f, __fsub_rn(s.nz.z, T2)));
+            if (f.ok)
+                atomicAdd(b.grec + 2 * f.j + 1, make_float4(__fmul_rn(__fmul_rn(-dn0, wh), f.sg), __fmul_rn(__fmul_rn(-dn1, wh), f.sg),
+                                                            __fmul_rn(__fmul_rn(-dn2, wh), f.sg), 0.0f));
+        }
+    }
+    if (!active || k != 0) return;
+    float dx0 = 0.0f, dx1 = 0.0f, dx2 = 0.0f;
+    if (b.g_est && !bad) {
+        // est = sum_c (x - p_i)_c n_ic: d(x - p_i) = g n_i, dn_i += g (x - p_i)
+        const float ge = b.g_est[n];
+        dx0 = __fmul_rn(ge, s.nz.x); dx1 = __fmul_rn(ge, s.nz.y); dx2 = __fmul_rn(ge, s.nz.z);
+        dn0 = __fadd_rn(dn0, __fmul_rn(ge, __fsub_rn(s.x0, s.pc.x)));
+        dn1 = __fadd_rn(dn1, __fmul_rn(ge, __fsub_rn(s.x1, s.pc.y)));
+        dn2 = __fadd_rn(dn2, __fmul_rn(ge, __fsub_rn(s.x2, s.pc.z)));
+        atomicAdd(b.grec + 2 * s.i, make_float4(-dx0, -dx1, -dx2, 0.0f));
+    }
+    if (!bad && (b.g_loss || b.g_est)) atomicAdd(b.grec + 2 * s.i + 1, make_float4(dn0, dn1, dn2, 0.0f));
+    // an index outside its array: this sample adds nothing and its dL/dx is NaN
+    if (bad) dx0 = dx1 = dx2 = __int_as_float(0x7fc00000);
+    if (b.dx) { b.dx[3 * n] = dx0; b.dx[3 * n + 1] = dx1; b.dx[3 * n + 2] = dx2; }
+}
+
+__global__ void __launch_bounds__(256) k_normal_chain(int P, const float* __restrict__ scaling, const float* __restrict__ quaternions,
+                                                      const float4* __restrict__ grec, float* __restrict__ d_points,
+                                                      float* __restrict__ d_quaternions) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= P) return;
+    const size_t p3 = 3 * (size_t)p, p4 = 4 * (size_t)p;
+    const float4 gp = grec[2 * (size_t)p], gn = grec[2 * (size_t)p + 1];
+    d_points[p3] = gp.x; d_points[p3 + 1] = gp.y; d_points[p3 + 2] = gp.z;
+    int km = 0;
+    float sm = scaling[p3];
+    if (scaling[p3 + 1] < sm) { sm = scaling[p3 + 1]; km = 1; }
+    if (scaling[p3 + 2] < sm) km = 2;
+    const float qr = quaternions[p4], qi = quaternions[p4 + 1], qj = quaternions[p4 + 2], qk = quaternions[p4 + 3];
+    float R[9], t;
+    quat_to_matrix_rn(qr, qi, qj, qk, R, t);
+    float G[9] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};  // dL/dR: only column km (the gather's backward)
+    G[km] = gn.x; G[3 + km] = gn.y; G[6 + km] = gn.z;
+    float dq[4];
+    quat_to_matrix_vjp(qr, qi, qj, qk, t, G, dq);
+    d_quaternions[p4] = dq[0]; d_quaternions[p4 + 1] = dq[1]; d_quaternions[p4 + 2] = dq[2]; d_quaternions[p4 + 3] = dq[3];
+}
+
+size_t sugar_sdf_normal_bytes(int P) { return 32 * (size_t)(P < 0 ? 0 : P); }
+
+static int normal_check(const char* who, int N, int K, int P, const float* x, const int64_t* gidx, const int64_t* knn,
+                        const float* points, const float* scaling, const float* quaternions, const float* opac, bool want_loss,
+                        void* ws, size_t ws_bytes, size_t need) {
+    if (N < 0 || P < 0) { set_error("%s: negative size (N = %d, P = %d)", who, N, P); return GSR_ERR_INVALID; }
+    if (K < 1 || K > FIELD_KMAX) { set_error("%s: K = %d outside 1..%d", who, K, FIELD_KMAX); return GSR_ERR_INVALID; }
+    if (N == 0) return GSR_OK;
+    if (!x || !gidx || !points || !scaling || !quaternions) {
+        set_error("%s: an output was requested without its inputs (x, gidx, points, scaling and quaternions are required)", who);
+        return GSR_ERR_INVALID;
+    }
+    if (want_loss && (!knn || !opac)) {
+        set_error("%s: the better-normal loss needs knn_idx and the opacities", who);
+        return GSR_ERR_INVALID;
+    }
+    if (!ws || ((uintptr_t)ws & 15) || ws_bytes < need) {
+        set_error("%s: workspace null, not 16-byte aligned or too small (%zu < %zu)", who, ws_bytes, need);
+        return GSR_ERR_WORKSPACE;
+    }
+    return GSR_OK;
+}
+
+// Without the loss every sample needs one lane.
+static int normal_width(int K, bool loss) { return loss ? seg_width(K) : 1; }
+
+template <int W>
+static void launch_normal(const NormalIn& a, float* l, float* e, cudaStream_t st) {
+    const size_t threads = (size_t)a.N * W;
+    k_normal<W><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(a, l, e);
+}
+template <int W>
+static void launch_normal_backward(const NormalIn& a, const NormalGrad& g, cudaStream_t st) {
+    const size_t threads = (size_t)a.N * W;
+    k_normal_backward<W><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(a, g);
+}
+
+int sugar_sdf_normal_impl(int N, int K, int P, const float* x, const int64_t* gidx, const int64_t* knn, const float* points,
+                          const float* scaling, const float* quaternions, const float* opac, float* out_loss, float* out_est, void* ws,
+                          size_t ws_bytes, cudaStream_t st) {
+    int rc = normal_check("gsr_sugar_sdf_normal", N, K, P, x, gidx, knn, points, scaling, quaternions, opac, out_loss != nullptr, ws,
+                          ws_bytes, sugar_sdf_normal_bytes(P));
+    if (rc != GSR_OK || N == 0) return rc;
+    if (!out_loss && !out_est) return GSR_OK;
+    float4* rec = (float4*)ws;
+    if (P > 0) k_normal_prepare<<<(P + 255) / 256, 256, 0, st>>>(P, points, scaling, quaternions, rec);
+    const NormalIn a{N, K, P, x, gidx, knn, opac, rec};
+    switch (normal_width(K, out_loss != nullptr)) {
+        case 1: launch_normal<1>(a, out_loss, out_est, st); break;
+        case 2: launch_normal<2>(a, out_loss, out_est, st); break;
+        case 4: launch_normal<4>(a, out_loss, out_est, st); break;
+        case 8: launch_normal<8>(a, out_loss, out_est, st); break;
+        case 16: launch_normal<16>(a, out_loss, out_est, st); break;
+        default: launch_normal<32>(a, out_loss, out_est, st); break;
+    }
+    return check_launch("gsr_sugar_sdf_normal", false, st);
+}
+
+int sugar_sdf_normal_backward_impl(int N, int K, int P, const float* x, const int64_t* gidx, const int64_t* knn, const float* points,
+                                   const float* scaling, const float* quaternions, const float* opac, const float* g_loss,
+                                   const float* g_est, float* dx, float* d_points, float* d_quaternions, void* ws, size_t ws_bytes,
+                                   cudaStream_t st) {
+    int rc = normal_check("gsr_sugar_sdf_normal_backward", N, K, P, x, gidx, knn, points, scaling, quaternions, opac, g_loss != nullptr,
+                          ws, ws_bytes, 2 * sugar_sdf_normal_bytes(P));
+    if (rc != GSR_OK || N == 0) return rc;
+    if (P > 0 && (!d_points || !d_quaternions)) {
+        set_error("gsr_sugar_sdf_normal_backward: dL_dpoints and dL_dquaternions are required");
+        return GSR_ERR_INVALID;
+    }
+    float4* rec = (float4*)ws;
+    float4* grec = rec + 2 * (size_t)P;
+    if (P > 0) {
+        k_normal_prepare<<<(P + 255) / 256, 256, 0, st>>>(P, points, scaling, quaternions, rec);
+        cudaMemsetAsync(grec, 0, sugar_sdf_normal_bytes(P), st);
+    }
+    const NormalIn a{N, K, P, x, gidx, knn, opac, rec};
+    const NormalGrad g{g_loss, g_est, dx, grec};
+    switch (normal_width(K, g_loss != nullptr)) {
+        case 1: launch_normal_backward<1>(a, g, st); break;
+        case 2: launch_normal_backward<2>(a, g, st); break;
+        case 4: launch_normal_backward<4>(a, g, st); break;
+        case 8: launch_normal_backward<8>(a, g, st); break;
+        case 16: launch_normal_backward<16>(a, g, st); break;
+        default: launch_normal_backward<32>(a, g, st); break;
+    }
+    if (P > 0) k_normal_chain<<<(P + 255) / 256, 256, 0, st>>>(P, scaling, quaternions, grec, d_points, d_quaternions);
+    return check_launch("gsr_sugar_sdf_normal_backward", false, st);
+}
+
 }  // namespace gsr

@@ -8,6 +8,13 @@ Opt in on the class (both take the methods' exact signatures and return what the
     SuGaR.get_field_values = get_field_values
     SuGaR.compute_density = compute_density
 
+The coarse trainers' projection estimate and better-normal loss ("CD/" = sugar/sugar_trainers/coarse_density.py:704-707 and
+:756-780) run through ``gsr_sugar_sdf_normal`` / ``gsr_sugar_sdf_normal_backward``; the trainer calls them in place of those lines::
+
+    from autovfx_b200.sugar_field import projection_estimate, better_normal_loss
+    sdf_estimation = projection_estimate(sugar, sdf_samples, sdf_gaussian_idx)
+    sdf_better_normal_loss = better_normal_loss(sugar, sdf_samples, sdf_gaussian_idx, fields['closest_gaussian_opacities'])
+
 The model is read through its getters (``points``, ``scaling``, ``quaternions``, ``strengths``, ``knn_idx``, ``beta_mode``), so
 autograd carries the gradients of x and of the getters' outputs back to the raw parameters.  No [N,K,3,3] tensor is built: the
 kernels gather one 64-byte record per (sample, neighbour) pair and recompute everything in the backward.
@@ -19,7 +26,7 @@ import torch
 
 from . import _lib
 
-__all__ = ["get_field_values", "compute_density", "FIELD_MAX_K"]
+__all__ = ["get_field_values", "compute_density", "projection_estimate", "better_normal_loss", "FIELD_MAX_K"]
 
 FIELD_MAX_K = 32
 
@@ -220,3 +227,104 @@ def compute_density(self, x, closest_gaussians_idx=None, density_factor=1., retu
     if return_closest_gaussian_opacities:
         return density, opac
     return density
+
+
+# ------------------------------------------------------------------------------------------------ better-normal loss, estimate
+def _sdf_normal_forward(want_loss, K, x, gidx, knn, points, scaling, quaternions, opac):
+    N, P = x.shape[0], points.shape[0]
+    out = torch.empty(N, dtype=torch.float32, device=x.device)
+    if N > 0:
+        L = _lib_handle()
+        nbytes = L.gsr_sugar_sdf_normal_bytes(P)
+        ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=x.device)
+        rc = L.gsr_sugar_sdf_normal(N, K, P, x.data_ptr(), gidx.data_ptr(), _ptr(knn), points.data_ptr(), scaling.data_ptr(),
+                                    quaternions.data_ptr(), _ptr(opac), out.data_ptr() if want_loss else None,
+                                    None if want_loss else out.data_ptr(), ws.data_ptr(), nbytes, _lib.stream_ptr(x.device))
+        _lib.check(rc, "gsr_sugar_sdf_normal")
+    return out
+
+
+class _SugarSdfNormal(torch.autograd.Function):
+    """One output: the better-normal loss [N] (want_loss) or the projection estimate [N]."""
+
+    @staticmethod
+    def forward(ctx, x, points, quaternions, scaling, gidx, knn, opac, want_loss, K):
+        ctx.set_materialize_grads(False)
+        ctx.want_loss, ctx.K = want_loss, K
+        ctx.save_for_backward(x, points, quaternions, scaling, gidx, knn, opac)
+        return _sdf_normal_forward(want_loss, K, x, gidx, knn, points, scaling, quaternions, opac)
+
+    @staticmethod
+    def backward(ctx, g):
+        x, points, quaternions, scaling, gidx, knn, opac = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        dx = torch.zeros_like(x) if need[0] else None
+        d_points = torch.zeros_like(points)
+        d_quaternions = torch.zeros_like(quaternions)
+        N, P = x.shape[0], points.shape[0]
+        if N > 0 and g is not None:
+            g = g.contiguous()
+            L = _lib_handle()
+            nbytes = 2 * L.gsr_sugar_sdf_normal_bytes(P)
+            ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=x.device)
+            rc = L.gsr_sugar_sdf_normal_backward(N, ctx.K, P, x.data_ptr(), gidx.data_ptr(), _ptr(knn), points.data_ptr(),
+                                                 scaling.data_ptr(), quaternions.data_ptr(), _ptr(opac),
+                                                 g.data_ptr() if ctx.want_loss else None, None if ctx.want_loss else g.data_ptr(),
+                                                 _ptr(dx), d_points.data_ptr(), d_quaternions.data_ptr(), ws.data_ptr(), nbytes,
+                                                 _lib.stream_ptr(x.device))
+            _lib.check(rc, "gsr_sugar_sdf_normal_backward")
+        return (dx, d_points if need[1] else None, d_quaternions if need[2] else None, None, None, None, None, None, None)
+
+
+def _sdf_normal(who, self, sdf_samples, sdf_gaussian_idx, opacities, want_loss):
+    if getattr(self, "binded_to_surface_mesh", False):
+        raise ValueError("%s: a model bound to a surface mesh is not supported (its normals are face normals; the refinement runs "
+                         "with regularize_sdf = False)" % who)
+    points, scaling, quaternions, _ = _model_tensors(who, self)
+    P = points.shape[0]
+    _check_tensor(who, "sdf_samples", sdf_samples, (None, 3), torch.float32)
+    N = sdf_samples.shape[0]
+    _check_tensor(who, "sdf_gaussian_idx", sdf_gaussian_idx, (N,), torch.int64)
+    knn = opac = None
+    K = 1
+    if want_loss:
+        knn = self.knn_idx
+        _check_tensor(who, "self.knn_idx", knn, (P, None), torch.int64)
+        K = knn.shape[1]
+        if not 1 <= K <= FIELD_MAX_K:
+            raise ValueError("%s: K = %d neighbours per Gaussian must be in 1..%d" % (who, K, FIELD_MAX_K))
+        _check_tensor(who, "closest_gaussian_opacities", opacities, (N, K), torch.float32)
+        knn = knn.contiguous()
+        opac = opacities.detach().contiguous()
+    _require_cuda(who, sdf_samples, sdf_gaussian_idx, knn, opac, points, scaling, quaternions)
+    gidx = sdf_gaussian_idx.contiguous()
+    x, points, quaternions = (t.contiguous() for t in (sdf_samples, points, quaternions))
+    scaling = scaling.detach().contiguous()
+    with torch.cuda.device(x.device):
+        diff = (quaternions,) if want_loss else (x, points, quaternions)
+        if torch.is_grad_enabled() and any(t.requires_grad for t in diff):
+            if want_loss:  # the loss carries no gradient to the samples or the centres
+                x, points = x.detach(), points.detach()
+            return _SugarSdfNormal.apply(x, points, quaternions, scaling, gidx, knn, opac, want_loss, K)
+        return _sdf_normal_forward(want_loss, K, x, gidx, knn, points, scaling, quaternions, opac)
+
+
+def projection_estimate(self, sdf_samples, sdf_gaussian_idx):
+    """The coarse trainers' projection estimate (CD/:706-707) in CUDA: ((sdf_samples - points[i]) * normals[i]).sum(-1) with
+    i = sdf_gaussian_idx and normals = self.get_normals() (the smallest axis).  Returns [N], differentiable with respect to the
+    samples, ``points`` and ``quaternions``.
+
+    Raises ValueError, naming the argument, for a wrong shape or dtype or a model bound to a surface mesh; RuntimeError for CPU
+    tensors (there is no CPU path)."""
+    return _sdf_normal("projection_estimate", self, sdf_samples, sdf_gaussian_idx, None, False)
+
+
+def better_normal_loss(self, sdf_samples, sdf_gaussian_idx, closest_gaussian_opacities):
+    """The coarse trainers' better-normal loss per sample (CD/:756-780, before the trainer's ``.mean()``) in CUDA, over the
+    neighbours self.knn_idx[sdf_gaussian_idx] (read in place, never gathered) weighted by closest_gaussian_opacities [N,K]
+    (read detached).  Returns [N], differentiable with respect to ``quaternions`` only: the trainer's
+    sdf_better_normal_gradient_through_normal_only detaches the weights, so the samples, points and scales get nothing.
+
+    Raises ValueError, naming the argument, for wrong shapes, dtypes or widths (the opacities' K must equal knn_idx's), K outside
+    1..32 and a model bound to a surface mesh; RuntimeError for CPU tensors (there is no CPU path)."""
+    return _sdf_normal("better_normal_loss", self, sdf_samples, sdf_gaussian_idx, closest_gaussian_opacities, True)

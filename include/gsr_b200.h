@@ -13,6 +13,8 @@
  *   gsr_knn           replaces  pytorch3d.ops.knn_points in SuGaR  sugar_scene/sugar_model.py:47, :233, :899, :914, :1213 (N = 1, D = 3)
  *   gsr_sugar_field   replaces  SuGaR.get_field_values / compute_density  sugar_scene/sugar_model.py:1118-1187, :1216-1239
  *                               (get_covariance :602-608, get_beta 'average' :1063-1066); gsr_sugar_field_backward their autograd
+ *   gsr_sugar_sdf_normal replaces the coarse trainers' better-normal loss and projection estimate
+ *                               sugar_trainers/coarse_density.py:704-707, :756-780; gsr_sugar_sdf_normal_backward their autograd
  *
  * and, for the render() wrapper around the two rasterizer passes ("GR/" = sugar/gaussian_splatting/gaussian_renderer/__init__.py):
  *
@@ -325,6 +327,31 @@ int gsr_sugar_field_backward(int32_t N, int32_t K, int32_t P, int32_t R, const f
                              const float* dL_dopacities, const float* dL_dbeta, const float* dL_dsdf, float* dL_dx, float* dL_dpoints,
                              float* dL_dscaling, float* dL_dquaternions, float* dL_dstrengths, void* workspace, size_t workspace_bytes,
                              void* stream);
+
+/* The coarse trainers' better-normal loss and projection estimate (sugar_trainers/coarse_density.py:704-707, :756-780) at N samples
+ * x [N,3], each in the Gaussian gidx[n] of P given by SuGaR's getters (points [P,3], scaling [P,3], quaternions [P,4]), with the K
+ * neighbours knn_idx[gidx[n], 0..K-1] of the int64 table knn_idx [P,K] (1 <= K <= 32) and their opacities [N,K].  n_g is column
+ * k_g of quaternion_to_matrix(q_g), k_g the lowest index of min(s_g); with i = gidx[n], per neighbour j:
+ *   sigma_j = sign(n_j . n_i), w_j = (o_nj * |(x - p_j) . sigma_j n_j|) / clamp(min s_j, 1e-6)^2, w_hat_j = w_j / clamp(sum w, 1e-6)
+ *   out_loss     [N] = |n_i - sum_j w_hat_j sigma_j n_j|^2
+ *   out_estimate [N] = (x - p_i) . n_i
+ * Either output may be NULL (not requested); knn_idx and opacities are read only for the loss.  N = 0 is a no-op.  Negative sizes,
+ * K outside 1..32 or a missing input for a requested output are GSR_ERR_INVALID; `workspace` (16-byte aligned) needs
+ * gsr_sugar_sdf_normal_bytes(P) bytes for the forward, twice that for the backward, else GSR_ERR_WORKSPACE.  An index outside its
+ * array is never read: the outputs that depend on it are NaN. */
+size_t gsr_sugar_sdf_normal_bytes(int32_t P);
+int gsr_sugar_sdf_normal(int32_t N, int32_t K, int32_t P, const float* x, const int64_t* gidx, const int64_t* knn_idx,
+                         const float* points, const float* scaling, const float* quaternions, const float* opacities, float* out_loss,
+                         float* out_estimate, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Backward of gsr_sugar_sdf_normal (same sizes and inputs; it recomputes the forward).  sigma, the weights, their sum, the
+ * opacities and the scales are constants, as in the trainer, so the loss reaches the quaternions only; the estimate reaches x,
+ * the points and the quaternions.  dL_dloss and dL_destimate may be NULL; dL_dx [N,3] may be NULL; dL_dpoints [P,3] and
+ * dL_dquaternions [P,4] are required and written in full.  A sample with an index outside its array adds nothing; its dL_dx is NaN. */
+int gsr_sugar_sdf_normal_backward(int32_t N, int32_t K, int32_t P, const float* x, const int64_t* gidx, const int64_t* knn_idx,
+                                  const float* points, const float* scaling, const float* quaternions, const float* opacities,
+                                  const float* dL_dloss, const float* dL_destimate, float* dL_dx, float* dL_dpoints,
+                                  float* dL_dquaternions, void* workspace, size_t workspace_bytes, void* stream);
 
 /* Device pointers into the workspaces of the last layout (P, capacity, W, H) — for parity tests that
  * compare per-stage buffers with the reference (SURVEY §4).  Pure pointer arithmetic, no CUDA calls. */
