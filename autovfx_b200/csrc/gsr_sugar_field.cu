@@ -150,8 +150,14 @@ __global__ void __launch_bounds__(256) k_field_backward(FieldIn a, FieldGrad b) 
     const float d = seg_sum<W>(f.o);
     float bsum = 0.0f;
     if (b.g_sdf) bsum = seg_sum<W>(f.smin);
+    // One lane with an index outside its array makes d and beta NaN for the whole segment, so the sample adds nothing to any
+    // Gaussian (not even through its valid lanes) and its dL/dx is NaN.
+    const unsigned seg = W == 32 ? 0xffffffffu : ((1u << W) - 1u) << ((threadIdx.x & 31u) & ~(unsigned)(W - 1));
+    const bool bad = (__ballot_sync(0xffffffffu, active && !f.ok) & seg) != 0u;
     float ds0 = 0.0f, ds1 = 0.0f, ds2 = 0.0f;  // dL/dshift of this pair
-    if (active) {
+    if (active && bad) {
+        ds0 = ds1 = ds2 = __int_as_float(0x7fc00000);
+    } else if (active) {  // every lane of the segment is inside its arrays
         // per-sample gradient reaching every o_nk through densities.sum(dim=-1)
         float G = b.g_density ? b.g_density[n] : 0.0f;
         float gbeta = b.g_beta ? b.g_beta[n] : 0.0f;
@@ -167,25 +173,21 @@ __global__ void __launch_bounds__(256) k_field_backward(FieldIn a, FieldGrad b) 
             const float gdh = dh >= a.opacity_min_clamp ? gcd : 0.0f;
             G = __fadd_rn(G, d >= 1.0f ? __fdiv_rn(gdh, __fadd_rn(d, 1e-12f)) : gdh);
         }
-        if (f.ok) {
-            const float go = b.g_opac ? __fadd_rn(G, b.g_opac[n * a.K + k]) : G;
-            const float dfs = __fmul_rn(go, f.e);
-            const float dqc = __fmul_rn(__fmul_rn(__fmul_rn(go, f.fs), f.e), -0.5f);
-            const float dq = (f.q <= 1e8f) ? dqc : 0.0f;  // clamp(0, 1e8) passes where 0 <= q <= 1e8
-            const float dw0 = __fmul_rn(2.0f, __fmul_rn(dq, f.w0)), dw1 = __fmul_rn(2.0f, __fmul_rn(dq, f.w1)),
-                        dw2 = __fmul_rn(2.0f, __fmul_rn(dq, f.w2));
-            ds0 = __fadd_rn(__fadd_rn(__fmul_rn(f.A[0], dw0), __fmul_rn(f.A[1], dw1)), __fmul_rn(f.A[2], dw2));
-            ds1 = __fadd_rn(__fadd_rn(__fmul_rn(f.A[3], dw0), __fmul_rn(f.A[4], dw1)), __fmul_rn(f.A[5], dw2));
-            ds2 = __fadd_rn(__fadd_rn(__fmul_rn(f.A[6], dw0), __fmul_rn(f.A[7], dw1)), __fmul_rn(f.A[8], dw2));
-            const float dmin = (b.g_beta || b.g_sdf) ? __fdiv_rn(gbeta, (float)a.K) : 0.0f;
-            float4* gr = b.grec + 4 * f.g;
-            atomicAdd(gr, make_float4(-ds0, -ds1, -ds2, dfs));
-            atomicAdd(gr + 1, make_float4(__fmul_rn(dw0, f.sx), __fmul_rn(dw1, f.sx), __fmul_rn(dw2, f.sx), __fmul_rn(dw0, f.sy)));
-            atomicAdd(gr + 2, make_float4(__fmul_rn(dw1, f.sy), __fmul_rn(dw2, f.sy), __fmul_rn(dw0, f.sz), __fmul_rn(dw1, f.sz)));
-            atomicAdd(gr + 3, make_float4(__fmul_rn(dw2, f.sz), dmin, 0.0f, 0.0f));
-        } else {
-            ds0 = ds1 = ds2 = __int_as_float(0x7fc00000);  // an index outside its array: NaN in this sample's dL/dx
-        }
+        const float go = b.g_opac ? __fadd_rn(G, b.g_opac[n * a.K + k]) : G;
+        const float dfs = __fmul_rn(go, f.e);
+        const float dqc = __fmul_rn(__fmul_rn(__fmul_rn(go, f.fs), f.e), -0.5f);
+        const float dq = (f.q <= 1e8f) ? dqc : 0.0f;  // clamp(0, 1e8) passes where 0 <= q <= 1e8
+        const float dw0 = __fmul_rn(2.0f, __fmul_rn(dq, f.w0)), dw1 = __fmul_rn(2.0f, __fmul_rn(dq, f.w1)),
+                    dw2 = __fmul_rn(2.0f, __fmul_rn(dq, f.w2));
+        ds0 = __fadd_rn(__fadd_rn(__fmul_rn(f.A[0], dw0), __fmul_rn(f.A[1], dw1)), __fmul_rn(f.A[2], dw2));
+        ds1 = __fadd_rn(__fadd_rn(__fmul_rn(f.A[3], dw0), __fmul_rn(f.A[4], dw1)), __fmul_rn(f.A[5], dw2));
+        ds2 = __fadd_rn(__fadd_rn(__fmul_rn(f.A[6], dw0), __fmul_rn(f.A[7], dw1)), __fmul_rn(f.A[8], dw2));
+        const float dmin = (b.g_beta || b.g_sdf) ? __fdiv_rn(gbeta, (float)a.K) : 0.0f;
+        float4* gr = b.grec + 4 * f.g;
+        atomicAdd(gr, make_float4(-ds0, -ds1, -ds2, dfs));
+        atomicAdd(gr + 1, make_float4(__fmul_rn(dw0, f.sx), __fmul_rn(dw1, f.sx), __fmul_rn(dw2, f.sx), __fmul_rn(dw0, f.sy)));
+        atomicAdd(gr + 2, make_float4(__fmul_rn(dw1, f.sy), __fmul_rn(dw2, f.sy), __fmul_rn(dw0, f.sz), __fmul_rn(dw1, f.sz)));
+        atomicAdd(gr + 3, make_float4(__fmul_rn(dw2, f.sz), dmin, 0.0f, 0.0f));
     }
     ds0 = seg_sum<W>(ds0);
     ds1 = seg_sum<W>(ds1);

@@ -310,7 +310,7 @@ int gsr_knn(int32_t P1, int32_t P2, int32_t K, const float* queries, const float
  * Any output may be NULL (not requested).  N = 0 is a no-op.  Negative sizes, K outside 1..32, row_idx NULL with R != N, or a
  * missing input when N > 0 are GSR_ERR_INVALID; `workspace` (16-byte aligned) needs gsr_sugar_field_bytes(P) bytes for the
  * forward, twice that for the backward, else GSR_ERR_WORKSPACE.  A row or Gaussian index outside its array is never read: the
- * sample's outputs are NaN. */
+ * sample's density, beta and sdf are NaN, and so are its opacities at the pairs whose index is outside (all K for a bad row). */
 size_t gsr_sugar_field_bytes(int32_t P);
 int gsr_sugar_field(int32_t N, int32_t K, int32_t P, int32_t R, const float* x, const int64_t* rows, const int64_t* row_idx,
                     const float* points, const float* scaling, const float* quaternions, const float* strengths, float density_factor,
@@ -320,7 +320,8 @@ int gsr_sugar_field(int32_t N, int32_t K, int32_t P, int32_t R, const float* x, 
 /* Backward of gsr_sugar_field (same sizes, inputs and constants; it recomputes the forward): the gradients of the four outputs in
  * (any may be NULL; dL_dsdf and dL_dbeta need no forward output), torch's backward formulas out: dL_dx [N,3] (may be NULL) and
  * dL_dpoints [P,3], dL_dscaling [P,3], dL_dquaternions [P,4], dL_dstrengths [P] (required, written in full).  Where torch's
- * gradient is not finite (d >= 1 with an sdf gradient: sqrt'(0)), this one is not either. */
+ * gradient is not finite (d >= 1 with an sdf gradient: sqrt'(0)), this one is not either.  A sample with a row or Gaussian index
+ * outside its array adds nothing to any Gaussian, through none of its K pairs; its dL_dx is NaN. */
 int gsr_sugar_field_backward(int32_t N, int32_t K, int32_t P, int32_t R, const float* x, const int64_t* rows, const int64_t* row_idx,
                              const float* points, const float* scaling, const float* quaternions, const float* strengths,
                              float density_factor, float opacity_min_clamp, float sdf_offset, const float* dL_ddensity,
