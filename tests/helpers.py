@@ -324,10 +324,24 @@ def grad_args(family: str, device=None, opacity_cap: float = 0.95) -> Dict:
 
 
 def isolated_image_grads(a: Dict, term: str, device=None):
-    """image_grads with all but one of dL/dcolor, dL/ddepth, dL/dalpha set to zero (term "all" keeps the three)."""
+    """image_grads with all but one of dL/dcolor, dL/ddepth, dL/dalpha set to zero (term "all" keeps the three, "extra", the loss
+    on the second colour set's image alone, none)."""
     dc, dd, da = image_grads(a, device=device)
-    keep = {"color": (1, 0, 0), "depth": (0, 1, 0), "alpha": (0, 0, 1), "all": (1, 1, 1)}[term]
+    keep = {"color": (1, 0, 0), "depth": (0, 1, 0), "alpha": (0, 0, 1), "all": (1, 1, 1), "extra": (0, 0, 0)}[term]
     return dc * keep[0], dd * keep[1], da * keep[2]
+
+
+def extra_pass(a: Dict, extra: torch.Tensor) -> Dict:
+    """The arguments of the pass that blends a second colour set extra [P,3] (the normals of render()) with the same weights: a's
+    geometry with colors_precomp = extra."""
+    return dict(a, shs=None, colors_precomp=extra)
+
+
+def extra_image_grad(a: Dict, term: str, device=None) -> torch.Tensor:
+    """dL/dE of the second colour set's image, ~ N(0,1) with seed 8, under the terms "extra" and "all"; zeros under the others."""
+    de = torch.randn(3, a["H"], a["W"], generator=torch.Generator().manual_seed(8))
+    de = de if term in ("extra", "all") else torch.zeros_like(de)
+    return de if device is None else de.to(device)
 
 
 def row_errors(g, g64) -> np.ndarray:
@@ -339,31 +353,51 @@ def row_errors(g, g64) -> np.ndarray:
     return ((g - g64).norm(dim=1)[keep] / n[keep]).numpy()
 
 
-def fp64_grads(a: Dict, fw, terms, oracle_decisions=False) -> Dict:
+def fp64_grads(a: Dict, fw, terms, oracle_decisions=False, extra=None) -> Dict:
     """{term: {name: fp64 autograd gradient}} of torch_ref.render on the oracle's tile lists, for each isolated loss term.  Names
     follow the oracle's dL_d* keys; dL_dmeans2D holds the pixel gradient scaled to the reference's units (0.5 W, 0.5 H).  The
     frustum clamp is differentiated as the reference does (Gaussians near the image border differ from the true gradient).
     oracle_decisions: the skip / terminate decisions are the oracle's fp32 ones, so that a row differs only by arithmetic (else
-    they are taken on the fp64 values)."""
+    they are taken on the fp64 values).
+    extra: (b, fb), the extra_pass arguments of a second colour set and the oracle's forward of them.  Each term's gradients are
+    then those of both passes summed, the second's loss being dL/dE (extra_image_grad) . E, and its dL/dcolors is dL_dextra."""
     from tests import torch_ref
-    color, depth, alpha, leaves, m2d = torch_ref.render(a, fw, reference_clamp_grad=True, oracle_decisions=oracle_decisions)
     names = {"means3D": "dL_dmeans3D", "opacities": "dL_dopacity", "shs": "dL_dsh", "scales": "dL_dscales", "rotations": "dL_drotations",
              "colors_precomp": "dL_dcolors", "cov3D_precomp": "dL_dcov3D"}
-    inputs = [(k, v) for k, v in leaves.items() if v is not None] + [("means2D", m2d)]
+    passes = [(a, fw, False)] + ([(extra[0], extra[1], True)] if extra is not None else [])
+    graphs = [torch_ref.render(p, f, reference_clamp_grad=True, oracle_decisions=oracle_decisions) + (second,) for p, f, second in passes]
     out = {}
     for term in terms:
-        dc, dd, da = isolated_image_grads(a, term)
-        loss = (color * dc.double()).sum() + (depth * dd.double()).sum() + (alpha * da.double()).sum()
-        gs = torch.autograd.grad(loss, [v for _, v in inputs], retain_graph=True, allow_unused=True)
         res = {}
-        for (k, v), gr in zip(inputs, gs):
-            gr = torch.zeros_like(v) if gr is None else gr
-            if k == "means2D":
-                res["dL_dmeans2D"] = gr * torch.tensor([0.5 * a["W"], 0.5 * a["H"]], dtype=torch.float64)
-            else:
-                res[names[k]] = gr
+        for color, depth, alpha, leaves, m2d, second in graphs:
+            weights = (extra_image_grad(a, term),) if second else isolated_image_grads(a, term)
+            loss = sum((img * w.double()).sum() for img, w in zip((color, depth, alpha), weights))
+            inputs = [(k, v) for k, v in leaves.items() if v is not None] + [("means2D", m2d)]
+            if any(bool(w.any()) for w in weights):
+                gs = torch.autograd.grad(loss, [v for _, v in inputs], retain_graph=True, allow_unused=True)
+            else:  # a pass the term leaves out of the loss: zero gradients without an autograd pass
+                gs = [None] * len(inputs)
+            for (k, v), gr in zip(inputs, gs):
+                gr = torch.zeros_like(v) if gr is None else gr
+                if k == "means2D":
+                    key, gr = "dL_dmeans2D", gr * torch.tensor([0.5 * a["W"], 0.5 * a["H"]], dtype=torch.float64)
+                else:
+                    key = "dL_dextra" if (second and k == "colors_precomp") else names[k]
+                res[key] = res[key] + gr if key in res else gr
         out[term] = res
     return out
+
+
+def oracle_two_pass_grads(a: Dict, fw, b: Dict, fb, dc, dd, da, de) -> Dict:
+    """comparable_grads of the oracle's backward of the colour pass a (loss dc, dd, da) plus that of the extra pass b (loss de on its
+    colour image): the gradients of a frame that blends both colour sets with the same weights, dL_dextra the second's dL/dcolors."""
+    o1 = comparable_grads(oracle_backward(a, fw, dc, dd, da), a)
+    o2 = comparable_grads(oracle_backward(b, fb, de, 0 * dd, 0 * da), b)
+    o = {k: (v + o2[k] if k in o2 and o2[k].shape == v.shape else v) for k, v in o1.items() if k != "dL_dcolors"}
+    o["dL_dextra"] = o2["dL_dcolors"]
+    if a["colors_precomp"] is not None:
+        o["dL_dcolors"] = o1["dL_dcolors"]
+    return o
 
 
 def comparable_grads(g: Dict, a: Dict) -> Dict:

@@ -3,15 +3,18 @@
 The GPU's per-Gaussian gradients on those cases are judged against the oracle's own per-row error with respect to fp64 autograd,
 so the oracle is pinned here on the same cases, and each case is shown to reach the regimes of the blend backward it is there
 for (tests/helpers.DENSE_CASES) before any GPU time is spent.  dense_tile's fp64 reference costs minutes; sort_regimes, with
-tiles of over 4,096 entries, stands in for it.
+tiles of over 4,096 entries, stands in for it.  The GPU's fused backward (a second colour set blended with the same weights) is
+judged against the oracle's colour pass plus its colors_precomp = extra pass, so the terms extra (that pass alone) and all (both
+summed) pin the second pass too, on every dense case but dense_tile.
 """
 import numpy as np
 import pytest
+import torch
 
 from tests import helpers as Hh
 
-TERMS = ("color", "depth", "alpha", "all")
-PINNED = ("sort_regimes", "faint_slab", "skip_band")
+TERMS = ("color", "depth", "alpha", "extra", "all")
+PINNED = ("sort_regimes", "faint_slab", "skip_band", "coplanar", "config1")
 
 # Oracle against fp64 autograd on the oracle's decisions, per-Gaussian relative error (rows with ||g64|| > 1e-6 of the largest).
 # Sums over hundreds of survivors cancel more than on the small cases of test_variants_cpu.py: measured over every case, term and
@@ -31,14 +34,15 @@ def test_dense_case_reaches_its_regimes(name):
 @pytest.fixture(scope="module", params=PINNED)
 def pinned(request):
     a = Hh.dense_case(request.param)
-    fw = Hh.run_oracle(a)
-    return request.param, a, fw, Hh.fp64_grads(a, fw, TERMS, oracle_decisions=True)
+    b = Hh.extra_pass(a, torch.rand(a["means3D"].shape[0], 3, generator=torch.Generator().manual_seed(21)))  # as the GPU test's
+    fw, fb = Hh.run_oracle(a), Hh.run_oracle(b)
+    return request.param, a, fw, b, fb, Hh.fp64_grads(a, fw, TERMS, oracle_decisions=True, extra=(b, fb))
 
 
 @pytest.mark.parametrize("term", TERMS)
 def test_oracle_dense_gradients_per_gaussian_match_fp64(pinned, term):
-    name, a, fw, g64 = pinned
-    og = Hh.comparable_grads(Hh.oracle_backward(a, fw, *Hh.isolated_image_grads(a, term)), a)
+    name, a, fw, b, fb, g64 = pinned
+    og = Hh.oracle_two_pass_grads(a, fw, b, fb, *Hh.isolated_image_grads(a, term), Hh.extra_image_grad(a, term))
     checked = 0
     for k, want in g64[term].items():
         # on the same decisions, the same Gaussians have a non-zero row
@@ -50,7 +54,7 @@ def test_oracle_dense_gradients_per_gaussian_match_fp64(pinned, term):
         stats = (np.median(e), np.quantile(e, 0.99), e.max())
         assert stats[0] <= ORACLE_MEDIAN_TOL and stats[1] <= ORACLE_Q99_TOL, (name, term, k, stats)
         checked += 1
-    assert checked >= 4
+    assert checked >= 4 and (term not in ("extra", "all") or "dL_dextra" in g64[term])
 
 
 def test_skip_band_splats_contribute_at_one_pixel_or_nowhere():

@@ -34,6 +34,9 @@ pytestmark = pytest.mark.gpu
 
 CASES = ["config1", "small_sh", "small_deg1_m25", "small_precomp", "big_splats", "dense_tile", "coplanar"]
 FAMILIES = ["precomp", "M25_D2_off", "M16_D3"]  # colours and covariances precomputed; M = 25 rows 4 bytes off alignment
+# the dense cases of tests/helpers.DENSE_CASES that CASES lacks: the backward's redo band, ballot block edge, top-row mask of
+# partial footprints and deep termination
+DENSE = ["skip_band", "faint_slab", "sort_regimes"]
 TERMS = ("color", "depth", "alpha", "extra", "all")
 NAMES = {"means3D": "dL_dmeans3D", "opacities": "dL_dopacity", "shs": "dL_dsh", "colors_precomp": "dL_dcolors", "scales": "dL_dscales",
          "rotations": "dL_drotations", "cov3D_precomp": "dL_dcov3D", "extra": "dL_dextra"}
@@ -69,7 +72,7 @@ def _extra(P, dev, seed=21):
 
 
 def _args(name, dev):
-    return Hh.grad_args(name, dev) if name in Hh.GRAD_FAMILIES else Hh.resolve(Hh.case_inputs(name), dev)
+    return Hh.grad_args(name, dev) if name in Hh.GRAD_FAMILIES else Hh.dense_case(name, dev)
 
 
 def _leaves(a, extra):
@@ -128,7 +131,7 @@ def _loss_imgs(a, term, dev, zeros=False):
     """Seeded gradients of the colour, depth, alpha and extra images; the images a term leaves out of the loss get None (so that
     they receive no gradient at all), or zeros."""
     dc, dd, da = Hh.image_grads(a, device=dev)
-    de = torch.randn(3, a["H"], a["W"], generator=torch.Generator().manual_seed(8)).to(dev)
+    de = Hh.extra_image_grad(a, "all", device=dev)
     keep = {"color": (1, 0, 0, 0), "depth": (0, 1, 0, 0), "alpha": (0, 0, 1, 0), "extra": (0, 0, 0, 1), "all": (1, 1, 1, 1)}[term]
     return tuple(g if k else (torch.zeros_like(g) if zeros else None) for g, k in zip((dc, dd, da, de), keep))
 
@@ -189,7 +192,7 @@ def test_forward_equals_one_pass_and_two_calls(dev, exact, name, tight):
 
 
 # ---- 2. against the two-call graph ----------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("name", CASES + FAMILIES)
+@pytest.mark.parametrize("name", CASES + FAMILIES + DENSE)
 def test_gradients_match_the_two_call_graph(dev, exact, name):
     a = _args(name, dev)
     extra = _extra(a["means3D"].shape[0], dev)
@@ -208,35 +211,12 @@ def test_gradients_match_the_two_call_graph(dev, exact, name):
 @pytest.fixture(scope="module", params=FAMILIES)
 def fp64_family(request, dev):
     """(name, a, extra, {term: fp64 gradients}, {term: the oracle's two passes summed}) for the terms 'extra' and 'all'."""
-    from tests import torch_ref
     a = Hh.grad_args(request.param, dev)
     extra = _extra(a["means3D"].shape[0], dev)
-    b = dict(a, shs=None, colors_precomp=extra)
+    b = Hh.extra_pass(a, extra)
     fa, fb = Hh.run_oracle(a), Hh.run_oracle(b)
-    ra, rb = torch_ref.render(a, fa, reference_clamp_grad=True), torch_ref.render(b, fb, reference_clamp_grad=True)
-    names = dict(NAMES, means2D="dL_dmeans2D")
-    g64, orc = {}, {}
-    for term in ("extra", "all"):
-        dc, dd, da, de = (t.cpu() for t in _loss_imgs(a, term, dev, zeros=True))
-        res = {}
-        for (color, depth, alpha, leaves, m2d), (gc, gd, ga), second in ((ra, (dc, dd, da), False), (rb, (de, 0 * dd, 0 * da), True)):
-            loss = (color * gc.double()).sum() + (depth * gd.double()).sum() + (alpha * ga.double()).sum()
-            inputs = [(k, v) for k, v in leaves.items() if v is not None] + [("means2D", m2d)]
-            gs = torch.autograd.grad(loss, [v for _, v in inputs], retain_graph=True, allow_unused=True)
-            for (k, v), gr in zip(inputs, gs):
-                gr = torch.zeros_like(v) if gr is None else gr
-                if k == "means2D":
-                    gr = gr * torch.tensor([0.5 * a["W"], 0.5 * a["H"]], dtype=torch.float64)
-                key = "dL_dextra" if (second and k == "colors_precomp") else names[k]
-                res[key] = res[key] + gr if key in res else gr
-        g64[term] = res
-        o1 = Hh.comparable_grads(Hh.oracle_backward(a, fa, dc, dd, da), a)
-        o2 = Hh.comparable_grads(Hh.oracle_backward(b, fb, de, 0 * dd, 0 * da), b)
-        o = {k: (v + o2[k] if k in o2 and o2[k].shape == v.shape else v) for k, v in o1.items() if k != "dL_dcolors"}
-        o["dL_dextra"] = o2["dL_dcolors"]
-        if a["colors_precomp"] is not None:
-            o["dL_dcolors"] = o1["dL_dcolors"]
-        orc[term] = o
+    g64 = Hh.fp64_grads(a, fa, ("extra", "all"), extra=(b, fb))
+    orc = {term: Hh.oracle_two_pass_grads(a, fa, b, fb, *(t.cpu() for t in _loss_imgs(a, term, dev, zeros=True))) for term in ("extra", "all")}
     return request.param, a, extra, g64, orc
 
 
@@ -452,7 +432,7 @@ def test_partly_null_extra_arguments_are_rejected(dev):
 
 
 # ---- 6. register budgets of the blend backward, each in a fresh process -----------------------------------------------------------
-VARIANT_CASES = ["dense_tile", "coplanar", "config1", "M25_D2_off", "precomp"]
+VARIANT_CASES = ["dense_tile", "coplanar", "config1", "M25_D2_off", "precomp"] + DENSE
 
 
 def _variant_grads(dev):

@@ -247,13 +247,15 @@ def test_clamped_alpha_gradients_against_oracle_and_reference(dev):
 # the 16-byte aligned M = 16 rows take the vector staging (cp.async under GSR_SH_STAGING=cpasync) at every degree
 VARIANT_LAYOUTS = [(1, 0, False), (4, 1, False), (9, 2, False), (16, 0, False), (16, 2, False), (16, 3, True), (25, 3, False),
                    (25, 1, False), (None, 0, False)]
-# named cases of test_gpu_parity.py (dense_tile: tiles of > 4096 instances; coplanar: equal depths, ties broken by id) and a scene
-# with tiles in each of the three sort regimes, so that the general (unpacked) path runs every per-tile sort
-VARIANT_CASES = ["dense_tile", "coplanar", "config1", "deg3_m25", "sort_regimes"]
+# named cases of test_gpu_parity.py (dense_tile: tiles of > 4096 instances; coplanar: equal depths, ties broken by id), a scene
+# with tiles in each of the three sort regimes, so that the general (unpacked) path runs every per-tile sort, and the dense
+# gradient cases that reach the blend backward's redo band, ballot block edge, partial footprints and deep termination
+# (tests/helpers.DENSE_CASES), so that every register budget of the backward runs them
+VARIANT_CASES = ["dense_tile", "coplanar", "config1", "deg3_m25", "sort_regimes", "skip_band", "faint_slab"]
 
 
 def _case_args(name, dev):
-    return Hh.resolve(Hh.sort_regimes_case() if name == "sort_regimes" else Hh.case_inputs(name), dev)
+    return Hh.dense_case(name, dev)
 
 
 def _variant_outputs(dev):
