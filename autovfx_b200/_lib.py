@@ -52,6 +52,14 @@ class gsr_object_xform(C.Structure):
                 ("scaling", C.c_float), ("log_scaling", C.c_float)]
 
 
+class gsr_densify_group(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("dst", C.c_void_p), ("m1_src", C.c_void_p), ("m1_dst", C.c_void_p), ("m2_src", C.c_void_p),
+                ("m2_dst", C.c_void_p), ("width", C.c_int32), ("role", C.c_int32)]
+
+
+GSR_DENSIFY_MAX_GROUPS = 8
+GSR_DENSIFY_ROLE_COPY, GSR_DENSIFY_ROLE_XYZ, GSR_DENSIFY_ROLE_SCALING = 0, 1, 2
+GSR_DENSIFY_ROTATION_3DGS, GSR_DENSIFY_ROTATION_SUGAR = 0, 1
 GSR_FLAG_FOR_BACKWARD = 1
 GSR_FLAG_SORTED_KEYS = 2
 GSR_FLAG_TIGHT_TILES = 4
@@ -67,7 +75,7 @@ EXPORTS = ("gsr_abi_version", "gsr_last_error", "gsr_geom_bytes", "gsr_binning_b
            "gsr_pack_frame", "gsr_activate_gaussians", "gsr_set_option", "gsr_backward_multi", "gsr_activate_gaussians_backward",
            "gsr_sugar_normals", "gsr_sugar_normals_backward", "gsr_sugar_colors", "gsr_sugar_colors_backward", "gsr_knn_bytes", "gsr_knn",
            "gsr_sugar_field_bytes", "gsr_sugar_field", "gsr_sugar_field_backward", "gsr_sugar_sdf_normal_bytes", "gsr_sugar_sdf_normal",
-           "gsr_sugar_sdf_normal_backward")
+           "gsr_sugar_sdf_normal_backward", "gsr_densify_stats", "gsr_densify_plan_bytes", "gsr_densify_plan", "gsr_densify_apply")
 
 
 def _load() -> C.CDLL:
@@ -89,7 +97,7 @@ def _load() -> C.CDLL:
         raise ImportError("autovfx_b200: ABI mismatch, rebuild with `python -m autovfx_b200.build --force`")
     lib.gsr_last_error.restype = C.c_char_p
     for n in ("gsr_geom_bytes", "gsr_image_bytes", "gsr_binning_bytes", "gsr_binning_capacity", "gsr_dist2_bytes", "gsr_knn_bytes",
-              "gsr_sugar_field_bytes", "gsr_sugar_sdf_normal_bytes"):
+              "gsr_sugar_field_bytes", "gsr_sugar_sdf_normal_bytes", "gsr_densify_plan_bytes"):
         getattr(lib, n).restype = C.c_size_t
     lib.gsr_geom_bytes.argtypes = [C.c_int32]
     lib.gsr_image_bytes.argtypes = [C.c_int32, C.c_int32]
@@ -146,6 +154,14 @@ def _load() -> C.CDLL:
     lib.gsr_sugar_sdf_normal.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 9 + [C.c_void_p, C.c_size_t, C.c_void_p]
     lib.gsr_sugar_sdf_normal_backward.restype = C.c_int
     lib.gsr_sugar_sdf_normal_backward.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 12 + [C.c_void_p, C.c_size_t, C.c_void_p]
+    lib.gsr_densify_stats.restype = C.c_int
+    lib.gsr_densify_stats.argtypes = [C.c_int32] * 2 + [C.c_void_p] * 7
+    lib.gsr_densify_plan_bytes.argtypes = [C.c_int32]
+    lib.gsr_densify_plan.restype = C.c_int
+    lib.gsr_densify_plan.argtypes = ([C.c_int32] + [C.c_void_p] * 4 + [C.c_float] * 3 + [C.c_int32] + [C.c_float] * 2 + [C.c_void_p] * 3 +
+                                     [C.c_size_t, C.c_void_p])
+    lib.gsr_densify_apply.restype = C.c_int
+    lib.gsr_densify_apply.argtypes = ([C.c_int32] * 3 + [C.POINTER(gsr_densify_group)] + [C.c_void_p] * 5 + [C.c_int32, C.c_void_p])
     lib.gsr_get_views.restype = C.c_int
     lib.gsr_get_views.argtypes = [C.POINTER(gsr_workspace), C.c_int32, C.c_int32, C.c_int32, C.POINTER(gsr_views)]
     lib.gsr_profile_begin.restype = C.c_int

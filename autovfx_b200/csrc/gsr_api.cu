@@ -62,6 +62,14 @@ int sugar_sdf_normal_backward_impl(int N, int K, int P, const float* x, const in
                                    const float* scaling, const float* quaternions, const float* opac, const float* g_loss,
                                    const float* g_est, float* dx, float* d_points, float* d_quaternions, void* ws, size_t ws_bytes,
                                    cudaStream_t st);
+int densify_stats_impl(int P, int C, const float* grad, const uint8_t* mask, const int32_t* radii, float* accum, float* denom,
+                       float* max_radii, cudaStream_t st);
+size_t densify_plan_bytes(int P);
+int densify_plan_impl(int P, const float* accum, const float* denom, const float* scaling, const float* opacity, float max_grad,
+                      float dense_thr, float min_opacity, int use_screen, float max_screen_size, float big_thr, int32_t* dst,
+                      int32_t* totals, void* ws, size_t ws_bytes, cudaStream_t st);
+int densify_apply_impl(int P, int S, int n_groups, const gsr_densify_group* groups, const int32_t* dst, const float* xyz,
+                       const float* scaling, const float* rotation, const float* eps, int rotation_mode, cudaStream_t st);
 int profile_begin(int max_frames, int stride);
 int set_option(const char* name, int value);
 int profile_end(float* ms, int* frames);
@@ -240,6 +248,25 @@ int gsr_sugar_sdf_normal_backward(int32_t N, int32_t K, int32_t P, const float* 
     NvtxRange nvtx_("gsr_sugar_sdf_normal_backward");
     return gsr::sugar_sdf_normal_backward_impl(N, K, P, x, gidx, knn_idx, points, scaling, quaternions, opacities, dL_dloss, dL_destimate,
                                                dL_dx, dL_dpoints, dL_dquaternions, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int gsr_densify_stats(int32_t P, int32_t C, const float* grad, const uint8_t* mask, const int32_t* radii, float* accum, float* denom,
+                      float* max_radii2D, void* stream) {
+    NvtxRange nvtx_("gsr_densify_stats");
+    return gsr::densify_stats_impl(P, C, grad, mask, radii, accum, denom, max_radii2D, (cudaStream_t)stream);
+}
+size_t gsr_densify_plan_bytes(int32_t P) { return gsr::densify_plan_bytes(P); }
+int gsr_densify_plan(int32_t P, const float* accum, const float* denom, const float* scaling, const float* opacity, float max_grad,
+                     float dense_thr, float min_opacity, int32_t use_screen, float max_screen_size, float big_thr, int32_t* dst,
+                     int32_t* totals, void* workspace, size_t workspace_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_densify_plan");
+    return gsr::densify_plan_impl(P, accum, denom, scaling, opacity, max_grad, dense_thr, min_opacity, use_screen, max_screen_size,
+                                  big_thr, dst, totals, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int gsr_densify_apply(int32_t P, int32_t S, int32_t n_groups, const gsr_densify_group* groups, const int32_t* dst, const float* xyz,
+                      const float* scaling, const float* rotation, const float* eps, int32_t rotation_mode, void* stream) {
+    NvtxRange nvtx_("gsr_densify_apply");
+    return gsr::densify_apply_impl(P, S, n_groups, groups, dst, xyz, scaling, rotation, eps, rotation_mode, (cudaStream_t)stream);
 }
 
 int gsr_profile_begin(int max_frames) { return gsr::profile_begin(max_frames, 1); }

@@ -15,6 +15,8 @@
  *                               (get_covariance :602-608, get_beta 'average' :1063-1066); gsr_sugar_field_backward their autograd
  *   gsr_sugar_sdf_normal replaces the coarse trainers' better-normal loss and projection estimate
  *                               sugar_trainers/coarse_density.py:704-707, :756-780; gsr_sugar_sdf_normal_backward their autograd
+ *   gsr_densify_stats, gsr_densify_plan, gsr_densify_apply replace the densification bookkeeping of GaussianModel
+ *                               (scene/gaussian_model.py:268-417) and SuGaRDensifier (sugar_scene/sugar_densifier.py:48-246)
  *
  * and, for the render() wrapper around the two rasterizer passes ("GR/" = sugar/gaussian_splatting/gaussian_renderer/__init__.py):
  *
@@ -353,6 +355,58 @@ int gsr_sugar_sdf_normal_backward(int32_t N, int32_t K, int32_t P, const float* 
                                   const float* points, const float* scaling, const float* quaternions, const float* opacities,
                                   const float* dL_dloss, const float* dL_destimate, float* dL_dx, float* dL_dpoints,
                                   float* dL_dquaternions, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Densification statistics (GaussianModel.add_densification_stats plus the trainers' max-radii line, gaussian_model.py:415-417,
+ * train.py:163-164; SuGaRDensifier.update_densification_stats, sugar_densifier.py:156-164).  For every row i < P with mask[i] != 0:
+ *   accum[i] += sqrt(grad[i,0]^2 + grad[i,1]^2)   (grad [P,C], C >= 2: the viewspace points' gradient)
+ *   denom[i] += 1
+ *   max_radii2D[i] = max(max_radii2D[i], float(radii[i]))   (only when both are given; NaN stays)
+ * Other rows are not touched.  No host synchronisation.  P = 0 is a no-op. */
+int gsr_densify_stats(int32_t P, int32_t C, const float* grad, const uint8_t* mask, const int32_t* radii, float* accum, float* denom,
+                      float* max_radii2D, void* stream);
+
+/* The decisions of densify_and_prune (gaussian_model.py:359-413, sugar_densifier.py:186-246) over the P original rows, given
+ * accum [P], denom [P], the raw scaling [P,3] (exp activation) and the raw opacity [P] (sigmoid activation).  Thresholds are the
+ * caller's Python floats rounded to float: max_grad, dense_thr = percent_dense * extent, min_opacity, max_screen_size (used only when
+ * use_screen, the truthiness of the Python value) and big_thr = 0.1 * extent.  With g = accum / denom (NaN -> 0) and m = max(exp(s)):
+ *   clone  = sqrt(g^2) >= max_grad and m <= dense_thr;  split = g >= max_grad and m > dense_thr
+ *   prune  = sigmoid(o) < min_opacity or (use_screen and (0 > max_screen_size or m' > big_thr)), m' = m of the row as it will be
+ *            (split children: scaling log(exp(s) * (1 / 1.6f))); max_radii2D is 0 there, as densification_postfix leaves it.
+ * dst [5,P] (int32) receives, per original row, its destination row in each of the four streams of the final order (surviving
+ * originals, surviving clones, surviving first split copies, surviving second split copies), -1 where there is none, and in row 4
+ * its index among the split-selected rows.  totals [2] (int32, device) receives {S = split-selected rows, P' = rows after}.
+ * `workspace` (16-byte aligned) needs gsr_densify_plan_bytes(P) bytes, else GSR_ERR_WORKSPACE. */
+size_t gsr_densify_plan_bytes(int32_t P);
+int gsr_densify_plan(int32_t P, const float* accum, const float* denom, const float* scaling, const float* opacity, float max_grad,
+                     float dense_thr, float min_opacity, int32_t use_screen, float max_screen_size, float big_thr, int32_t* dst,
+                     int32_t* totals, void* workspace, size_t workspace_bytes, void* stream);
+
+#define GSR_DENSIFY_MAX_GROUPS 8
+enum { GSR_DENSIFY_ROLE_COPY = 0, GSR_DENSIFY_ROLE_XYZ = 1, GSR_DENSIFY_ROLE_SCALING = 2 };
+enum { GSR_DENSIFY_ROTATION_3DGS = 0, GSR_DENSIFY_ROTATION_SUGAR = 1 };
+/* One optimizer parameter group of gsr_densify_apply: the parameter [P,width] -> [P',width] and, when the group has Adam state, its
+ * two moments (both pointers of a moment NULL otherwise). */
+typedef struct gsr_densify_group {
+    const float* src;
+    float* dst;
+    const float* m1_src;
+    float* m1_dst;
+    const float* m2_src;
+    float* m2_dst;
+    int32_t width; /* floats per row (0 allowed) */
+    int32_t role;  /* GSR_DENSIFY_ROLE_*: how split children are written */
+} gsr_densify_group;
+
+/* Writes every row of the new parameters and moments from gsr_densify_plan's dst [5,P]: kept rows and their moments are copied,
+ * clones copied with zero moments, split children (zero moments) copied except
+ *   ROLE_XYZ (width 3):     R(q) (eps * exp(s)) + xyz, eps row k*S + j for copy k of split row j (eps [2S,3] standard normal),
+ *                           R = build_rotation(q) (GSR_DENSIFY_ROTATION_3DGS, general_utils.py:78-99) or pytorch3d
+ *                           quaternion_to_matrix(F.normalize(q)) (GSR_DENSIFY_ROTATION_SUGAR), from the raw xyz [P,3],
+ *                           scaling [P,3] and rotation [P,4]
+ *   ROLE_SCALING (width 3): log(exp(s) * (1 / 1.6f))
+ * n_groups <= GSR_DENSIFY_MAX_GROUPS (host array).  The outputs must not alias the inputs. */
+int gsr_densify_apply(int32_t P, int32_t S, int32_t n_groups, const gsr_densify_group* groups, const int32_t* dst, const float* xyz,
+                      const float* scaling, const float* rotation, const float* eps, int32_t rotation_mode, void* stream);
 
 /* Device pointers into the workspaces of the last layout (P, capacity, W, H) — for parity tests that
  * compare per-stage buffers with the reference (SURVEY §4).  Pure pointer arithmetic, no CUDA calls. */
