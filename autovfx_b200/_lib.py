@@ -75,7 +75,8 @@ EXPORTS = ("gsr_abi_version", "gsr_last_error", "gsr_geom_bytes", "gsr_binning_b
            "gsr_pack_frame", "gsr_activate_gaussians", "gsr_set_option", "gsr_backward_multi", "gsr_activate_gaussians_backward",
            "gsr_sugar_normals", "gsr_sugar_normals_backward", "gsr_sugar_colors", "gsr_sugar_colors_backward", "gsr_knn_bytes", "gsr_knn",
            "gsr_sugar_field_bytes", "gsr_sugar_field", "gsr_sugar_field_backward", "gsr_sugar_sdf_normal_bytes", "gsr_sugar_sdf_normal",
-           "gsr_sugar_sdf_normal_backward", "gsr_densify_stats", "gsr_densify_plan_bytes", "gsr_densify_plan", "gsr_densify_apply")
+           "gsr_sugar_sdf_normal_backward", "gsr_densify_stats", "gsr_densify_plan_bytes", "gsr_densify_plan", "gsr_densify_apply",
+           "gsr_sugar_sample_bytes", "gsr_sugar_sample", "gsr_sugar_sample_backward")
 
 
 def _load() -> C.CDLL:
@@ -97,7 +98,7 @@ def _load() -> C.CDLL:
         raise ImportError("autovfx_b200: ABI mismatch, rebuild with `python -m autovfx_b200.build --force`")
     lib.gsr_last_error.restype = C.c_char_p
     for n in ("gsr_geom_bytes", "gsr_image_bytes", "gsr_binning_bytes", "gsr_binning_capacity", "gsr_dist2_bytes", "gsr_knn_bytes",
-              "gsr_sugar_field_bytes", "gsr_sugar_sdf_normal_bytes", "gsr_densify_plan_bytes"):
+              "gsr_sugar_field_bytes", "gsr_sugar_sdf_normal_bytes", "gsr_densify_plan_bytes", "gsr_sugar_sample_bytes"):
         getattr(lib, n).restype = C.c_size_t
     lib.gsr_geom_bytes.argtypes = [C.c_int32]
     lib.gsr_image_bytes.argtypes = [C.c_int32, C.c_int32]
@@ -162,6 +163,11 @@ def _load() -> C.CDLL:
                                      [C.c_size_t, C.c_void_p])
     lib.gsr_densify_apply.restype = C.c_int
     lib.gsr_densify_apply.argtypes = ([C.c_int32] * 3 + [C.POINTER(gsr_densify_group)] + [C.c_void_p] * 5 + [C.c_int32, C.c_void_p])
+    lib.gsr_sugar_sample_bytes.argtypes = [C.c_int32]
+    lib.gsr_sugar_sample.restype = C.c_int
+    lib.gsr_sugar_sample.argtypes = ([C.c_int32] * 2 + [C.c_float, C.c_int32] + [C.c_void_p] * 10 + [C.c_void_p, C.c_size_t, C.c_void_p])
+    lib.gsr_sugar_sample_backward.restype = C.c_int
+    lib.gsr_sugar_sample_backward.argtypes = [C.c_int32] * 2 + [C.c_float] + [C.c_void_p] * 10
     lib.gsr_get_views.restype = C.c_int
     lib.gsr_get_views.argtypes = [C.POINTER(gsr_workspace), C.c_int32, C.c_int32, C.c_int32, C.POINTER(gsr_views)]
     lib.gsr_profile_begin.restype = C.c_int

@@ -70,6 +70,13 @@ int densify_plan_impl(int P, const float* accum, const float* denom, const float
                       int32_t* totals, void* ws, size_t ws_bytes, cudaStream_t st);
 int densify_apply_impl(int P, int S, int n_groups, const gsr_densify_group* groups, const int32_t* dst, const float* xyz,
                        const float* scaling, const float* rotation, const float* eps, int rotation_mode, cudaStream_t st);
+size_t sugar_sample_bytes(int P);
+int sugar_sample_impl(int N, int P, float f, int volume, const uint8_t* mask, const float* strengths, const double* u, const float* z,
+                      const float* points, const float* scaling, const float* quaternions, float* out_points, int64_t* out_idx,
+                      double* out_total, void* ws, size_t ws_bytes, cudaStream_t st);
+int sugar_sample_backward_impl(int N, int P, float f, const int64_t* idx, const float* z, const float* scaling, const float* quaternions,
+                               const double* total, const float* dL_dsamples, float* d_points, float* d_scaling, float* d_quaternions,
+                               cudaStream_t st);
 int profile_begin(int max_frames, int stride);
 int set_option(const char* name, int value);
 int profile_end(float* ms, int* frames);
@@ -267,6 +274,23 @@ int gsr_densify_apply(int32_t P, int32_t S, int32_t n_groups, const gsr_densify_
                       const float* scaling, const float* rotation, const float* eps, int32_t rotation_mode, void* stream) {
     NvtxRange nvtx_("gsr_densify_apply");
     return gsr::densify_apply_impl(P, S, n_groups, groups, dst, xyz, scaling, rotation, eps, rotation_mode, (cudaStream_t)stream);
+}
+
+size_t gsr_sugar_sample_bytes(int32_t P) { return gsr::sugar_sample_bytes(P); }
+int gsr_sugar_sample(int32_t N, int32_t P, float sampling_scale_factor, int32_t proportional_to_volume, const uint8_t* mask,
+                     const float* strengths, const double* u, const float* z, const float* points, const float* scaling,
+                     const float* quaternions, float* out_samples, int64_t* out_idx, double* out_total, void* workspace,
+                     size_t workspace_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_sugar_sample");
+    return gsr::sugar_sample_impl(N, P, sampling_scale_factor, proportional_to_volume, mask, strengths, u, z, points, scaling, quaternions,
+                                  out_samples, out_idx, out_total, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+int gsr_sugar_sample_backward(int32_t N, int32_t P, float sampling_scale_factor, const int64_t* idx, const float* z, const float* scaling,
+                              const float* quaternions, const double* total, const float* dL_dsamples, float* dL_dpoints,
+                              float* dL_dscaling, float* dL_dquaternions, void* stream) {
+    NvtxRange nvtx_("gsr_sugar_sample_backward");
+    return gsr::sugar_sample_backward_impl(N, P, sampling_scale_factor, idx, z, scaling, quaternions, total, dL_dsamples, dL_dpoints,
+                                           dL_dscaling, dL_dquaternions, (cudaStream_t)stream);
 }
 
 int gsr_profile_begin(int max_frames) { return gsr::profile_begin(max_frames, 1); }

@@ -457,6 +457,47 @@ struct BlendArgs {
 void launch_blend_lists(const BlendArgs& a, cudaStream_t st);
 __host__ __device__ inline size_t bal_row_base(uint32_t range_x, int tile) { return (size_t)(range_x >> 5) + (size_t)tile; }
 
+// Exclusive scan of n entries in place, one CTA of 1024 threads: uint32_t for the radix sort of gsr_knn / gsr_dist2 and for
+// gsr_densify_plan, double for the prefix sums of gsr_sugar_sample.  Internal linkage: each translation unit has its own copy.
+namespace {
+template <typename T>
+__global__ void __launch_bounds__(1024) k_rs_scan(T* hist, int n) {
+    __shared__ T wsum[32];
+    __shared__ T carry;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) carry = T(0);
+    __syncthreads();
+    for (int base = 0; base < n; base += 1024) {
+        const int i = base + tid;
+        const T v = i < n ? hist[i] : T(0);
+        T incl = v;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const T t = __shfl_up_sync(GSR_FULL, incl, o);
+            if (lane >= o) incl += t;
+        }
+        if (lane == 31) wsum[warp] = incl;
+        __syncthreads();
+        if (warp == 0) {
+            const T s = wsum[lane];
+            T si = s;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const T t = __shfl_up_sync(GSR_FULL, si, o);
+                if (lane >= o) si += t;
+            }
+            wsum[lane] = si - s;
+        }
+        __syncthreads();
+        const T excl = carry + wsum[warp] + incl - v;
+        if (i < n) hist[i] = excl;
+        __syncthreads();
+        if (tid == 1023) carry = excl + v;
+        __syncthreads();
+    }
+}
+}  // namespace
+
 void set_error(const char* fmt, ...);
 const char* last_error();
 int check_launch(const char* what, bool debug, cudaStream_t stream);

@@ -5,7 +5,7 @@
 //   k_plan_flags       the reference's clone, split and final-prune decisions for every original row, as 5 bits per row
 //                      (original kept, clone kept, first split copy kept, second split copy kept, split-selected), and the
 //                      per-block count of each bit.
-//   k_rs_scan          (gsr_knn.cu) exclusive scan of the counts, laid out stream-major: the destination of every kept row in
+//   k_rs_scan          (gsr_common.cuh) exclusive scan of the counts, laid out stream-major: the destination of every kept row in
 //                      the reference's final order (originals, clones, first copies, second copies) and the split indices.
 //   k_plan_offsets     per-row destinations (-1: no row) and the totals {S, P'}.
 //   k_densify_apply    one pass over every element of every parameter group and both Adam moments: kept rows copied with
@@ -16,8 +16,6 @@
 #include "gsr_common.cuh"
 
 namespace gsr {
-
-__global__ void k_rs_scan(uint32_t* hist, int n);  // gsr_knn.cu
 
 namespace {
 

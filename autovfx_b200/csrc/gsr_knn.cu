@@ -123,41 +123,6 @@ __global__ void __launch_bounds__(RS_WARPS * 32) k_rs_hist(int P, const uint32_t
         for (int d = lane; d < 256; d += 32) hist[(size_t)d * nchunks + chunk] = cnt[warp][d];
     }
 }
-__global__ void __launch_bounds__(1024) k_rs_scan(uint32_t* hist, int n) {  // exclusive scan of n entries, one CTA
-    __shared__ uint32_t wsum[32];
-    __shared__ uint32_t carry;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) carry = 0;
-    __syncthreads();
-    for (int base = 0; base < n; base += 1024) {
-        const int i = base + tid;
-        const uint32_t v = i < n ? hist[i] : 0;
-        uint32_t incl = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t t = __shfl_up_sync(GSR_FULL, incl, o);
-            if (lane >= o) incl += t;
-        }
-        if (lane == 31) wsum[warp] = incl;
-        __syncthreads();
-        if (warp == 0) {
-            const uint32_t s = wsum[lane];
-            uint32_t si = s;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const uint32_t t = __shfl_up_sync(GSR_FULL, si, o);
-                if (lane >= o) si += t;
-            }
-            wsum[lane] = si - s;
-        }
-        __syncthreads();
-        const uint32_t excl = carry + wsum[warp] + incl - v;
-        if (i < n) hist[i] = excl;
-        __syncthreads();
-        if (tid == 1023) carry = excl + v;
-        __syncthreads();
-    }
-}
 __global__ void __launch_bounds__(RS_WARPS * 32) k_rs_scatter(int P, const uint32_t* __restrict__ keys, const uint32_t* __restrict__ vals,
                                                               int shift, int nchunks, const uint32_t* __restrict__ hist,
                                                               uint32_t* __restrict__ keys_out, uint32_t* __restrict__ vals_out) {

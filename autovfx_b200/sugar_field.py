@@ -15,6 +15,11 @@ The coarse trainers' projection estimate and better-normal loss ("CD/" = sugar/s
     sdf_estimation = projection_estimate(sugar, sdf_samples, sdf_gaussian_idx)
     sdf_better_normal_loss = better_normal_loss(sugar, sdf_samples, sdf_gaussian_idx, fields['closest_gaussian_opacities'])
 
+SuGaR's sampler of the SDF-regularisation points (SS/:757-799) runs through ``gsr_sugar_sample`` / ``gsr_sugar_sample_backward``::
+
+    from autovfx_b200.sugar_field import sample_points_in_gaussians
+    SuGaR.sample_points_in_gaussians = sample_points_in_gaussians
+
 The model is read through its getters (``points``, ``scaling``, ``quaternions``, ``strengths``, ``knn_idx``, ``beta_mode``), so
 autograd carries the gradients of x and of the getters' outputs back to the raw parameters.  No [N,K,3,3] tensor is built: the
 kernels gather one 64-byte record per (sample, neighbour) pair and recompute everything in the backward.
@@ -26,7 +31,8 @@ import torch
 
 from . import _lib
 
-__all__ = ["get_field_values", "compute_density", "projection_estimate", "better_normal_loss", "FIELD_MAX_K"]
+__all__ = ["get_field_values", "compute_density", "projection_estimate", "better_normal_loss", "sample_points_in_gaussians",
+           "FIELD_MAX_K"]
 
 FIELD_MAX_K = 32
 
@@ -328,3 +334,105 @@ def better_normal_loss(self, sdf_samples, sdf_gaussian_idx, closest_gaussian_opa
     Raises ValueError, naming the argument, for wrong shapes, dtypes or widths (the opacities' K must equal knn_idx's), K outside
     1..32 and a model bound to a surface mesh; RuntimeError for CPU tensors (there is no CPU path)."""
     return _sdf_normal("better_normal_loss", self, sdf_samples, sdf_gaussian_idx, closest_gaussian_opacities, True)
+
+
+# ------------------------------------------------------------------------------------------------ SDF-regularisation samples
+def _sample_forward(N, f, volume, mask, strengths, u, z, points, scaling, quaternions):
+    dev, P = points.device, points.shape[0]
+    out = torch.empty((N, 3), dtype=torch.float32, device=dev)
+    idx = torch.empty(N, dtype=torch.int64, device=dev)
+    total = torch.empty(1, dtype=torch.float64, device=dev)
+    L = _lib_handle()
+    nbytes = L.gsr_sugar_sample_bytes(P)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    rc = L.gsr_sugar_sample(N, P, f, int(volume), _ptr(mask), _ptr(strengths), u.data_ptr(), z.data_ptr(), points.data_ptr(),
+                            scaling.data_ptr(), quaternions.data_ptr(), out.data_ptr(), idx.data_ptr(), total.data_ptr(),
+                            ws.data_ptr(), nbytes, _lib.stream_ptr(dev))
+    _lib.check(rc, "gsr_sugar_sample")
+    return out, idx, total
+
+
+class _SugarSample(torch.autograd.Function):
+    """Outputs: the samples [N,3] (differentiable with respect to points, scaling and quaternions) and their rows [N]."""
+
+    @staticmethod
+    def forward(ctx, points, scaling, quaternions, N, f, volume, mask, strengths, u, z):
+        ctx.set_materialize_grads(False)
+        out, idx, total = _sample_forward(N, f, volume, mask, strengths, u, z, points, scaling, quaternions)
+        ctx.f = f
+        ctx.mark_non_differentiable(idx)
+        ctx.save_for_backward(scaling, quaternions, z, idx, total)
+        return out, idx
+
+    @staticmethod
+    def backward(ctx, g, _g_idx):
+        scaling, quaternions, z, idx, total = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        if g is None:
+            return (None,) * 10
+        g = g.contiguous()
+        N, P = idx.shape[0], scaling.shape[0]
+        d_points = torch.empty((P, 3), dtype=torch.float32, device=g.device)
+        d_scaling = torch.empty((P, 3), dtype=torch.float32, device=g.device)
+        d_quaternions = torch.empty((P, 4), dtype=torch.float32, device=g.device)
+        rc = _lib_handle().gsr_sugar_sample_backward(N, P, ctx.f, idx.data_ptr(), z.data_ptr(), scaling.data_ptr(),
+                                                     quaternions.data_ptr(), total.data_ptr(), g.data_ptr(), d_points.data_ptr(),
+                                                     d_scaling.data_ptr(), d_quaternions.data_ptr(), _lib.stream_ptr(g.device))
+        _lib.check(rc, "gsr_sugar_sample_backward")
+        return (d_points if need[0] else None, d_scaling if need[1] else None, d_quaternions if need[2] else None,
+                None, None, None, None, None, None, None)
+
+
+def sample_points_in_gaussians(self, num_samples, sampling_scale_factor=1., mask=None, probabilities_proportional_to_opacity=False,
+                               probabilities_proportional_to_volume=True):
+    """SuGaR.sample_points_in_gaussians (SS/:757-799) in CUDA: (random_points [N,3] float32, random_indices [N] int64), the indices
+    being rows of the model (as after SuGaR's valid_indices[...]).  Selected rows are mask's True rows (all rows when mask is None);
+    a selected row's weight w is |s0 * s1 * s2| (or 1 without probabilities_proportional_to_volume), times strengths with
+    probabilities_proportional_to_opacity.  As in SuGaR, whose torch.multinomial is handed cumsum(w) / sum(w) as the weights,
+    selected row k is drawn with probability proportional to the cumulative weight C_k = sum of w up to k (float64 here).  Each
+    sample is points[i] + quaternion_apply(quaternions[i], (sampling_scale_factor * scaling[i]) * z), z ~ N(0, 1)^3, pytorch3d's
+    quaternion_apply op for op.  random_points is differentiable with respect to the getters' points, scaling and quaternions; the
+    weights get no gradient.
+
+    The draws come from the CUDA generator of the points' device, in this order: u = torch.rand(N, dtype=float64) (row i is the
+    first whose float64 prefix of C over the selected rows exceeds u * total), then z = torch.randn(N, 3).  torch.manual_seed
+    controls a run; the samples for a seed differ from SuGaR's (which draws through torch.multinomial), the distribution is the
+    same.  Nothing is read back to the host.  An empty selection, or a zero or non-finite total, gives index 0 and NaN samples
+    (SuGaR asserts on the device; its trainers call it only when the mask has a True row).
+
+    Raises ValueError, naming the argument, for num_samples < 1, a wrong shape or dtype (float32 getters, a bool mask [P]) or a
+    model without rows; RuntimeError for CPU tensors (there is no CPU path)."""
+    who = "sample_points_in_gaussians"
+    if isinstance(num_samples, bool) or not isinstance(num_samples, (int, np.integer)) or num_samples < 1:
+        raise ValueError("%s: num_samples must be an int >= 1, got %r" % (who, num_samples))
+    if isinstance(sampling_scale_factor, bool) or not isinstance(sampling_scale_factor, (int, float)):
+        raise ValueError("%s: sampling_scale_factor must be a Python number, got %r" % (who, sampling_scale_factor))
+    points, scaling, quaternions = self.points, self.scaling, self.quaternions
+    _check_tensor(who, "self.points", points, (None, 3), torch.float32)
+    P = points.shape[0]
+    if P < 1:
+        raise ValueError("%s: self.points has no rows" % who)
+    _check_tensor(who, "self.scaling", scaling, (P, 3), torch.float32)
+    _check_tensor(who, "self.quaternions", quaternions, (P, 4), torch.float32)
+    strengths = None
+    if probabilities_proportional_to_opacity:
+        strengths = self.strengths
+        if not isinstance(strengths, torch.Tensor) or strengths.shape not in ((P, 1), (P,)):
+            raise ValueError("%s: self.strengths must have shape [%d, 1], got %s" % (who, P, getattr(strengths, "shape", None)))
+        _check_tensor(who, "self.strengths", strengths, tuple(strengths.shape), torch.float32)
+        strengths = strengths.detach().reshape(P).contiguous()
+    if mask is not None:
+        _check_tensor(who, "mask", mask, (P,), torch.bool)
+    _require_cuda(who, points, scaling, quaternions, strengths, mask)
+    N = int(num_samples)
+    f = float(sampling_scale_factor)
+    dev = points.device
+    mask = None if mask is None else mask.contiguous()
+    ins = [t.contiguous() for t in (points, scaling, quaternions)]
+    with torch.cuda.device(dev):
+        u = torch.rand(N, dtype=torch.float64, device=dev)
+        z = torch.randn((N, 3), dtype=torch.float32, device=dev)
+        if torch.is_grad_enabled() and any(t.requires_grad for t in ins):
+            return _SugarSample.apply(*ins, N, f, bool(probabilities_proportional_to_volume), mask, strengths, u, z)
+        out, idx, _ = _sample_forward(N, f, probabilities_proportional_to_volume, mask, strengths, u, z, *ins)
+        return out, idx

@@ -17,6 +17,8 @@
  *                               sugar_trainers/coarse_density.py:704-707, :756-780; gsr_sugar_sdf_normal_backward their autograd
  *   gsr_densify_stats, gsr_densify_plan, gsr_densify_apply replace the densification bookkeeping of GaussianModel
  *                               (scene/gaussian_model.py:268-417) and SuGaRDensifier (sugar_scene/sugar_densifier.py:48-246)
+ *   gsr_sugar_sample  replaces  SuGaR.sample_points_in_gaussians               sugar_scene/sugar_model.py:757-799;
+ *                               gsr_sugar_sample_backward its autograd backward
  *
  * and, for the render() wrapper around the two rasterizer passes ("GR/" = sugar/gaussian_splatting/gaussian_renderer/__init__.py):
  *
@@ -355,6 +357,35 @@ int gsr_sugar_sdf_normal_backward(int32_t N, int32_t K, int32_t P, const float* 
                                   const float* points, const float* scaling, const float* quaternions, const float* opacities,
                                   const float* dL_dloss, const float* dL_destimate, float* dL_dx, float* dL_dpoints,
                                   float* dL_dquaternions, void* workspace, size_t workspace_bytes, void* stream);
+
+/* SuGaR.sample_points_in_gaussians (sugar_model.py:757-799) given its random draws: N samples among P >= 1 Gaussians given by
+ * SuGaR's getters, points [P,3], scaling [P,3], quaternions [P,4] (as the getters return them).  A row is selected where mask [P]
+ * (bool bytes) is non-zero, every row when mask is NULL.  A selected row's weight is w = |s0 * s1 * s2| (float32, left to right) when
+ * proportional_to_volume, else 1, times strengths [P] when strengths is not NULL (proportional to opacity).  As in SuGaR, whose
+ * torch.multinomial receives cumsum(w) / sum(w) as the weights, selected row k is drawn with probability proportional to
+ * C_k = sum of w over the selected rows up to k.  In float64, with T_i = sum_{j <= i, j selected} C_j and total = T_{P-1}:
+ *   out_idx     [N] (int64) = the first row i whose T_i exceeds u[n] * total (capped below the total); a row of zero C or an
+ *                             unselected row is never returned.  u [N] (float64) is uniform in [0, 1).
+ *   out_samples [N,3]       = points[i] + quaternion_apply(quaternions[i], (sampling_scale_factor * scaling[i]) * z[n]), pytorch3d's
+ *                             raw_multiply(raw_multiply(q, (0, v)), conjugate(q)) op for op in float32 (a non-unit q scales by |q|^2).
+ *                             z [N,3] (float32) is standard normal.
+ *   out_total   [1] (float64) = total, for the backward.
+ * No host synchronisation.  When the total is zero (an empty selection), infinite or NaN, every index is 0 and every sample NaN.
+ * N = 0 is a no-op.  N < 0, P < 1 or a missing pointer other than mask and strengths is GSR_ERR_INVALID; `workspace` (16-byte
+ * aligned) needs gsr_sugar_sample_bytes(P) bytes, else GSR_ERR_WORKSPACE. */
+size_t gsr_sugar_sample_bytes(int32_t P);
+int gsr_sugar_sample(int32_t N, int32_t P, float sampling_scale_factor, int32_t proportional_to_volume, const uint8_t* mask,
+                     const float* strengths, const double* u, const float* z, const float* points, const float* scaling,
+                     const float* quaternions, float* out_samples, int64_t* out_idx, double* out_total, void* workspace,
+                     size_t workspace_bytes, void* stream);
+
+/* Backward of gsr_sugar_sample (same N, P, factor, z, scaling and quaternions; idx and total as it wrote them): the gradient of the
+ * samples dL_dsamples [N,3] in, dL_dpoints [P,3], dL_dscaling [P,3] and dL_dquaternions [P,4] out (required, written in full; the
+ * per-sample terms are added with atomics, so the summation order is not fixed).  The weights get no gradient, as through
+ * torch.multinomial.  When the total is zero, infinite or NaN the gradients are zero. */
+int gsr_sugar_sample_backward(int32_t N, int32_t P, float sampling_scale_factor, const int64_t* idx, const float* z, const float* scaling,
+                              const float* quaternions, const double* total, const float* dL_dsamples, float* dL_dpoints,
+                              float* dL_dscaling, float* dL_dquaternions, void* stream);
 
 /* Densification statistics (GaussianModel.add_densification_stats plus the trainers' max-radii line, gaussian_model.py:415-417,
  * train.py:163-164; SuGaRDensifier.update_densification_stats, sugar_densifier.py:156-164).  For every row i < P with mask[i] != 0:
