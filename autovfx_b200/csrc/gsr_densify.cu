@@ -11,7 +11,7 @@
 //   k_densify_apply    one pass over every element of every parameter group and both Adam moments: kept rows copied with
 //                      their moments, new rows (clones, split children) written with zero moments.
 //
-// The decisions use torch's float32 roundings op by op: grads = accum / denom, norm = sqrt(g * g), exp and sigmoid as ATen
+// The decisions use torch's float32 roundings op by op: grads = accum / denom, norm = |g|, exp and sigmoid as ATen
 // evaluates them (sigmoid = 1 / (1 + exp(-x))), maxima that propagate NaN, thresholds rounded to float by the caller.
 #include "gsr_common.cuh"
 
@@ -59,7 +59,8 @@ __global__ void __launch_bounds__(PLAN_BLOCK) k_plan_flags(PlanArgs a) {
         if (g != g) g = 0.0f;
         const float s0 = a.scaling[3 * (size_t)i], s1 = a.scaling[3 * (size_t)i + 1], s2 = a.scaling[3 * (size_t)i + 2];
         const float mx = max3_exp(s0, s1, s2);
-        const bool clone = __fsqrt_rn(__fmul_rn(g, g)) >= a.max_grad && mx <= a.dense_thr;
+        // torch.norm over grads' single column is |g|: no rounded square, which would underflow for |g| < 1.1e-19
+        const bool clone = fabsf(g) >= a.max_grad && mx <= a.dense_thr;
         const bool split = g >= a.max_grad && mx > a.dense_thr;
         const float op = __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-a.opacity[i])));
         // the final prune sees max_radii2D = 0 (densification_postfix reset it)

@@ -113,7 +113,9 @@ __global__ void __launch_bounds__(256) k_sample_points(SampleArgs a) {
     int i = 0;
     if (ok) {
         double x = a.u[n] * total;
-        if (!(x < total)) x = nextafter(total, 0.0);  // u * total can round up to the total when u is within an ulp of 1
+        // a guard only: for u < 1, fl(u * total) < total whenever the total is a normal float64, and a total built from float32
+        // weights is at least 1.4e-45, far above float64's subnormal range
+        if (!(x < total)) x = nextafter(total, 0.0);
         int lo = 0, hi = a.P - 1;                      // |T[P-1]| = total > x: the first crossing is at most P-1
         while (lo < hi) {
             const int mid = (lo + hi) >> 1;

@@ -95,7 +95,7 @@ def plan_map(accum, denom, scaling, opacity, max_grad, min_opacity, extent, max_
     g = torch.where(g.isnan(), torch.zeros_like(g), g)
     mx = torch.exp(scaling).max(dim=1).values
     f32 = lambda x: torch.tensor(x, dtype=torch.float64).float().item()  # noqa: E731
-    clone = (torch.sqrt(g * g) >= f32(max_grad)) & (mx <= f32(percent_dense * extent))
+    clone = (torch.norm(g[:, None], dim=-1) >= f32(max_grad)) & (mx <= f32(percent_dense * extent))
     split = (g >= f32(max_grad)) & (mx > f32(percent_dense * extent))
     low = torch.sigmoid(opacity.reshape(P)) < f32(min_opacity)
     child = torch.log(torch.exp(scaling) * (1.0 / torch.tensor(1.6, dtype=torch.float32)))
