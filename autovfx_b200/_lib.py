@@ -67,6 +67,7 @@ GSR_FLAG_REUSE_GEOMETRY = 8
 GSR_FLAG_EXACT_IMAGES = 16
 GSR_FLAG_BINNING_ONLY = 32
 GSR_FLAG_RESUME = 64
+GSR_SLAB_SHIFT = 16
 ABI_VERSION = 4
 
 EXPORTS = ("gsr_abi_version", "gsr_last_error", "gsr_geom_bytes", "gsr_binning_bytes", "gsr_binning_capacity", "gsr_image_bytes",
@@ -76,7 +77,7 @@ EXPORTS = ("gsr_abi_version", "gsr_last_error", "gsr_geom_bytes", "gsr_binning_b
            "gsr_sugar_normals", "gsr_sugar_normals_backward", "gsr_sugar_colors", "gsr_sugar_colors_backward", "gsr_knn_bytes", "gsr_knn",
            "gsr_sugar_field_bytes", "gsr_sugar_field", "gsr_sugar_field_backward", "gsr_sugar_sdf_normal_bytes", "gsr_sugar_sdf_normal",
            "gsr_sugar_sdf_normal_backward", "gsr_densify_stats", "gsr_densify_plan_bytes", "gsr_densify_plan", "gsr_densify_apply",
-           "gsr_sugar_sample_bytes", "gsr_sugar_sample", "gsr_sugar_sample_backward")
+           "gsr_sugar_sample_bytes", "gsr_sugar_sample", "gsr_sugar_sample_backward", "gsr_binning_bytes_slab", "gsr_binning_capacity_slab")
 
 
 def _load() -> C.CDLL:
@@ -104,6 +105,9 @@ def _load() -> C.CDLL:
     lib.gsr_image_bytes.argtypes = [C.c_int32, C.c_int32]
     lib.gsr_binning_bytes.argtypes = [C.c_size_t]
     lib.gsr_binning_capacity.argtypes = [C.c_size_t]
+    for n in ("gsr_binning_bytes_slab", "gsr_binning_capacity_slab"):
+        getattr(lib, n).restype = C.c_size_t
+        getattr(lib, n).argtypes = [C.c_size_t, C.c_int32, C.c_int32, C.c_int32]
     lib.gsr_dist2_bytes.argtypes = [C.c_int32]
     lib.gsr_forward.restype = C.c_int
     lib.gsr_forward.argtypes = [C.POINTER(gsr_frame), C.POINTER(gsr_workspace), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -99,6 +99,16 @@ const char* gsr_last_error(void) { return gsr::last_error(); }
 size_t gsr_geom_bytes(int32_t P) { return gsr::GeomLayout((size_t)(P < 0 ? 0 : P)).total; }
 size_t gsr_binning_bytes(size_t capacity) { return gsr::BinLayout(capacity < 1 ? 1 : capacity).total; }
 size_t gsr_binning_capacity(size_t bytes) { return gsr::BinLayout::capacity_of(bytes); }
+size_t gsr_binning_bytes_slab(size_t capacity, int32_t W, int32_t H, int32_t slab_stride) {
+    if (slab_stride <= 0) return gsr_binning_bytes(capacity);
+    const gsr::ImageLayout il(W < 1 ? 1 : W, H < 1 ? 1 : H);
+    return gsr::BinLayout::bytes_with_slab(capacity < 1 ? 1 : capacity, (size_t)il.tiles * (size_t)slab_stride);
+}
+size_t gsr_binning_capacity_slab(size_t bytes, int32_t W, int32_t H, int32_t slab_stride) {
+    if (slab_stride <= 0) return gsr_binning_capacity(bytes);
+    const gsr::ImageLayout il(W < 1 ? 1 : W, H < 1 ? 1 : H);
+    return gsr::BinLayout::slab_offset(gsr::BinLayout::capacity_of(bytes), (size_t)il.tiles * (size_t)slab_stride) / 8;
+}
 size_t gsr_image_bytes(int32_t W, int32_t H) { return gsr::ImageLayout(W < 1 ? 1 : W, H < 1 ? 1 : H).total; }
 
 int gsr_forward(const gsr_frame* frame, const gsr_workspace* ws, float* out_color, float* out_depth, float* out_alpha,

@@ -67,6 +67,11 @@ struct BinLayout {
     }
     __host__ __device__ static size_t fixed_bytes() { return 32 * (size_t)GSR_BAL_SLACK_TILES + 512; }
     __host__ __device__ static size_t capacity_of(size_t bytes) { return bytes > fixed_bytes() ? (bytes - fixed_bytes()) / 13 : 0; }
+    // Slab emission (slab stride S > 0): `slots` = tiles x S pairs occupy the END of the pairs region, 256-byte aligned, so the
+    // offsets of every region stay a function of the workspace size alone (the backward and gsr_get_views do not know S).  The
+    // compact capacity is what lies below the slab; 0 if the slab does not fit.
+    __host__ __device__ static size_t slab_offset(size_t cap, size_t slots) { return slots < cap ? (8 * (cap - slots)) & ~(size_t)255 : 0; }
+    __host__ __device__ static size_t bytes_with_slab(size_t cap, size_t slots) { return BinLayout(cap + slots + 32).total; }
 };
 
 // ---- camera block staged in shared memory ------------------------------------------------------------
@@ -295,6 +300,41 @@ __device__ __forceinline__ uint32_t strip_tile_mask(const StripCtx& s, int tx, i
     }
     return mask;
 }
+// The emission's masks (k_emit, and k_project on the slab path; both must produce the same bits): the rows [ylo, yhi] the two
+// strips of tile column tx cover, as bit masks over the (at most 32) 4-row bands from row Y0 = 16 ty_lo down: band k = rows
+// [Y0 + 4k, Y0 + 4k + 3] is touched iff ylo <= Y0 + 4k + 3 and yhi >= Y0 + 4k, i.e. ceil((ylo - Y0 - 3) / 4) <= k <= floor((yhi - Y0) / 4).
+// Two conversions per strip instead of eight comparisons per tile; near a band boundary the subtractions are exact (Y0 is an
+// integer within a factor two of y), and the strips carry a 0.01-pixel margin anyway.  strips = s.ok && !s.none.
+__device__ __forceinline__ void column_bands(const StripCtx& s, bool strips, int tx, int ty_lo, uint32_t& bands0, uint32_t& bands1) {
+    float ylo0 = 0.f, yhi0 = 0.f, ylo1 = 0.f, yhi1 = 0.f;
+    bool v0 = false, v1 = false;
+    if (strips) {
+        v0 = strip_rows(s, (float)(tx * GSR_TILE), 8.f, ylo0, yhi0);
+        v1 = strip_rows(s, (float)(tx * GSR_TILE + 8), 8.f, ylo1, yhi1);
+    }
+    const float Y0 = (float)(ty_lo * GSR_TILE);
+    auto band_bits = [&](const bool v, const float ylo, const float yhi) -> uint32_t {
+        const float a = fminf(fmaxf((ylo - Y0 - 3.f) * 0.25f, -1.f), 33.f), b = fminf(fmaxf((yhi - Y0) * 0.25f, -1.f), 33.f);
+        const int klo = max((int)ceilf(a), 0), khi = min((int)floorf(b), 31);
+        return (v && klo <= khi) ? (0xffffffffu >> (31 - khi)) & (0xffffffffu << klo) : 0u;
+    };
+    bands0 = band_bits(v0, ylo0, yhi0);
+    bands1 = band_bits(v1, ylo1, yhi1);
+}
+// footprint mask of the tile r rows below ty_lo: its four bands of both strips, interleaved (bit 2q + i = band q of strip i)
+__device__ __forceinline__ uint32_t bands_tile_mask(uint32_t bands0, uint32_t bands1, int r) {
+    uint32_t n0 = (bands0 >> (4 * r)) & 15u, n1 = (bands1 >> (4 * r)) & 15u;
+    n0 = (n0 | (n0 << 2)) & 0x33u; n0 = (n0 | (n0 << 1)) & 0x55u;
+    n1 = (n1 | (n1 << 2)) & 0x33u; n1 = (n1 | (n1 << 1)) & 0x55u;
+    return n0 | (n1 << 1);
+}
+// strip context of a splat over its whole tile rectangle [x0, x1) x [y0, y1) (the margins bound |x - px|, |y - py| over it)
+__device__ __forceinline__ StripCtx rect_strip_ctx(float px, float py, float a, float b, float c, float tau, int x0, int y0, int x1, int y1) {
+    const float um = fmaxf(px - (float)(x0 * GSR_TILE), (float)(x1 * GSR_TILE) - px);
+    const float vm = fmaxf(py - (float)(y0 * GSR_TILE), (float)(y1 * GSR_TILE) - py);
+    return strip_ctx(px, py, a, b, c, tau, um, vm);
+}
+
 // one (splat, tile) pair, any conic
 __device__ __forceinline__ uint32_t tile_foot_mask_any(float px, float py, float a, float b, float c, float tau, int tx, int ty) {
     const float um = fabsf(px - ((float)(tx * GSR_TILE) + 7.5f)) + 7.5f, vm = fabsf(py - ((float)(ty * GSR_TILE) + 7.5f)) + 7.5f;

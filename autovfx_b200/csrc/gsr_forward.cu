@@ -7,8 +7,11 @@
 // Pipeline (results are identical, see DESIGN.md):
 //   k_project     every Gaussian: near cull, conservative screen test, EWA projection, radius, tile rectangle, ranked per-tile
 //                 tickets, SH -> RGB from a TMA-staged row, the whole record, the compact list of visible Gaussians;
-//   k_tile_scan   exclusive scan over the tiles: ranges, R and the overflow flag stay on the device (no host round trip);
-//   k_emit        every VISIBLE Gaussian: one (depth bits, id, footprint mask) pair per (Gaussian, tile) scattered to
+//                 with a slab stride S (GSR_SLAB_SHIFT, packed keys, no tight tiles) it also writes every (depth bits, id, footprint mask) pair
+//                 straight into its tile's slab, slab[tile * S + ticket], and k_emit does not run;
+//   k_tile_scan   exclusive scan over the tiles: ranges, R and the overflow flag (R > capacity, or max_tile > S) stay on the device
+//                 (no host round trip);
+//   k_emit        (no slab) every VISIBLE Gaussian: one (depth bits, id, footprint mask) pair per (Gaussian, tile) scattered to
 //                 ranges[tile].x + rank;
 //   k_sort_tiles  one CTA per tile sorts its bucket by (depth bits, id) — exactly the order of the reference's stable radix sort
 //                 of (tile | depth) keys, because the reference emits every (tile, Gaussian) pair once in ascending Gaussian id
@@ -59,6 +62,8 @@ struct PreParams {
     uint32_t* ranks;
     uint32_t* vis_list;
     gsr_counters* counters;
+    unsigned long long* slab;  // non-null: write the sort pairs to slab[tile * slab_stride + ticket] (no ranks, no k_emit)
+    uint32_t slab_stride;
 };
 
 constexpr int PRE_THREADS = 128;
@@ -424,7 +429,8 @@ __global__ void __launch_bounds__(PRE_THREADS, 8) k_project(const PreParams p) {
             }
         }
     }
-    {
+    const bool slab = !TIGHT && p.slab != nullptr;  // grid-uniform; tight tiles keep the ranked emission (measured faster)
+    if (!slab) {
         const bool big = rect_n > 8;
         uint32_t* tb = p.tile_big;
         if (TIGHT) {
@@ -466,7 +472,7 @@ __global__ void __launch_bounds__(PRE_THREADS, 8) k_project(const PreParams p) {
             rec[1] = make_float4(con_c, opacity, depth, __int_as_float(radius));
             rec[2] = make_float4(rgb[0], rgb[1], rgb[2], log2f(opacity));  // .w: log2(opacity) for the default blend
             if (p.for_backward) p.clamped[idx] = (uint8_t)clamp_bits;
-            if (rect_n <= 8) {
+            if (rect_n <= 8 && !slab) {
                 uint4* rr = reinterpret_cast<uint4*>(p.ranks + 8 * (size_t)idx);
                 rr[0] = make_uint4(rk[0], rk[1], rk[2], rk[3]);
                 if (rect_n > 4) rr[1] = make_uint4(rk[4], rk[5], rk[6], rk[7]);
@@ -476,6 +482,53 @@ __global__ void __launch_bounds__(PRE_THREADS, 8) k_project(const PreParams p) {
                 for (int k = 0; k < 6; k++) p.cov3D[6 * (size_t)idx + k] = c3[k];
             }
         }
+    }
+    if (slab) {
+        // Emission (what k_emit does on the ranked path), after the record store so that the SH staging registers are dead: one
+        // (depth bits, id << 8 | footprint mask) pair per (Gaussian, tile) at slab[tile * S + ticket].  k_sort_tiles orders each
+        // tile by the whole key, so the arrival order of the tickets does not matter.  A ticket >= S writes nothing; the count
+        // still rises, k_tile_scan's max_tile exceeds S and the frame reports an overflow.
+        const uint32_t S = p.slab_stride, lo_id = (uint32_t)idx << 8, dbits = __float_as_uint(depth);
+        const StripCtx sc = rect_n > 0 ? rect_strip_ctx(px, py, con_a, con_b, con_c, tau, x0, y0, x1, y1) : StripCtx{};
+        if (rect_n > 0 && rect_n <= 8) {  // the tickets drawn above, column-major like the ticket loop
+            uint32_t b0 = 0, b1 = 0;
+            int tx = x0, ty = y0;
+#pragma unroll
+            for (int k = 0; k < 8; k++) {
+                if (k < rect_n) {
+                    if (ty == y0) column_bands(sc, sc.ok && !sc.none, tx, y0, b0, b1);
+                    if (rk[k] < S) {
+                        const uint32_t mask = sc.ok ? bands_tile_mask(b0, b1, ty - y0) : tile_foot_mask(px, py, con_a, con_b, con_c, tau, tx, ty);
+                        p.slab[(size_t)(ty * p.gx + tx) * S + rk[k]] = ((unsigned long long)dbits << 32) | (lo_id | mask);
+                    }
+                    if (++ty == y1) { ty = y0; tx++; }
+                }
+            }
+        }
+        // Larger rectangles: warp-cooperative walk, the slot is the tile counter's old value.  Only the owner's id travels; each lane
+        // re-reads the owner's record (stored above, ordered by the walk's __syncwarp) and derives what k_emit derives from it: the
+        // strip context of the whole rectangle, bands relative to the tile's 8-row chunk of its column.
+        const bool big = rect_n > 8;
+        const uint32_t pay[1] = {(uint32_t)idx};
+        for_each_tile<0, 1>(big ? x0 : 0, big ? y0 : 0, big ? x1 : 0, big ? y1 : 0, p.gx, pay, [&](int tile, int tx, int ty, const uint32_t(&o)[1]) {
+            const float4 r0 = p.records[3 * (size_t)o[0]], r1 = p.records[3 * (size_t)o[0] + 1];
+            const float gtau = footprint_tau(r1.y);
+            const uint32_t slot = atomicAdd(&p.tile_count[tile], 1u);
+            if (slot >= S) return;
+            int gx0, gy0, gx1, gy1;
+            tile_rect(r0.x, r0.y, __float_as_int(r1.w), p.gx, p.gy, gx0, gy0, gx1, gy1);
+            const StripCtx c2 = rect_strip_ctx(r0.x, r0.y, r0.z, r0.w, r1.x, gtau, gx0, gy0, gx1, gy1);
+            uint32_t mask;
+            if (c2.ok) {
+                const int ty_lo = gy0 + ((ty - gy0) & ~7);
+                uint32_t b0, b1;
+                column_bands(c2, !c2.none, tx, ty_lo, b0, b1);
+                mask = bands_tile_mask(b0, b1, ty - ty_lo);
+            } else {
+                mask = tile_foot_mask(r0.x, r0.y, r0.z, r0.w, r1.x, gtau, tx, ty);
+            }
+            p.slab[(size_t)tile * S + slot] = ((unsigned long long)__float_as_uint(r1.z) << 32) | ((o[0] << 8) | mask);
+        });
     }
     // compact list of the visible Gaussians (order is irrelevant: every entry is processed independently)
     const unsigned vm = __ballot_sync(GSR_FULL, vis);
@@ -492,7 +545,7 @@ __global__ void __launch_bounds__(PRE_THREADS, 8) k_project(const PreParams p) {
 // =====================================================================================================
 __global__ void __launch_bounds__(1024) k_tile_scan(const uint32_t* __restrict__ tile_count, const uint32_t* __restrict__ tile_big,
                                                     uint32_t* __restrict__ tile_fill, uint2* __restrict__ ranges,
-                                                    gsr_counters* counters, int tiles, uint32_t capacity) {
+                                                    gsr_counters* counters, int tiles, uint32_t capacity, uint32_t slab_stride) {
     // Every thread owns SCAN_PER consecutive tiles (16-byte loads and stores; the arrays are 256-byte aligned), so a 1080p frame
     // (8,160 tiles) is one pass with two barriers instead of eight chunks of 1024 tiles with three barriers each.
     constexpr int SCAN_PER = 8;
@@ -570,7 +623,7 @@ __global__ void __launch_bounds__(1024) k_tile_scan(const uint32_t* __restrict__
         const uint32_t m = __reduce_max_sync(GSR_FULL, warp_max[lane]);
         if (lane == 0) {
             counters->num_rendered = carry;
-            counters->overflow = carry > capacity ? 1u : 0u;
+            counters->overflow = (carry > capacity || (slab_stride > 0 && m > slab_stride)) ? 1u : 0u;  // slab_stride 0: no slab
             counters->max_tile = m;
         }
     }
@@ -629,11 +682,7 @@ __global__ void __launch_bounds__(PRE_THREADS, EMIT_MINB) k_emit(const EmitParam
     float* own = s_own + warp * 16 * 32;
     {
         StripCtx sc = {};
-        if (PACKED && cnt > 0) {
-            const float um = fmaxf(r0.x - (float)(x0 * GSR_TILE), (float)(x1 * GSR_TILE) - r0.x);
-            const float vm = fmaxf(r0.y - (float)(y0 * GSR_TILE), (float)(y1 * GSR_TILE) - r0.y);
-            sc = strip_ctx(r0.x, r0.y, r0.z, r0.w, r1.x, tau, um, vm);
-        }
+        if (PACKED && cnt > 0) sc = rect_strip_ctx(r0.x, r0.y, r0.z, r0.w, r1.x, tau, x0, y0, x1, y1);
         own[0 * 32 + lane] = r0.x; own[1 * 32 + lane] = r0.y; own[2 * 32 + lane] = r0.w; own[3 * 32 + lane] = sc.det;
         own[4 * 32 + lane] = sc.rc; own[5 * 32 + lane] = sc.cT; own[6 * 32 + lane] = sc.sstar;
         own[7 * 32 + lane] = __uint_as_float((sc.ok ? 1u : 0u) | (sc.none ? 2u : 0u) | (cnt > 8 ? 4u : 0u));
@@ -669,26 +718,13 @@ __global__ void __launch_bounds__(PRE_THREADS, EMIT_MINB) k_emit(const EmitParam
         const uint32_t lo_id = PACKED ? gid << 8 : gid;
         const bool big = fl & 4u;
         const float gpx = own[0 * 32 + g], gpy = own[1 * 32 + g], gb = own[2 * 32 + g];
-        float ylo0 = 0.f, yhi0 = 0.f, ylo1 = 0.f, yhi1 = 0.f;
-        bool v0 = false, v1 = false;
-        if (PACKED && (fl & 1u) && !(fl & 2u)) {
+        uint32_t bands0 = 0, bands1 = 0;  // the column chunk's 4-row bands of both strips
+        if (PACKED) {
             StripCtx c2;
             c2.px = gpx; c2.py = gpy; c2.b = gb; c2.det = own[3 * 32 + g]; c2.rc = own[4 * 32 + g]; c2.cT = own[5 * 32 + g]; c2.sstar = own[6 * 32 + g];
             c2.ok = true; c2.none = false;
-            v0 = strip_rows(c2, (float)(tx * GSR_TILE), 8.f, ylo0, yhi0);
-            v1 = strip_rows(c2, (float)(tx * GSR_TILE + 8), 8.f, ylo1, yhi1);
+            column_bands(c2, (fl & 1u) && !(fl & 2u), tx, ty_lo, bands0, bands1);
         }
-        // The rows [ylo, yhi] a strip covers, as a bit mask over the (at most 32) 4-row bands of this column chunk: band k = rows
-        // [Y0 + 4k, Y0 + 4k + 3] is touched iff ylo <= Y0 + 4k + 3 and yhi >= Y0 + 4k, i.e. ceil((ylo - Y0 - 3) / 4) <= k <= floor((yhi - Y0) / 4).
-        // Two conversions per strip instead of eight comparisons per tile; near a band boundary the subtractions are exact (Y0 is an
-        // integer within a factor two of y), and the strips carry a 0.01-pixel margin anyway.
-        const float Y0 = (float)(ty_lo * GSR_TILE);
-        auto band_bits = [&](const bool v, const float ylo, const float yhi) -> uint32_t {
-            const float a = fminf(fmaxf((ylo - Y0 - 3.f) * 0.25f, -1.f), 33.f), b = fminf(fmaxf((yhi - Y0) * 0.25f, -1.f), 33.f);
-            const int klo = max((int)ceilf(a), 0), khi = min((int)floorf(b), 31);
-            return (v && klo <= khi) ? (0xffffffffu >> (31 - khi)) & (0xffffffffu << klo) : 0u;
-        };
-        const uint32_t bands0 = band_bits(v0, ylo0, yhi0), bands1 = band_bits(v1, ylo1, yhi1);
         // Slots of the column's (at most 8) tiles first — rank + start of the tile's bucket, or a ticket from the per-tile cursor for
         // rectangles of > 8 tiles — so that up to 16 independent loads / atomics are in flight while the masks are computed.
         const uint32_t* rk = p.ranks + 8 * (size_t)gid + col * gh + (ty_lo - gy0);  // column-major ranks of a <= 8-tile rectangle
@@ -716,12 +752,7 @@ __global__ void __launch_bounds__(PRE_THREADS, EMIT_MINB) k_emit(const EmitParam
                 uint32_t mask = 0;
                 if (PACKED) {
                     if (!(fl & 1u)) mask = tile_foot_mask(gpx, gpy, own[12 * 32 + g], gb, own[13 * 32 + g], own[14 * 32 + g], tx, ty);
-                    else {  // the tile's four bands of both strips, interleaved: bit 2q + i = band q of strip i
-                        uint32_t n0 = (bands0 >> (4 * r)) & 15u, n1 = (bands1 >> (4 * r)) & 15u;
-                        n0 = (n0 | (n0 << 2)) & 0x33u; n0 = (n0 | (n0 << 1)) & 0x55u;
-                        n1 = (n1 | (n1 << 2)) & 0x33u; n1 = (n1 | (n1 << 1)) & 0x55u;
-                        mask = n0 | (n1 << 1);
-                    }
+                    else mask = bands_tile_mask(bands0, bands1, r);
                 }
                 p.pairs[pos[r]] = make_uint2(lo_id | mask, dbits);  // little endian: u64 = depth bits << 32 | low word
             }
@@ -1072,26 +1103,27 @@ __device__ void foot_ballots(const FootArgs& fa, const unsigned long long* keys,
     }
 }
 
-// Sorts the bucket of one tile (pairs[rg.x..rg.y) by (depth bits, id)) and writes the ids to point_list.
+// Sorts the bucket of one tile by (depth bits, id) and writes the ids to point_list.  The tile's keys are read from g: its slab
+// (slab emission) or pairs[rg.x..rg.y) (ranked emission); keep_pairs: the sorted keys go to pairs[rg.x..rg.y) either way.
 // s: SORT_CAP u64 of shared memory, hist: SORT_BUCKETS+1 u32.  Block-wide (SORT_THREADS threads), ends without a barrier.
 template <bool PACKED>
-__device__ void sort_tile(const uint2 rg, unsigned long long* __restrict__ pairs, uint32_t* __restrict__ point_list, int keep_pairs,
-                          unsigned long long* s, uint32_t* hist, uint16_t* tk16, const FootArgs& fa, int tile) {
+__device__ void sort_tile(const uint2 rg, unsigned long long* __restrict__ g, unsigned long long* pairs, uint32_t* __restrict__ point_list,
+                          int keep_pairs, unsigned long long* s, uint32_t* hist, uint16_t* tk16, const FootArgs& fa, int tile) {
     const uint32_t n = rg.y - rg.x;
     const uint32_t tid = threadIdx.x;
     if (n == 0) return;
-    unsigned long long* g = pairs + rg.x;
+    unsigned long long* keep = keep_pairs ? pairs + rg.x : nullptr;
     uint32_t* out = point_list + rg.x;
     if (n <= SORT_SMALL && tk16 != nullptr) {
-        sort_bucket_small<PACKED>(g, n, out, keep_pairs ? g : nullptr, s, hist, tk16, fa, rg.x, tile);
+        sort_bucket_small<PACKED>(g, n, out, keep, s, hist, tk16, fa, rg.x, tile);
         return;
     }
     if (n <= SORT_CAP) {
-        sort_bucket<PACKED>(g, n, out, keep_pairs ? g : nullptr, s, hist);
+        sort_bucket<PACKED>(g, n, out, keep, s, hist);
         foot_ballots<PACKED>(fa, s, n, rg.x, tile);  // s[] still holds the sorted keys (only read after the sort's last barrier)
         return;
     }
-    // ---- large tile: chunks sorted in shared memory, cross-chunk steps in global (L2) memory ----
+    // ---- large tile: chunks sorted in shared memory, cross-chunk steps in global (L2) memory, in place in g ----
     const uint32_t N = next_pow2(n);
     for (uint32_t c0 = 0; c0 < n; c0 += SORT_CAP) {
         const uint32_t m = min((uint32_t)SORT_CAP, n - c0);
@@ -1128,21 +1160,23 @@ __device__ void sort_tile(const uint2 rg, unsigned long long* __restrict__ pairs
         const unsigned long long x = g[i];
         const uint32_t id = PACKED ? (uint32_t)x >> 8 : (uint32_t)x;
         out[i] = id;
-        if (PACKED && keep_pairs) g[i] = (x & 0xffffffff00000000ull) | id;
+        if (PACKED && keep) keep[i] = (x & 0xffffffff00000000ull) | id;  // !PACKED: the sorted keys are in place already
     }
 }
 
-// stand-alone per-tile sort kernel
+// stand-alone per-tile sort kernel; slab != nullptr: tile t's keys are slab[t * slab_stride ...] (PACKED only)
 template <bool PACKED>
-__global__ void __launch_bounds__(SORT_THREADS, 5) k_sort_tiles(const uint2* __restrict__ ranges, unsigned long long* __restrict__ pairs,
-                                                             uint32_t* __restrict__ point_list,
+__global__ void __launch_bounds__(SORT_THREADS, 5) k_sort_tiles(const uint2* __restrict__ ranges, unsigned long long* pairs,
+                                                             unsigned long long* slab, uint32_t slab_stride, uint32_t* __restrict__ point_list,
                                                              const gsr_counters* __restrict__ counters, int keep_pairs, const FootArgs fa,
                                                              const int sort_small_enabled) {
     if (counters->overflow) return;  // set by k_tile_scan, before this kernel started
     __shared__ unsigned long long s[SORT_CAP];
     __shared__ uint32_t hist[SORT_BUCKETS + 1];
     __shared__ uint16_t tk16[SORT_SMALL];
-    sort_tile<PACKED>(ranges[blockIdx.x], pairs, point_list, keep_pairs, s, hist, sort_small_enabled ? tk16 : nullptr, fa, (int)blockIdx.x);
+    const uint2 rg = ranges[blockIdx.x];
+    unsigned long long* g = slab ? slab + (size_t)blockIdx.x * slab_stride : pairs + rg.x;
+    sort_tile<PACKED>(rg, g, pairs, point_list, keep_pairs, s, hist, sort_small_enabled ? tk16 : nullptr, fa, (int)blockIdx.x);
 }
 
 // =====================================================================================================
@@ -1296,6 +1330,20 @@ int forward_impl(const gsr_frame* f, const gsr_workspace* ws, float* out_color, 
     if (cap < 1) { set_error("gsr_forward: binning workspace too small"); return GSR_ERR_WORKSPACE; }
     char* geo = (char*)ws->geom;
     char* bin = (char*)ws->binning;
+    // footprint masks travel in the low byte of the pair's id word when the ids fit 24 bits; GSR_PACKED_KEYS=0 forces the
+    // general path (masks computed by k_sort_tiles from gathered records), which is what P > 2^24 uses
+    static int packed_ok = -1;
+    if (packed_ok < 0) { const char* e = getenv("GSR_PACKED_KEYS"); packed_ok = (e && e[0] == '0') ? 0 : 1; }
+    const bool packed = packed_ok && f->P <= (1 << 24);
+    // slab emission needs packed keys and is not used with tight tiles; otherwise a slab stride is ignored and the ranked emission runs
+    const uint32_t slab_stride = packed && !(flags & GSR_FLAG_TIGHT_TILES) ? 32u * ((uint32_t)flags >> GSR_SLAB_SHIFT) : 0u;
+    unsigned long long* slab = nullptr;
+    if (slab_stride) {
+        const size_t off = BinLayout::slab_offset(cap_nominal, (size_t)il.tiles * slab_stride);
+        if (off < 8) { set_error("gsr_forward: binning workspace too small for slab stride %u (%d tiles)", slab_stride, il.tiles); return GSR_ERR_WORKSPACE; }
+        slab = (unsigned long long*)(bin + bl.pairs + off);
+        cap = cap < off / 8 ? cap : off / 8;  // compact keys of the sorted-keys output stay below the slab
+    }
 
     if (flags & GSR_FLAG_REUSE_GEOMETRY) {
         // `radii` is an INPUT here: the radii of the pass whose workspaces are being reused
@@ -1335,6 +1383,7 @@ int forward_impl(const gsr_frame* f, const gsr_workspace* ws, float* out_color, 
     pp.records = (float4*)(geo + gl.records); pp.cov3D = (float*)(geo + gl.cov3D); pp.clamped = (uint8_t*)(geo + gl.clamped);
     pp.radii = radii; pp.tile_count = (uint32_t*)(img + il.tile_count); pp.tile_big = (uint32_t*)(img + il.tile_big);
     pp.ranks = (uint32_t*)(geo + gl.ranks); pp.counters = counters;
+    pp.slab = slab; pp.slab_stride = slab_stride;
 
     pp.vis_list = (uint32_t*)(geo + gl.vis_list);
     uint2* ranges = (uint2*)(img + il.ranges);
@@ -1355,22 +1404,18 @@ int forward_impl(const gsr_frame* f, const gsr_workspace* ws, float* out_color, 
         prof_mark(1, st);
         if ((rc = check_launch("gsr_forward/project", debug, st))) return rc;
 
-        k_tile_scan<<<1, 1024, 0, st>>>(pp.tile_count, pp.tile_big, (uint32_t*)(img + il.tile_fill), ranges, counters, il.tiles, (uint32_t)(cap > 0xffffffffull ? 0xffffffffull : cap));
+        k_tile_scan<<<1, 1024, 0, st>>>(pp.tile_count, pp.tile_big, (uint32_t*)(img + il.tile_fill), ranges, counters, il.tiles, (uint32_t)(cap > 0xffffffffull ? 0xffffffffull : cap),
+                                       slab_stride);
         prof_mark(2, st);
         if ((rc = check_launch("gsr_forward/tile_scan", debug, st))) return rc;
     }
     if (flags & GSR_FLAG_BINNING_ONLY) return GSR_OK;
 
-    // footprint masks travel in the low byte of the pair's id word when the ids fit 24 bits; GSR_PACKED_KEYS=0 forces the
-    // general path (masks computed by k_sort_tiles from gathered records), which is what P > 2^24 uses
-    static int packed_ok = -1;
-    if (packed_ok < 0) { const char* e = getenv("GSR_PACKED_KEYS"); packed_ok = (e && e[0] == '0') ? 0 : 1; }
-    const bool packed = packed_ok && f->P <= (1 << 24);
-    EmitParams ep;
-    ep.P = f->P; ep.gx = il.gx; ep.gy = il.gy;
-    ep.records = pp.records; ep.ranks = pp.ranks; ep.vis_list = pp.vis_list;
-    ep.ranges = ranges; ep.tile_fill = (uint32_t*)(img + il.tile_fill); ep.pairs = (uint2*)(bin + bl.pairs); ep.counters = counters;
-    {
+    if (!slab) {  // ranked emission (the slab path wrote its pairs in k_project; its emission slot of the profile reads ~0)
+        EmitParams ep;
+        ep.P = f->P; ep.gx = il.gx; ep.gy = il.gy;
+        ep.records = pp.records; ep.ranks = pp.ranks; ep.vis_list = pp.vis_list;
+        ep.ranges = ranges; ep.tile_fill = (uint32_t*)(img + il.tile_fill); ep.pairs = (uint2*)(bin + bl.pairs); ep.counters = counters;
         const int grid = (f->P + PRE_THREADS - 1) / PRE_THREADS;  // sized for P; blocks past the visible list exit at once
         if (pp.tight) { if (packed) k_emit<true, true><<<grid, PRE_THREADS, 0, st>>>(ep); else k_emit<true, false><<<grid, PRE_THREADS, 0, st>>>(ep); }
         else          { if (packed) k_emit<false, true><<<grid, PRE_THREADS, 0, st>>>(ep); else k_emit<false, false><<<grid, PRE_THREADS, 0, st>>>(ep); }
@@ -1381,8 +1426,9 @@ int forward_impl(const gsr_frame* f, const gsr_workspace* ws, float* out_color, 
     const int keep_pairs = (flags & GSR_FLAG_SORTED_KEYS) ? 1 : 0;
     uint32_t* n_contrib = (flags & GSR_FLAG_FOR_BACKWARD) ? (uint32_t*)(img + il.n_contrib) : nullptr;
     FootArgs fa{pp.records, (uint32_t*)(bin + bl.bal), il.gx};
-    if (packed) k_sort_tiles<true><<<il.tiles, SORT_THREADS, 0, st>>>(ranges, (unsigned long long*)(bin + bl.pairs), (uint32_t*)(bin + bl.point_list), counters, keep_pairs, fa, g_opt.sort_single_pass);
-    else k_sort_tiles<false><<<il.tiles, SORT_THREADS, 0, st>>>(ranges, (unsigned long long*)(bin + bl.pairs), (uint32_t*)(bin + bl.point_list), counters, keep_pairs, fa, g_opt.sort_single_pass);
+    unsigned long long* pairs = (unsigned long long*)(bin + bl.pairs);
+    if (packed) k_sort_tiles<true><<<il.tiles, SORT_THREADS, 0, st>>>(ranges, pairs, slab, slab_stride, (uint32_t*)(bin + bl.point_list), counters, keep_pairs, fa, g_opt.sort_single_pass);
+    else k_sort_tiles<false><<<il.tiles, SORT_THREADS, 0, st>>>(ranges, pairs, nullptr, 0u, (uint32_t*)(bin + bl.point_list), counters, keep_pairs, fa, g_opt.sort_single_pass);
     prof_mark(4, st);
     if ((rc = check_launch("gsr_forward/sort", debug, st))) return rc;
     BlendArgs ba{ranges, (const uint32_t*)(bin + bl.point_list), pp.records, extra_colors, f->W, f->H, il.gx, il.gy, f->bg,

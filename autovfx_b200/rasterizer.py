@@ -143,6 +143,7 @@ class FrameTicket:
         s = self.stats()
         if s["overflow"]:
             self._state.grow(needed_capacity(s))
+            self._state.grow_slab(s["max_tile"])
         return not s["overflow"]
 
 
@@ -151,12 +152,36 @@ def needed_capacity(stats: Dict[str, int]) -> int:
     return int(stats["num_rendered"])
 
 
+# Slab emission (GSR_SLAB_SHIFT): every tile gets a slab of S sort pairs, so k_project writes the pairs itself and the separate
+# emission pass goes away.  The slab costs tiles * S pairs whatever the frame, so one crowded tile (a far camera that puts most
+# Gaussians into a few tiles) would make it huge: it is only used while its pairs take at most SLAB_BUDGET times the compact pairs
+# of the binning capacity; otherwise the ranked emission runs, with the same outputs.
+SLAB_BUDGET = 2
+SLAB_ALIGN = 32
+
+
+def slab_stride(P: int, W: int, H: int, capacity: int, want: int, flags: int = 0) -> int:
+    """Slab stride S of a frame (0: ranked emission).  ``want`` is the stride the counters of earlier frames asked for (0: none
+    yet, the first guess is the largest stride the budget allows).  Tight tiles keep the ranked emission (measured faster there)."""
+    tiles = ((W + 15) // 16) * ((H + 15) // 16)
+    if P <= 0 or P > (1 << 24) or tiles <= 0 or flags & _lib.GSR_FLAG_TIGHT_TILES:
+        return 0  # no slab without packed keys (ids of 24 bits)
+    limit = SLAB_BUDGET * capacity // tiles // SLAB_ALIGN * SLAB_ALIGN
+    S = limit if want <= 0 else want
+    return S if 0 < S <= limit and S // SLAB_ALIGN < (1 << 15) else 0
+
+
+def slab_flags(S: int) -> int:
+    return (S // SLAB_ALIGN) << _lib.GSR_SLAB_SHIFT
+
+
 class _DeviceState:
     RING = 64
 
     def __init__(self, device: torch.device):
         self.device = device
         self.capacity = 1 << 20
+        self.slab_want = 0  # slab stride asked for by the counters of an overflowed frame (0: none yet)
         self.pinned = torch.zeros((self.RING, 8), dtype=torch.int32).pin_memory()
         self.events = [None] * self.RING
         self.tickets = [None] * self.RING  # weak references to the ticket reading each slot
@@ -169,6 +194,14 @@ class _DeviceState:
 
     def grow(self, needed: int) -> None:
         self.capacity = max(self.capacity, int(needed * 1.25) + 4096)
+
+    def grow_slab(self, max_tile: int) -> None:
+        """After an overflow: a slab stride that holds 1.25 x the longest tile list, like the capacity's growth."""
+        want = -(-int(max_tile * 1.25) // SLAB_ALIGN) * SLAB_ALIGN
+        self.slab_want = max(self.slab_want, want)
+
+    def slab_stride(self, P: int, W: int, H: int, flags: int = 0) -> int:
+        return slab_stride(P, W, H, self.capacity, self.slab_want, flags)
 
     def ensure_capacity(self, P: int, W: int = 0, H: int = 0) -> None:
         # first guess: a few instances per Gaussian; corrected from the counters of real frames
@@ -390,20 +423,22 @@ def forward_raw(means3D, shs, colors_precomp, opacities, scales, rotations, cov3
             if not for_backward:
                 st.geom_cache.pop(stream.cuda_stream, None)  # the shared workspaces are about to be rewritten (also by a P == 0 call)
             while True:
-                binning = st.workspace("binning", _L.gsr_binning_bytes(st.capacity), for_backward)
+                S = st.slab_stride(P, W, H, flags)
+                binning = st.workspace("binning", _L.gsr_binning_bytes_slab(st.capacity, W, H, S), for_backward)
                 ws = _workspace(geom, binning, image)
                 if extra is not None and P == 0:
                     extra_out.zero_()
-                cap_now = _L.gsr_binning_capacity(binning.numel())
+                cap_now = _L.gsr_binning_capacity_slab(binning.numel(), W, H, S)
+                frame_flags = flags | slab_flags(S)
                 if do_sync and P > 0 and not settings.debug:
                     # safe mode: the frame is issued in two halves; the counters are final after the first (projection + tile scan), so
                     # the host waits for THAT copy while colour / emission / sort / blend are already queued behind it
-                    launch(ws, radii, flags | _lib.GSR_FLAG_BINNING_ONLY)
+                    launch(ws, radii, frame_flags | _lib.GSR_FLAG_BINNING_ONLY)
                     check = st.issue_ticket(counters, stream, cap_now, early=True)
-                    launch(ws, radii, flags | _lib.GSR_FLAG_RESUME)
+                    launch(ws, radii, frame_flags | _lib.GSR_FLAG_RESUME)
                     ticket = st.issue_ticket(counters, stream, cap_now)  # the frame's final counters (exact_redos)
                 else:
-                    launch(ws, radii, flags)
+                    launch(ws, radii, frame_flags)
                     check = ticket = st.issue_ticket(counters, stream, cap_now)
                 if not do_sync:
                     break
@@ -413,6 +448,7 @@ def forward_raw(means3D, shs, colors_precomp, opacities, scales, rotations, cov3
                 if not s["overflow"]:
                     break
                 st.grow(needed_capacity(s))  # rare: first frames of a new scene; re-run with a larger binning buffer
+                st.grow_slab(s["max_tile"])
             if not for_backward and P > 0:
                 # remember which geometry the shared workspaces now hold (tensors kept alive so their storage cannot be recycled)
                 st.geom_cache[stream.cuda_stream] = (gkey, (means3D, opacities, scales, rotations, cov3D_precomp, view, proj, campos), radii,
@@ -474,8 +510,10 @@ class PreparedForward:
         self.out_ptrs = (color.data_ptr(), depth.data_ptr(), alpha.data_ptr(), radii.data_ptr() if self.P > 0 else None)
         self.extra_ptrs = (_ptr(extra) if self.P > 0 else None, _ptr(extra_out) if extra is not None and self.P > 0 else None)
         self.extra_out = extra_out
-        self.flags = _mode_flags(tight, exact)
+        self.mode_flags = _mode_flags(tight, exact)
+        self.flags = self.mode_flags
         self._cap = -1
+        self._slab_want = -1
         self.ws = None
         self._bufs = None
 
@@ -485,12 +523,14 @@ class PreparedForward:
             geom = st.workspace("geom", _L.gsr_geom_bytes(self.P), False)
             image = st.workspace("image", _L.gsr_image_bytes(self.W, self.H), False)
             st.ensure_capacity(self.P, self.W, self.H)
-            binning = st.workspace("binning", _L.gsr_binning_bytes(st.capacity), False)
+            S = st.slab_stride(self.P, self.W, self.H, self.mode_flags)
+            binning = st.workspace("binning", _L.gsr_binning_bytes_slab(st.capacity, self.W, self.H, S), False)
         self._bufs = (geom, binning, image)
         self.ws = _workspace(geom, binning, image)
-        self._cap = st.capacity
+        self._cap, self._slab_want = st.capacity, st.slab_want
+        self.flags = self.mode_flags | slab_flags(S)
         self._counters = image[:32].view(torch.int32)
-        self._capacity_instances = _L.gsr_binning_capacity(binning.numel())
+        self._capacity_instances = _L.gsr_binning_capacity_slab(binning.numel(), self.W, self.H, S)
 
     def launch(self, tanfovx: float, tanfovy: float) -> FrameTicket:
         """Issue the frame on the current stream; never synchronises.  Validate the returned ticket before trusting the images."""
@@ -500,7 +540,7 @@ class PreparedForward:
     def _launch(self, tanfovx: float, tanfovy: float) -> FrameTicket:
         st = self.st
         stream = torch.cuda.current_stream(self.device)
-        if self._cap != st.capacity or self.ws is None:
+        if self._cap != st.capacity or self._slab_want != st.slab_want or self.ws is None:
             self._bind_workspaces()
         else:  # the cached workspaces may have been re-allocated (grown) by another caller on this stream
             g2, b2, i2 = st.cache.get(("geom", stream.cuda_stream)), st.cache.get(("binning", stream.cuda_stream)), st.cache.get(("image", stream.cuda_stream))

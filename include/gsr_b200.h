@@ -89,6 +89,12 @@ enum {
     GSR_FLAG_RESUME = 64,       /* second half: same arguments and workspaces as the GSR_FLAG_BINNING_ONLY call; runs colour +
                                   emission, the tile sort and the blend. */
 };
+/* Slab emission: flags | ((S / 32) << GSR_SLAB_SHIFT) gives every tile a slab of S sort pairs (S a multiple of 32, 0 = off), so
+ * the projection writes each (Gaussian, tile) pair the moment it draws the tile's ticket, and the separate emission pass and its
+ * per-Gaussian ranks go away.  The slab takes tiles * S instances at the end of the binning workspace's pair region: size the
+ * workspace with gsr_binning_bytes_slab().  A tile with more than S instances sets gsr_counters.overflow (max_tile says how many
+ * it had), like a capacity overflow.  Outputs are identical with and without a slab; it is ignored when P > 2^24 and with GSR_FLAG_TIGHT_TILES. */
+#define GSR_SLAB_SHIFT 16
 
 /* One rasterizer invocation = the argument list of Rasterizer::forward (DGR/cuda_rasterizer/rasterizer.h:33-58). */
 typedef struct gsr_frame {
@@ -145,6 +151,10 @@ size_t gsr_binning_bytes(size_t capacity_instances);
 size_t gsr_image_bytes(int32_t W, int32_t H);
 /* Largest capacity (in instances) a binning workspace of `bytes` bytes provides. */
 size_t gsr_binning_capacity(size_t bytes);
+/* The same two queries for a forward with slab stride S (GSR_SLAB_SHIFT) on a W x H image: the workspace holds `capacity`
+ * instances besides the slab.  S = 0 gives gsr_binning_bytes / gsr_binning_capacity; 0 from the second means the slab does not fit. */
+size_t gsr_binning_bytes_slab(size_t capacity_instances, int32_t W, int32_t H, int32_t slab_stride);
+size_t gsr_binning_capacity_slab(size_t bytes, int32_t W, int32_t H, int32_t slab_stride);
 
 /* Forward: projection (+ per-tile histogram) -> tile scan -> colour + key emission (+ footprint masks) -> per-tile depth sort
  * (+ footprint ballot matrix) -> blend (one warp per 8x4-pixel footprint).
