@@ -57,6 +57,13 @@ class gsr_densify_group(C.Structure):
                 ("m2_dst", C.c_void_p), ("width", C.c_int32), ("role", C.c_int32)]
 
 
+class gsr_adam_tensor(C.Structure):
+    _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p), ("numel", C.c_int64),
+                ("lerp_weight", C.c_float), ("beta2", C.c_float), ("one_minus_beta2", C.c_float), ("bias_correction2_sqrt", C.c_float),
+                ("eps", C.c_float), ("step_size", C.c_float)]
+
+
+GSR_ADAM_MAX_TENSORS = 32
 GSR_DENSIFY_MAX_GROUPS = 8
 GSR_DENSIFY_ROLE_COPY, GSR_DENSIFY_ROLE_XYZ, GSR_DENSIFY_ROLE_SCALING = 0, 1, 2
 GSR_DENSIFY_ROTATION_3DGS, GSR_DENSIFY_ROTATION_SUGAR = 0, 1
@@ -77,7 +84,8 @@ EXPORTS = ("gsr_abi_version", "gsr_last_error", "gsr_geom_bytes", "gsr_binning_b
            "gsr_sugar_normals", "gsr_sugar_normals_backward", "gsr_sugar_colors", "gsr_sugar_colors_backward", "gsr_knn_bytes", "gsr_knn",
            "gsr_sugar_field_bytes", "gsr_sugar_field", "gsr_sugar_field_backward", "gsr_sugar_sdf_normal_bytes", "gsr_sugar_sdf_normal",
            "gsr_sugar_sdf_normal_backward", "gsr_densify_stats", "gsr_densify_plan_bytes", "gsr_densify_plan", "gsr_densify_apply",
-           "gsr_sugar_sample_bytes", "gsr_sugar_sample", "gsr_sugar_sample_backward", "gsr_binning_bytes_slab", "gsr_binning_capacity_slab")
+           "gsr_sugar_sample_bytes", "gsr_sugar_sample", "gsr_sugar_sample_backward", "gsr_binning_bytes_slab", "gsr_binning_capacity_slab",
+           "gsr_adam_step")
 
 
 def _load() -> C.CDLL:
@@ -172,6 +180,8 @@ def _load() -> C.CDLL:
     lib.gsr_sugar_sample.argtypes = ([C.c_int32] * 2 + [C.c_float, C.c_int32] + [C.c_void_p] * 10 + [C.c_void_p, C.c_size_t, C.c_void_p])
     lib.gsr_sugar_sample_backward.restype = C.c_int
     lib.gsr_sugar_sample_backward.argtypes = [C.c_int32] * 2 + [C.c_float] + [C.c_void_p] * 10
+    lib.gsr_adam_step.restype = C.c_int
+    lib.gsr_adam_step.argtypes = [C.c_int32, C.POINTER(gsr_adam_tensor), C.c_void_p]
     lib.gsr_get_views.restype = C.c_int
     lib.gsr_get_views.argtypes = [C.POINTER(gsr_workspace), C.c_int32, C.c_int32, C.c_int32, C.POINTER(gsr_views)]
     lib.gsr_profile_begin.restype = C.c_int

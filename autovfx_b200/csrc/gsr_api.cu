@@ -70,6 +70,7 @@ int densify_plan_impl(int P, const float* accum, const float* denom, const float
                       int32_t* totals, void* ws, size_t ws_bytes, cudaStream_t st);
 int densify_apply_impl(int P, int S, int n_groups, const gsr_densify_group* groups, const int32_t* dst, const float* xyz,
                        const float* scaling, const float* rotation, const float* eps, int rotation_mode, cudaStream_t st);
+int adam_step_impl(int n, const gsr_adam_tensor* tensors, cudaStream_t st);
 size_t sugar_sample_bytes(int P);
 int sugar_sample_impl(int N, int P, float f, int volume, const uint8_t* mask, const float* strengths, const double* u, const float* z,
                       const float* points, const float* scaling, const float* quaternions, float* out_points, int64_t* out_idx,
@@ -301,6 +302,11 @@ int gsr_sugar_sample_backward(int32_t N, int32_t P, float sampling_scale_factor,
     NvtxRange nvtx_("gsr_sugar_sample_backward");
     return gsr::sugar_sample_backward_impl(N, P, sampling_scale_factor, idx, z, scaling, quaternions, total, dL_dsamples, dL_dpoints,
                                            dL_dscaling, dL_dquaternions, (cudaStream_t)stream);
+}
+
+int gsr_adam_step(int32_t n, const gsr_adam_tensor* tensors, void* stream) {
+    NvtxRange nvtx_("gsr_adam_step");
+    return gsr::adam_step_impl(n, tensors, (cudaStream_t)stream);
 }
 
 int gsr_profile_begin(int max_frames) { return gsr::profile_begin(max_frames, 1); }

@@ -19,6 +19,8 @@
  *                               (scene/gaussian_model.py:268-417) and SuGaRDensifier (sugar_scene/sugar_densifier.py:48-246)
  *   gsr_sugar_sample  replaces  SuGaR.sample_points_in_gaussians               sugar_scene/sugar_model.py:757-799;
  *                               gsr_sugar_sample_backward its autograd backward
+ *   gsr_adam_step     replaces  torch.optim.Adam.step() (foreach) of every trainer  GS/train.py:183-184, scene_representation.py:538-540,
+ *                               sugar_trainers/coarse_density.py:822
  *
  * and, for the render() wrapper around the two rasterizer passes ("GR/" = sugar/gaussian_splatting/gaussian_renderer/__init__.py):
  *
@@ -448,6 +450,34 @@ typedef struct gsr_densify_group {
  * n_groups <= GSR_DENSIFY_MAX_GROUPS (host array).  The outputs must not alias the inputs. */
 int gsr_densify_apply(int32_t P, int32_t S, int32_t n_groups, const gsr_densify_group* groups, const int32_t* dst, const float* xyz,
                       const float* scaling, const float* rotation, const float* eps, int32_t rotation_mode, void* stream);
+
+/* One tensor of gsr_adam_step: a parameter, its gradient and its two Adam moments (numel floats each), and the scalars
+ * torch.optim.Adam's foreach path computes for it on the host in double (torch/optim/adam.py:_multi_tensor_adam), each rounded to
+ * float as the foreach kernels receive it, for the step count after this step's increment: */
+typedef struct gsr_adam_tensor {
+    float* param;
+    const float* grad;
+    float* exp_avg;
+    float* exp_avg_sq;
+    int64_t numel;
+    float lerp_weight;           /* 1 - beta1                                  */
+    float beta2;                 /* beta2                                      */
+    float one_minus_beta2;       /* 1 - beta2                                  */
+    float bias_correction2_sqrt; /* (1 - beta2 ** step) ** 0.5                 */
+    float eps;                   /* eps                                        */
+    float step_size;             /* (lr / (1 - beta1 ** step)) * -1            */
+} gsr_adam_tensor;
+#define GSR_ADAM_MAX_TENSORS 32
+
+/* torch.optim.Adam.step() with its defaults (no amsgrad, weight_decay 0, not maximize, foreach) over n tensors, in place and
+ * bit-identical to torch's seven list ops:
+ *   exp_avg    = lerp(exp_avg, grad, lerp_weight)
+ *   exp_avg_sq = exp_avg_sq * beta2 + one_minus_beta2 * grad * grad
+ *   param      = param + step_size * exp_avg / (sqrt(exp_avg_sq) / bias_correction2_sqrt + eps)
+ * with torch's roundings (see gsr_adam.cu).  Descriptors travel in the kernel parameters (host array, no copy); n beyond
+ * GSR_ADAM_MAX_TENSORS takes one launch per GSR_ADAM_MAX_TENSORS.  Float4 accesses where all four pointers of a tensor are 16-byte
+ * aligned.  No workspace, no host synchronisation.  n = 0 is a no-op. */
+int gsr_adam_step(int32_t n, const gsr_adam_tensor* tensors, void* stream);
 
 /* Device pointers into the workspaces of the last layout (P, capacity, W, H) — for parity tests that
  * compare per-stage buffers with the reference (SURVEY §4).  Pure pointer arithmetic, no CUDA calls. */

@@ -4,9 +4,12 @@ and get_normal, against render_raw() (activations, normals and their backward in
 One step is the one tools/bench_train_render.py times: render one trajectory camera, L1 on "render", "depth" and "normal" against
 "pseudo_normal".detach(), loss.backward().  The two paths alternate step by step in one process, each step timed with CUDA events
 after warm-up.  --profile instead counts, with torch.profiler, the kernels each path launches in one step (a separate run: tracing
-slows the host).
+slows the host).  --optimizer torch|library ends every step with the optimizer step train.py runs after the backward
+(torch.optim.Adam(l, lr=0.0, eps=1e-15) over the six param groups with the trainer's learning rates, then the gradients set to
+None): torch's default foreach Adam, or the same optimizer switched to the library's CUDA step (autovfx_b200.optim.use_cuda_adam).
 
     python tools/bench_train_raw.py --steps 40 --warmup 5 [--gaussians 3000000] [--width 1920 --height 1080] [--profile]
+                                    [--optimizer none|torch|library]
 """
 from __future__ import annotations
 
@@ -64,9 +67,18 @@ def main():
     ap.add_argument("--width", type=int, default=1920)
     ap.add_argument("--height", type=int, default=1080)
     ap.add_argument("--profile", action="store_true", help="count the kernels of one step per path instead of timing")
+    ap.add_argument("--optimizer", choices=("none", "torch", "library"), default="none",
+                    help="end each step with the trainer's Adam step: torch's foreach Adam or the library's CUDA step")
     args = ap.parse_args()
     dev = torch.device("cuda:0")
     pc = RawModel({k: v.to(dev) for k, v in scene.config3_scene(P=args.gaussians).items()})
+    optimizer = None
+    if args.optimizer != "none":  # GaussianModel.training_setup (gaussian_model.py:164-173), spatial_lr_scale 5
+        lrs = (0.00016 * 5.0, 0.0025, 0.0025 / 20.0, 0.05, 0.005, 0.001)
+        optimizer = torch.optim.Adam([{"params": [p], "lr": lr} for p, lr in zip(pc.params(), lrs)], lr=0.0, eps=1e-15)
+        if args.optimizer == "library":
+            from autovfx_b200.optim import use_cuda_adam
+            use_cuda_adam(optimizer)
     cams = scene.cameras_from_trajectory(scene.trajectory_dict(radius=4.0, num_views=300, theta=30.0, w=args.width, h=args.height,
                                                                fov_x_deg=60.0))
     pipe = types.SimpleNamespace(debug=False, compute_cov3D_python=False, convert_SHs_python=False)
@@ -90,13 +102,16 @@ def main():
         loss = (out["render"] - gt_rgb).abs().mean() + (out["depth"] - gt_depth).abs().mean() + \
             (out["normal"] - out["pseudo_normal"].detach()).abs().mean()
         loss.backward()
+        if optimizer is not None:
+            optimizer.step()
+            optimizer.zero_grad(set_to_none=True)
 
     for i in range(args.warmup):
         for path in paths:
             step(path, i)
     torch.cuda.synchronize()
     res = {"workload": "training step from raw parameters, %.1fM Gaussians SH-deg 3, %dx%d, 300-camera trajectory, L1 on render/depth/normal"
-                       % (args.gaussians / 1e6, args.width, args.height), "card": card()}
+                       % (args.gaussians / 1e6, args.width, args.height), "optimizer": args.optimizer, "card": card()}
     if args.profile:
         from torch.profiler import ProfilerActivity, profile
         for path in paths:
