@@ -64,6 +64,7 @@ class gsr_adam_tensor(C.Structure):
 
 
 GSR_ADAM_MAX_TENSORS = 32
+GSR_LOSS_REDUCE_BYTES = 256 + 16 * 1024
 GSR_DENSIFY_MAX_GROUPS = 8
 GSR_DENSIFY_ROLE_COPY, GSR_DENSIFY_ROLE_XYZ, GSR_DENSIFY_ROLE_SCALING = 0, 1, 2
 GSR_DENSIFY_ROTATION_3DGS, GSR_DENSIFY_ROTATION_SUGAR = 0, 1
@@ -85,7 +86,8 @@ EXPORTS = ("gsr_abi_version", "gsr_last_error", "gsr_geom_bytes", "gsr_binning_b
            "gsr_sugar_field_bytes", "gsr_sugar_field", "gsr_sugar_field_backward", "gsr_sugar_sdf_normal_bytes", "gsr_sugar_sdf_normal",
            "gsr_sugar_sdf_normal_backward", "gsr_densify_stats", "gsr_densify_plan_bytes", "gsr_densify_plan", "gsr_densify_apply",
            "gsr_sugar_sample_bytes", "gsr_sugar_sample", "gsr_sugar_sample_backward", "gsr_binning_bytes_slab", "gsr_binning_capacity_slab",
-           "gsr_adam_step")
+           "gsr_adam_step", "gsr_photometric_loss_bytes", "gsr_photometric_loss", "gsr_photometric_loss_backward", "gsr_normal_loss",
+           "gsr_normal_loss_backward", "gsr_anisotropic_loss", "gsr_anisotropic_loss_backward")
 
 
 def _load() -> C.CDLL:
@@ -182,6 +184,21 @@ def _load() -> C.CDLL:
     lib.gsr_sugar_sample_backward.argtypes = [C.c_int32] * 2 + [C.c_float] + [C.c_void_p] * 10
     lib.gsr_adam_step.restype = C.c_int
     lib.gsr_adam_step.argtypes = [C.c_int32, C.POINTER(gsr_adam_tensor), C.c_void_p]
+    lib.gsr_photometric_loss_bytes.restype = C.c_size_t
+    lib.gsr_photometric_loss_bytes.argtypes = [C.c_int32] * 5
+    lib.gsr_photometric_loss.restype = C.c_int
+    lib.gsr_photometric_loss.argtypes = [C.c_int32] * 4 + [C.c_void_p] * 5 + [C.c_int32] + [C.c_void_p] * 3 + [C.c_size_t, C.c_void_p]
+    lib.gsr_photometric_loss_backward.restype = C.c_int
+    lib.gsr_photometric_loss_backward.argtypes = [C.c_int32] * 4 + [C.c_void_p] * 9 + [C.c_size_t, C.c_void_p]
+    lib.gsr_normal_loss.restype = C.c_int
+    lib.gsr_normal_loss.argtypes = [C.c_int64] + [C.c_void_p] * 5 + [C.c_int64, C.c_float, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+    lib.gsr_normal_loss_backward.restype = C.c_int
+    lib.gsr_normal_loss_backward.argtypes = ([C.c_int64] + [C.c_void_p] * 5 + [C.c_int64, C.c_float] + [C.c_void_p] * 3 +
+                                             [C.c_size_t, C.c_void_p])
+    lib.gsr_anisotropic_loss.restype = C.c_int
+    lib.gsr_anisotropic_loss.argtypes = [C.c_int64, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+    lib.gsr_anisotropic_loss_backward.restype = C.c_int
+    lib.gsr_anisotropic_loss_backward.argtypes = [C.c_int64, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.gsr_get_views.restype = C.c_int
     lib.gsr_get_views.argtypes = [C.POINTER(gsr_workspace), C.c_int32, C.c_int32, C.c_int32, C.POINTER(gsr_views)]
     lib.gsr_profile_begin.restype = C.c_int

@@ -71,6 +71,20 @@ int densify_plan_impl(int P, const float* accum, const float* denom, const float
 int densify_apply_impl(int P, int S, int n_groups, const gsr_densify_group* groups, const int32_t* dst, const float* xyz,
                        const float* scaling, const float* rotation, const float* eps, int rotation_mode, cudaStream_t st);
 int adam_step_impl(int n, const gsr_adam_tensor* tensors, cudaStream_t st);
+size_t photometric_loss_bytes(int B, int C, int H, int W, int for_backward);
+int photometric_loss_impl(int B, int C, int H, int W, const float* x, const int64_t* xs, const float* y, const int64_t* ys,
+                          const float* window, int for_backward, float* out_l1, float* out_ssim, void* ws, size_t ws_bytes,
+                          cudaStream_t st);
+int photometric_loss_backward_impl(int B, int C, int H, int W, const float* x, const int64_t* xs, const float* y, const int64_t* ys,
+                                   const float* window, const float* g_l1, const float* g_ssim, float* dx, const void* ws,
+                                   size_t ws_bytes, cudaStream_t st);
+int normal_loss_impl(int64_t n, const float* pred, const int64_t* ps, const float* gt, const int64_t* gs, const float* depth,
+                     int64_t d_sp, float scene_scale, float* out, void* ws, size_t ws_bytes, cudaStream_t st);
+int normal_loss_backward_impl(int64_t n, const float* pred, const int64_t* ps, const float* gt, const int64_t* gs, const float* depth,
+                              int64_t d_sp, float scene_scale, const float* g_out, float* d_pred, const void* ws, size_t ws_bytes,
+                              cudaStream_t st);
+int anisotropic_loss_impl(int64_t P, const float* scales, float r, float* out, void* ws, size_t ws_bytes, cudaStream_t st);
+int anisotropic_loss_backward_impl(int64_t P, const float* scales, float r, const float* g_out, float* d_scales, cudaStream_t st);
 size_t sugar_sample_bytes(int P);
 int sugar_sample_impl(int N, int P, float f, int volume, const uint8_t* mask, const float* strengths, const double* u, const float* z,
                       const float* points, const float* scaling, const float* quaternions, float* out_points, int64_t* out_idx,
@@ -307,6 +321,53 @@ int gsr_sugar_sample_backward(int32_t N, int32_t P, float sampling_scale_factor,
 int gsr_adam_step(int32_t n, const gsr_adam_tensor* tensors, void* stream) {
     NvtxRange nvtx_("gsr_adam_step");
     return gsr::adam_step_impl(n, tensors, (cudaStream_t)stream);
+}
+
+size_t gsr_photometric_loss_bytes(int32_t B, int32_t C, int32_t H, int32_t W, int32_t for_backward) {
+    return gsr::photometric_loss_bytes(B, C, H, W, for_backward);
+}
+
+int gsr_photometric_loss(int32_t B, int32_t C, int32_t H, int32_t W, const float* x, const int64_t* x_strides, const float* y,
+                         const int64_t* y_strides, const float* window, int32_t for_backward, float* out_l1, float* out_ssim,
+                         void* workspace, size_t workspace_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_photometric_loss");
+    return gsr::photometric_loss_impl(B, C, H, W, x, x_strides, y, y_strides, window, for_backward, out_l1, out_ssim, workspace,
+                                      workspace_bytes,
+                                      (cudaStream_t)stream);
+}
+
+int gsr_photometric_loss_backward(int32_t B, int32_t C, int32_t H, int32_t W, const float* x, const int64_t* x_strides, const float* y,
+                                  const int64_t* y_strides, const float* window, const float* g_l1, const float* g_ssim, float* dx,
+                                  const void* workspace, size_t workspace_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_photometric_loss_backward");
+    return gsr::photometric_loss_backward_impl(B, C, H, W, x, x_strides, y, y_strides, window, g_l1, g_ssim, dx, workspace,
+                                               workspace_bytes, (cudaStream_t)stream);
+}
+
+int gsr_normal_loss(int64_t n, const float* pred, const int64_t* pred_strides, const float* gt, const int64_t* gt_strides,
+                    const float* depth, int64_t depth_stride, float scene_scale, float* out, void* workspace, size_t workspace_bytes,
+                    void* stream) {
+    NvtxRange nvtx_("gsr_normal_loss");
+    return gsr::normal_loss_impl(n, pred, pred_strides, gt, gt_strides, depth, depth_stride, scene_scale, out, workspace,
+                                 workspace_bytes, (cudaStream_t)stream);
+}
+
+int gsr_normal_loss_backward(int64_t n, const float* pred, const int64_t* pred_strides, const float* gt, const int64_t* gt_strides,
+                             const float* depth, int64_t depth_stride, float scene_scale, const float* g_out, float* d_pred,
+                             const void* workspace, size_t workspace_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_normal_loss_backward");
+    return gsr::normal_loss_backward_impl(n, pred, pred_strides, gt, gt_strides, depth, depth_stride, scene_scale, g_out, d_pred,
+                                          workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int gsr_anisotropic_loss(int64_t P, const float* scales, float r, float* out, void* workspace, size_t workspace_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_anisotropic_loss");
+    return gsr::anisotropic_loss_impl(P, scales, r, out, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int gsr_anisotropic_loss_backward(int64_t P, const float* scales, float r, const float* g_out, float* d_scales, void* stream) {
+    NvtxRange nvtx_("gsr_anisotropic_loss_backward");
+    return gsr::anisotropic_loss_backward_impl(P, scales, r, g_out, d_scales, (cudaStream_t)stream);
 }
 
 int gsr_profile_begin(int max_frames) { return gsr::profile_begin(max_frames, 1); }

@@ -21,6 +21,10 @@
  *                               gsr_sugar_sample_backward its autograd backward
  *   gsr_adam_step     replaces  torch.optim.Adam.step() (foreach) of every trainer  GS/train.py:183-184, scene_representation.py:538-540,
  *                               sugar_trainers/coarse_density.py:822
+ *   gsr_photometric_loss replaces l1_loss and ssim of every trainer's objective  GS/utils/loss_utils.py:17-18, :33-62 (train.py:98-99,
+ *                               coarse_density.py:550-590, scene_representation.py:513-515); gsr_photometric_loss_backward their autograd
+ *   gsr_normal_loss   replaces  normal_loss                                       GS/utils/loss_utils.py:118-132; gsr_normal_loss_backward
+ *   gsr_anisotropic_loss replaces anisotropic_loss                                GS/utils/loss_utils.py:159-168; gsr_anisotropic_loss_backward
  *
  * and, for the render() wrapper around the two rasterizer passes ("GR/" = sugar/gaussian_splatting/gaussian_renderer/__init__.py):
  *
@@ -478,6 +482,47 @@ typedef struct gsr_adam_tensor {
  * GSR_ADAM_MAX_TENSORS takes one launch per GSR_ADAM_MAX_TENSORS.  Float4 accesses where all four pointers of a tensor are 16-byte
  * aligned.  No workspace, no host synchronisation.  n = 0 is a no-op. */
 int gsr_adam_step(int32_t n, const gsr_adam_tensor* tensors, void* stream);
+
+/* The training objective's terms (gsr_loss.cu).  Every value is a float32 device scalar written by the call; every mean is a
+ * fixed-order reduction (per-CTA float partials, one ordered double sum), bit-identical from call to call.  Upstream gradients are
+ * device pointers, so nothing synchronises with the host. */
+#define GSR_LOSS_REDUCE_BYTES (256 + 16 * 1024) /* the workspace of gsr_normal_loss[_backward] and gsr_anisotropic_loss              */
+
+/* Workspace of gsr_photometric_loss for [B,C,H,W] images: the partial sums, and with for_backward != 0 three float maps of
+ * B*C*H*W.  0 for an empty or oversized shape (B*C >= 65536). */
+size_t gsr_photometric_loss_bytes(int32_t B, int32_t C, int32_t H, int32_t W, int32_t for_backward);
+/* out_l1[0] = mean |x - y| (skipped when out_l1 is NULL), out_ssim[0] = mean SSIM of ssim(x, y) with the 11-tap window `window` (host [11], the 1-D
+ * float weights of create_window; applied separably), zero padding of 5, C1 = 0.01^2, C2 = 0.03^2.  x and y are [B,C,H,W] float
+ * images addressed by element strides x_strides / y_strides (host [4]: b, c, y, x), so a channel-innermost view needs no copy.
+ * `workspace` (16-byte aligned) needs gsr_photometric_loss_bytes(B, C, H, W, for_backward), else GSR_ERR_WORKSPACE; with
+ * for_backward != 0 it keeps the three per-pixel SSIM maps dS/d(mu_x, E[x^2], E[xy]) for gsr_photometric_loss_backward. */
+int gsr_photometric_loss(int32_t B, int32_t C, int32_t H, int32_t W, const float* x, const int64_t* x_strides, const float* y,
+                         const int64_t* y_strides, const float* window, int32_t for_backward, float* out_l1, float* out_ssim,
+                         void* workspace, size_t workspace_bytes, void* stream);
+/* dx (contiguous [B,C,H,W]) = g_ssim * d mean SSIM / dx + g_l1 * d mean |x - y| / dx, the upstream gradients read on the device
+ * (NULL = zero); the abs's gradient is 0 where x == y.  `workspace` is the forward's, run with for_backward on the same
+ * images.  Each pixel is written by one thread; no atomics. */
+int gsr_photometric_loss_backward(int32_t B, int32_t C, int32_t H, int32_t W, const float* x, const int64_t* x_strides, const float* y,
+                                  const int64_t* y_strides, const float* window, const float* g_l1, const float* g_ssim, float* dx,
+                                  const void* workspace, size_t workspace_bytes, void* stream);
+/* normal_loss over n pixels: pred and gt are [n,3] by (pixel, component) element strides (host [2] each).  Each is normalised as
+ * F.normalize does (norm clamped at 1e-12); out[0] = mean |n - g| + 0.1 * (-mean n.g) over the selected pixels: all, or with
+ * depth != NULL those with depth[i * depth_stride] in (0, scene_scale).  No selected pixel gives NaN, as torch's mean of an empty
+ * tensor.  `workspace` (16-byte aligned) needs GSR_LOSS_REDUCE_BYTES; it keeps the selected count for the backward. */
+int gsr_normal_loss(int64_t n, const float* pred, const int64_t* pred_strides, const float* gt, const int64_t* gt_strides,
+                    const float* depth, int64_t depth_stride, float scene_scale, float* out, void* workspace, size_t workspace_bytes,
+                    void* stream);
+/* d_pred (contiguous [n,3]) = g_out[0] * d out / d pred, through normalize's Jacobian (divided by 1e-12 below the clamp); zero for
+ * pixels outside the selection.  `workspace` is the forward's. */
+int gsr_normal_loss_backward(int64_t n, const float* pred, const int64_t* pred_strides, const float* gt, const int64_t* gt_strides,
+                             const float* depth, int64_t depth_stride, float scene_scale, const float* g_out, float* d_pred,
+                             const void* workspace, size_t workspace_bytes, void* stream);
+/* out[0] = mean over P Gaussians of clamp_min(max / (min + 1e-6), r) - r of contiguous scales [P,3].  `workspace` (16-byte aligned)
+ * needs GSR_LOSS_REDUCE_BYTES. */
+int gsr_anisotropic_loss(int64_t P, const float* scales, float r, float* out, void* workspace, size_t workspace_bytes, void* stream);
+/* d_scales [P,3] = g_out[0] * d out / d scales: the max's and the min's gradient go to the first extreme index (NaN first), as
+ * torch's max(dim) / min(dim) return it; nothing where the ratio is below r (clamp_min passes ratio == r).  One thread per Gaussian. */
+int gsr_anisotropic_loss_backward(int64_t P, const float* scales, float r, const float* g_out, float* d_scales, void* stream);
 
 /* Device pointers into the workspaces of the last layout (P, capacity, W, H) — for parity tests that
  * compare per-stage buffers with the reference (SURVEY §4).  Pure pointer arithmetic, no CUDA calls. */
