@@ -87,7 +87,7 @@ EXPORTS = ("gsr_abi_version", "gsr_last_error", "gsr_geom_bytes", "gsr_binning_b
            "gsr_sugar_sdf_normal_backward", "gsr_densify_stats", "gsr_densify_plan_bytes", "gsr_densify_plan", "gsr_densify_apply",
            "gsr_sugar_sample_bytes", "gsr_sugar_sample", "gsr_sugar_sample_backward", "gsr_binning_bytes_slab", "gsr_binning_capacity_slab",
            "gsr_adam_step", "gsr_photometric_loss_bytes", "gsr_photometric_loss", "gsr_photometric_loss_backward", "gsr_normal_loss",
-           "gsr_normal_loss_backward", "gsr_anisotropic_loss", "gsr_anisotropic_loss_backward")
+           "gsr_normal_loss_backward", "gsr_anisotropic_loss", "gsr_anisotropic_loss_backward", "gsr_backward_det_bytes", "gsr_backward_det")
 
 
 def _load() -> C.CDLL:
@@ -151,6 +151,11 @@ def _load() -> C.CDLL:
     lib.gsr_backward_multi.restype = C.c_int
     lib.gsr_backward_multi.argtypes = [C.POINTER(gsr_frame), C.POINTER(gsr_workspace), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(gsr_grads), C.c_void_p]
+    lib.gsr_backward_det_bytes.restype = C.c_size_t
+    lib.gsr_backward_det_bytes.argtypes = [C.c_size_t, C.c_int32, C.c_int32, C.c_int]
+    lib.gsr_backward_det.restype = C.c_int
+    lib.gsr_backward_det.argtypes = [C.POINTER(gsr_frame), C.POINTER(gsr_workspace)] + [C.c_void_p] * 8 + [C.POINTER(gsr_grads), C.c_void_p,
+                                                                                          C.c_size_t, C.c_void_p]
     lib.gsr_mark_visible.restype = C.c_int
     lib.gsr_mark_visible.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.gsr_dist2.restype = C.c_int

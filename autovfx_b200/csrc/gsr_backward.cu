@@ -69,7 +69,11 @@ struct BwdArgs {
     float *dL_dmean2D /*[P,3]*/, *dL_dconic /*[P,4]*/, *dL_dopacity, *dL_dcolors /*[P,3]*/, *dL_ddepths;
     const float *extra /*[P,3]*/, *dL_dpixel_extra /*[3,H,W]*/;  // NX = 3 only
     float* dL_dextra /*[P,3]*/;
+    // DET only: partials of (list entry e, footprint f) at det_slots[(e * 8 + f) * DET_NV(NX)], e < det_cap; footprint warp_last [tiles][8]
+    float* det_slots; uint32_t* det_last; uint32_t det_cap;
 };
+// floats per (list entry, footprint) slot of the deterministic backward: half 0's v0..v4, half 1's v0..v4, then (NX = 3) the second colour
+__host__ __device__ constexpr int det_nv(int nx) { return nx ? 13 : 10; }
 
 constexpr int BWL_WARPS = 4;
 constexpr float BWL_LOG2E = 1.4426950408889634f;
@@ -101,7 +105,21 @@ __device__ __forceinline__ float2 lds64b(uint32_t a) {
     return v;
 }
 
-template <int NX, int OCC>
+// DET: instead of the global reductions every (footprint, survivor) partial is stored in its own slot of a.det_slots, and each
+// warp stores its warp_last, so that k_det_reduce can sum them in a fixed order (DESIGN.md §4, "Deterministic gradients").
+// DET: the slot of the survivor staged at shared address sa (its 1-based list position is at sa + 80) for footprint f; NULL beyond
+// the scratch's capacity
+// the survivor loop keeps neither the tile's list start nor f in a register: they are re-derived (an L1 hit) at each batch
+template <int NX>
+__device__ __forceinline__ float* det_slot(const BwdArgs& a, uint32_t sa) {
+    constexpr int PARTS = GSR_FOOTS / BWL_WARPS;
+    const int f = (int)(blockIdx.x % PARTS) * BWL_WARPS + (int)(threadIdx.x >> 5);
+    const uint32_t range_x = __ldg(&a.ranges[blockIdx.y * a.gx + blockIdx.x / PARTS].x);
+    const uint32_t e = range_x + __float_as_uint(lds32b(sa + 80)) - 1u;
+    return e < a.det_cap ? a.det_slots + ((size_t)e * GSR_FOOTS + f) * det_nv(NX) : nullptr;
+}
+
+template <int NX, int OCC, bool DET>
 __global__ void __launch_bounds__(BWL_WARPS * 32, OCC) k_blend_backward(const BwdArgs a) {
     static_assert(NX == 0 || NX == 3, "the blend backward takes no or one extra colour set");
     typedef BwlCfg<NX> Cfg;
@@ -121,12 +139,16 @@ __global__ void __launch_bounds__(BWL_WARPS * 32, OCC) k_blend_backward(const Bw
     uint32_t* ring = reinterpret_cast<uint32_t*>(sm + (size_t)warp * Cfg::WB + Cfg::REC + Cfg::WS + Cfg::DLP);
 
     const uint2 rg = a.ranges[tile];
-    if (rg.y == rg.x) return;
+    if (rg.y == rg.x) {
+        if (DET && lane == 0) a.det_last[tile * GSR_FOOTS + f] = 0u;
+        return;
+    }
     const size_t pid = (size_t)a.W * pyi + pxi, HW = (size_t)a.H * a.W;
     const uint32_t last_contributor = inside ? a.n_contrib[pid] : 0u;  // 1-based position of the pixel's last contributor
     uint32_t warp_last = last_contributor;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) warp_last = max(warp_last, __shfl_xor_sync(GSR_FULL, warp_last, o));
+    if (DET && lane == 0) a.det_last[tile * GSR_FOOTS + f] = warp_last;
     if (warp_last == 0u) return;  // nothing contributed anywhere in this footprint
 
     // ---- pixel state (phase 1) ----
@@ -373,6 +395,10 @@ __global__ void __launch_bounds__(BWL_WARPS * 32, OCC) k_blend_backward(const Bw
                 gc2 += __shfl_xor_sync(GSR_FULL, gc2, 16); gd += __shfl_xor_sync(GSR_FULL, gd, 16);
                 S0 += __shfl_xor_sync(GSR_FULL, S0, 16); Sx += __shfl_xor_sync(GSR_FULL, Sx, 16); Sy += __shfl_xor_sync(GSR_FULL, Sy, 16);
                 Sxx += __shfl_xor_sync(GSR_FULL, Sxx, 16); Sxy += __shfl_xor_sync(GSR_FULL, Sxy, 16); Syy += __shfl_xor_sync(GSR_FULL, Syy, 16);
+                float* dslot = nullptr;  // DET: this (entry, footprint)'s slot, NULL beyond the scratch's capacity
+                if constexpr (DET) {
+                    if (mine) dslot = det_slot<NX>(a, rec_base + (uint32_t)((sub + j) >> 1) * Cfg::PAIRB + (uint32_t)((sub + j) & 1) * 4);
+                }
                 if constexpr (NX != 0) {
                     // half 0 sends the second colour's r and b, half 1 its g
                     float ge0, ge1;
@@ -380,7 +406,12 @@ __global__ void __launch_bounds__(BWL_WARPS * 32, OCC) k_blend_backward(const Bw
                     const float u = h ? ge1 : ge0, uo = h ? ge0 : ge1;
                     const float v = h ? 0.f : ge2;
                     const float su = u + __shfl_xor_sync(GSR_FULL, uo, 16), sv = v + __shfl_xor_sync(GSR_FULL, ge2, 16);
-                    if (mine) {
+                    if constexpr (DET) {
+                        if (dslot) {
+                            dslot[10 + h] = su;
+                            if (!h) dslot[12] = sv;
+                        }
+                    } else if (mine) {
                         float* const pe = a.dL_dextra + 3 * (size_t)gid;
                         if (su != 0.0f) atomicAdd(pe + h, su);
                         if (!h && sv != 0.0f) atomicAdd(pe + 2, sv);
@@ -394,22 +425,128 @@ __global__ void __launch_bounds__(BWL_WARPS * 32, OCC) k_blend_backward(const Bw
                     const float v2 = h ? 0.5f * nop * Sxy : gc2;
                     const float v3 = h ? 0.5f * nop * Syy : gd;
                     const float v4 = h ? S0 : nop * half_w * fmaf(ca, Sx, cb * Sy);
-                    float* const p0 = h ? a.dL_dmean2D + 3 * (size_t)gid + 1 : a.dL_dcolors + 3 * (size_t)gid;
-                    float* const p1 = h ? a.dL_dconic + 4 * (size_t)gid : a.dL_dcolors + 3 * (size_t)gid + 1;
-                    float* const p2 = h ? a.dL_dconic + 4 * (size_t)gid + 1 : a.dL_dcolors + 3 * (size_t)gid + 2;
-                    float* const p3 = h ? a.dL_dconic + 4 * (size_t)gid + 3 : a.dL_ddepths + gid;
-                    float* const p4 = h ? a.dL_dopacity + gid : a.dL_dmean2D + 3 * (size_t)gid;
-                    if (v0 != 0.0f) atomicAdd(p0, v0);
-                    if (v1 != 0.0f) atomicAdd(p1, v1);
-                    if (v2 != 0.0f) atomicAdd(p2, v2);
-                    if (v3 != 0.0f) atomicAdd(p3, v3);
-                    if (v4 != 0.0f) atomicAdd(p4, v4);
+                    if constexpr (DET) {
+                        if (dslot) {
+                            float* const q = dslot + 5 * h;
+                            q[0] = v0; q[1] = v1; q[2] = v2; q[3] = v3; q[4] = v4;
+                        }
+                    } else {
+                        float* const p0 = h ? a.dL_dmean2D + 3 * (size_t)gid + 1 : a.dL_dcolors + 3 * (size_t)gid;
+                        float* const p1 = h ? a.dL_dconic + 4 * (size_t)gid : a.dL_dcolors + 3 * (size_t)gid + 1;
+                        float* const p2 = h ? a.dL_dconic + 4 * (size_t)gid + 1 : a.dL_dcolors + 3 * (size_t)gid + 2;
+                        float* const p3 = h ? a.dL_dconic + 4 * (size_t)gid + 3 : a.dL_ddepths + gid;
+                        float* const p4 = h ? a.dL_dopacity + gid : a.dL_dmean2D + 3 * (size_t)gid;
+                        if (v0 != 0.0f) atomicAdd(p0, v0);
+                        if (v1 != 0.0f) atomicAdd(p1, v1);
+                        if (v2 != 0.0f) atomicAdd(p2, v2);
+                        if (v3 != 0.0f) atomicAdd(p3, v3);
+                        if (v4 != 0.0f) atomicAdd(p4, v4);
+                    }
+                }
+            } else if constexpr (DET) {
+                // no pixel of the footprint hit any splat of the batch: the batch's partials are zero (k_det_reduce reads every
+                // visited slot, so each is written)
+                float* const q = j < c16 ? det_slot<NX>(a, rec_base + (uint32_t)((sub + j) >> 1) * Cfg::PAIRB + (uint32_t)((sub + j) & 1) * 4)
+                                         : nullptr;
+                if (q) {
+                    for (int c = 5 * h; c < 5 * h + 5; c++) q[c] = 0.f;
+                    if (NX) {
+                        q[10 + h] = 0.f;
+                        if (!h) q[12] = 0.f;
+                    }
                 }
             }
             __syncwarp();  // the (w, s) rows and, after the second batch, the staged records are free again
         }
     }
 }
+
+// -----------------------------------------------------------------------------------------------------------------------
+// Fixed-order reduction of the deterministic backward (k_blend_backward<.., DET = true> filled the slots).
+//
+// One thread per Gaussian.  For every component the result is a sequential fp32 sum from +0.0 over the Gaussian's partials:
+// tiles of its rectangle (recomputed from the record with the forward's tile_rect) in row-major order, then footprints 0..7,
+// counting only the (entry, footprint) pairs the blend backward visited (ballot bit set, list position < warp_last).  The
+// Gaussian's position in a tile list is found by binary search over the list's (depth bits, id) order (k_sort_tiles); a tile
+// that does not list it (tight tiles) is skipped.  Every row of the outputs is written: zeros for culled Gaussians, for the
+// mean2D z slot and for conic slot 2.  A visited slot beyond the scratch's capacity makes the Gaussian's sums NaN.
+// -----------------------------------------------------------------------------------------------------------------------
+struct DetReduceArgs {
+    int P, gx, gy;
+    const int* radii; const uint2* ranges; const uint32_t* point_list; const float4* records; const uint32_t* bal;
+    const float* slots; const uint32_t* last; uint32_t cap;
+    float *dL_dmean2D, *dL_dconic, *dL_dopacity, *dL_dcolors, *dL_ddepths, *dL_dextra;
+};
+
+template <int NX>
+__global__ void __launch_bounds__(128) k_det_reduce(const DetReduceArgs r) {
+    constexpr int NV = det_nv(NX);
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= r.P) return;
+    float acc[NV];
+#pragma unroll
+    for (int c = 0; c < NV; c++) acc[c] = 0.f;
+    if (r.radii[idx] > 0) {
+        const float4 r0 = r.records[3 * (size_t)idx], r1 = r.records[3 * (size_t)idx + 1];
+        const unsigned long long key = ((unsigned long long)__float_as_uint(r1.z) << 32) | (uint32_t)idx;
+        const float* depth_of = reinterpret_cast<const float*>(r.records) + 6;  // depth of Gaussian g: depth_of[12 g]
+        int x0, y0, x1, y1;
+        tile_rect(r0.x, r0.y, __float_as_int(r1.w), r.gx, r.gy, x0, y0, x1, y1);
+        for (int ty = y0; ty < y1; ty++) {
+            for (int tx = x0; tx < x1; tx++) {
+                const int tile = ty * r.gx + tx;
+                const uint2 rg = r.ranges[tile];
+                uint32_t lo = rg.x, hi = rg.y;  // first list entry whose key is >= the Gaussian's
+                while (lo < hi) {
+                    const uint32_t mid = (lo + hi) >> 1, g = r.point_list[mid];
+                    const unsigned long long k = ((unsigned long long)__float_as_uint(depth_of[12 * (size_t)g]) << 32) | g;
+                    if (k < key) lo = mid + 1;
+                    else hi = mid;
+                }
+                if (lo == rg.y || r.point_list[lo] != (uint32_t)idx) continue;  // not in this tile's list (tight tiles)
+                const uint32_t j = lo - rg.x;
+                const uint32_t* row = r.bal + (bal_row_base(rg.x, tile) + (j >> 5)) * GSR_FOOTS;
+                uint32_t bits[GSR_FOOTS];
+#pragma unroll
+                for (int f = 0; f < GSR_FOOTS; f++) bits[f] = row[f];
+                const uint4 l0 = reinterpret_cast<const uint4*>(r.last)[2 * tile], l1 = reinterpret_cast<const uint4*>(r.last)[2 * tile + 1];
+                const uint32_t wl[GSR_FOOTS] = {l0.x, l0.y, l0.z, l0.w, l1.x, l1.y, l1.z, l1.w};
+#pragma unroll
+                for (int f = 0; f < GSR_FOOTS; f++) {
+                    if (!((bits[f] >> (j & 31u)) & 1u) || j >= wl[f]) continue;
+                    if (lo >= r.cap) {
+#pragma unroll
+                        for (int c = 0; c < NV; c++) acc[c] = __int_as_float(0x7fc00000);
+                        continue;
+                    }
+                    const float* s = r.slots + ((size_t)lo * GSR_FOOTS + f) * NV;
+#pragma unroll
+                    for (int c = 0; c < NV; c++) acc[c] = __fadd_rn(acc[c], s[c]);
+                }
+            }
+        }
+    }
+    // slot layout: colour r, g, b, depth, mean2D.x | mean2D.y, conic xx, xy, yy, opacity | second colour r, g, b
+    const size_t i = (size_t)idx;
+    r.dL_dcolors[3 * i] = acc[0]; r.dL_dcolors[3 * i + 1] = acc[1]; r.dL_dcolors[3 * i + 2] = acc[2];
+    r.dL_ddepths[i] = acc[3];
+    r.dL_dmean2D[3 * i] = acc[4]; r.dL_dmean2D[3 * i + 1] = acc[5]; r.dL_dmean2D[3 * i + 2] = 0.f;
+    r.dL_dconic[4 * i] = acc[6]; r.dL_dconic[4 * i + 1] = acc[7]; r.dL_dconic[4 * i + 2] = 0.f; r.dL_dconic[4 * i + 3] = acc[8];
+    r.dL_dopacity[i] = acc[9];
+    if constexpr (NX != 0) { r.dL_dextra[3 * i] = acc[10]; r.dL_dextra[3 * i + 1] = acc[11]; r.dL_dextra[3 * i + 2] = acc[12]; }
+}
+
+// Scratch of the deterministic backward: the [tiles][8] warp_last table, then the slots of every list entry (R of them).
+struct DetLayout {
+    size_t last, slots, total;
+    __host__ __device__ DetLayout(size_t R, int tiles, bool extra) {
+        last = 0;
+        slots = align_up((size_t)tiles * GSR_FOOTS * sizeof(uint32_t), 256);
+        total = slots + R * slot_bytes(extra);
+    }
+    __host__ __device__ static size_t slot_bytes(bool extra) { return (size_t)GSR_FOOTS * det_nv(extra ? 3 : 0) * sizeof(float); }
+};
+size_t backward_det_bytes(size_t R, int W, int H, bool extra) { return DetLayout(R, ImageLayout(W < 1 ? 1 : W, H < 1 ? 1 : H).tiles, extra).total; }
 
 // =====================================================================================================
 // per-Gaussian backward (fused computeCov2DCUDA + preprocessCUDA backward)
@@ -723,18 +860,19 @@ __global__ void __launch_bounds__(GB_THREADS) k_gaussian_backward(const GBParams
 // Resident CTAs per SM the blend backward is compiled for: GSR_BWD_OCC=8|6|5 (64 / 80 / 96 registers), an experiment knob.
 // Default 6 for the plain kernel; 5 for the one with a second colour set, whose three more live values per survivor and per
 // pixel do not fit in 80 registers without spilling.
-template <int NX>
+template <int NX, bool DET>
 static void launch_blend_backward(const BwdArgs& ba, dim3 grid, cudaStream_t st) {
     static int occ = -1;
     if (occ < 0) { const char* e = getenv("GSR_BWD_OCC"); occ = e ? atoi(e) : 0; }
-    if (occ == 8) k_blend_backward<NX, 8><<<grid, BWL_WARPS * 32, 0, st>>>(ba);
-    else if (occ == 5 || (NX && occ != 6)) k_blend_backward<NX, 5><<<grid, BWL_WARPS * 32, 0, st>>>(ba);
-    else k_blend_backward<NX, 6><<<grid, BWL_WARPS * 32, 0, st>>>(ba);
+    if (occ == 8) k_blend_backward<NX, 8, DET><<<grid, BWL_WARPS * 32, 0, st>>>(ba);
+    else if (occ == 5 || (NX && occ != 6)) k_blend_backward<NX, 5, DET><<<grid, BWL_WARPS * 32, 0, st>>>(ba);
+    else k_blend_backward<NX, 6, DET><<<grid, BWL_WARPS * 32, 0, st>>>(ba);
 }
 
+// det: the deterministic backward (gsr_backward_det) with `scratch` of scratch_bytes; otherwise scratch is unused.
 int backward_impl(const gsr_frame* f, const gsr_workspace* ws, const int32_t* radii, const float* out_alpha, const float* dL_dc,
                   const float* dL_dd, const float* dL_da, const float* extra_colors, const float* dL_de, float* dL_dextra,
-                  const gsr_grads* g, cudaStream_t st) {
+                  const gsr_grads* g, bool det, void* scratch, size_t scratch_bytes, cudaStream_t st) {
     if (!f || !ws || !g) { set_error("gsr_backward: null argument"); return GSR_ERR_INVALID; }
     const int n_extra = (extra_colors != nullptr) + (dL_de != nullptr) + (dL_dextra != nullptr);
     if (n_extra != 0 && n_extra != 3) {
@@ -750,13 +888,24 @@ int backward_impl(const gsr_frame* f, const gsr_workspace* ws, const int32_t* ra
     }
     if (f->shs && !g->dL_dsh) { set_error("gsr_backward: dL_dsh missing"); return GSR_ERR_INVALID; }
     if (f->scales && (!g->dL_dscales || !g->dL_drotations)) { set_error("gsr_backward: dL_dscales/dL_drotations missing"); return GSR_ERR_INVALID; }
-    // accumulated gradients start from zero
-    cudaMemsetAsync(g->dL_dmeans2D, 0, 12 * P, st);
-    cudaMemsetAsync(g->dL_dconic, 0, 16 * P, st);
-    cudaMemsetAsync(g->dL_dopacity, 0, 4 * P, st);
-    cudaMemsetAsync(g->dL_dcolors, 0, 12 * P, st);
-    cudaMemsetAsync(g->dL_ddepths, 0, 4 * P, st);
-    if (multi) cudaMemsetAsync(dL_dextra, 0, 12 * P, st);
+    if (det) {  // every argument is checked before anything is enqueued; no memset: k_det_reduce writes every row
+        if (!scratch) { set_error("gsr_backward_det: scratch is NULL"); return GSR_ERR_INVALID; }
+        if ((uintptr_t)scratch & 15) { set_error("gsr_backward_det: scratch is not 16-byte aligned"); return GSR_ERR_INVALID; }
+        if (f->P > 0 && (!radii || !out_alpha || !dL_dc || !dL_dd || !dL_da)) { set_error("gsr_backward_det: null input"); return GSR_ERR_INVALID; }
+        if (scratch_bytes < backward_det_bytes(0, f->W, f->H, multi)) {
+            set_error("gsr_backward_det: scratch of %zu bytes is too small: gsr_backward_det_bytes(num_rendered, W, H, with_extra) = "
+                      "%zu + %zu per rendered instance", scratch_bytes, backward_det_bytes(0, f->W, f->H, multi), DetLayout::slot_bytes(multi));
+            return GSR_ERR_WORKSPACE;
+        }
+    }
+    if (!det) {  // accumulated gradients start from zero
+        cudaMemsetAsync(g->dL_dmeans2D, 0, 12 * P, st);
+        cudaMemsetAsync(g->dL_dconic, 0, 16 * P, st);
+        cudaMemsetAsync(g->dL_dopacity, 0, 4 * P, st);
+        cudaMemsetAsync(g->dL_dcolors, 0, 12 * P, st);
+        cudaMemsetAsync(g->dL_ddepths, 0, 4 * P, st);
+        if (multi) cudaMemsetAsync(dL_dextra, 0, 12 * P, st);
+    }
     if (P == 0) return check_launch("gsr_backward(P=0)", debug, st);
     if (!radii || !out_alpha || !dL_dc || !dL_dd || !dL_da) { set_error("gsr_backward: null input"); return GSR_ERR_INVALID; }
     const ImageLayout il(f->W, f->H);
@@ -773,10 +922,34 @@ int backward_impl(const gsr_frame* f, const gsr_workspace* ws, const int32_t* ra
     ba.dL_dpixels = dL_dc; ba.dL_dpixel_depths = dL_dd; ba.dL_dpixel_alphas = dL_da;
     ba.dL_dmean2D = g->dL_dmeans2D; ba.dL_dconic = g->dL_dconic; ba.dL_dopacity = g->dL_dopacity; ba.dL_dcolors = g->dL_dcolors; ba.dL_ddepths = g->dL_ddepths;
     ba.extra = extra_colors; ba.dL_dpixel_extra = dL_de; ba.dL_dextra = dL_dextra;
+    ba.det_slots = nullptr; ba.det_last = nullptr; ba.det_cap = 0;
+    if (det) {
+        const DetLayout dl(0, il.tiles, multi);
+        const size_t cap = (scratch_bytes - dl.slots) / DetLayout::slot_bytes(multi);  // list entries whose slots fit
+        ba.det_cap = (uint32_t)(cap < 0xffffffffull ? cap : 0xffffffffull);
+        ba.det_last = (uint32_t*)((char*)scratch + dl.last);
+        ba.det_slots = (float*)((char*)scratch + dl.slots);
+    }
     {
         const dim3 grid(il.gx * (GSR_FOOTS / BWL_WARPS), il.gy);
-        if (multi) launch_blend_backward<3>(ba, grid, st);
-        else launch_blend_backward<0>(ba, grid, st);
+        if (det) {
+            if (multi) launch_blend_backward<3, true>(ba, grid, st);
+            else launch_blend_backward<0, true>(ba, grid, st);
+        } else {
+            if (multi) launch_blend_backward<3, false>(ba, grid, st);
+            else launch_blend_backward<0, false>(ba, grid, st);
+        }
+    }
+    if (det) {
+        DetReduceArgs ra;
+        ra.P = f->P; ra.gx = il.gx; ra.gy = il.gy;
+        ra.radii = radii; ra.ranges = ba.ranges; ra.point_list = ba.point_list; ra.records = ba.records; ra.bal = ba.bal;
+        ra.slots = ba.det_slots; ra.last = ba.det_last; ra.cap = ba.det_cap;
+        ra.dL_dmean2D = g->dL_dmeans2D; ra.dL_dconic = g->dL_dconic; ra.dL_dopacity = g->dL_dopacity; ra.dL_dcolors = g->dL_dcolors;
+        ra.dL_ddepths = g->dL_ddepths; ra.dL_dextra = dL_dextra;
+        const int blocks = (f->P + 127) / 128;
+        if (multi) k_det_reduce<3><<<blocks, 128, 0, st>>>(ra);
+        else k_det_reduce<0><<<blocks, 128, 0, st>>>(ra);
     }
     int rc = check_launch("gsr_backward/blend", debug, st);
     if (rc) return rc;

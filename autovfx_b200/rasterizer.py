@@ -27,6 +27,7 @@ from typing import Dict, NamedTuple, Optional, Tuple
 
 import torch
 import torch.nn as nn
+import torch.utils.deterministic
 
 from . import _lib
 from ._lib import lib as _L
@@ -115,11 +116,12 @@ def get_tight_tiles() -> bool:
 class FrameTicket:
     """Handle on the device-side counters of one forward call (gsr_counters, include/gsr_b200.h)."""
 
-    __slots__ = ("event", "slot", "capacity", "_state", "_snap", "__weakref__")
+    __slots__ = ("event", "slot", "capacity", "_state", "_snap", "binned", "__weakref__")
 
     def __init__(self, event, slot, capacity, state):
         self.event, self.slot, self.capacity, self._state = event, slot, capacity, state
         self._snap = None
+        self.binned = None  # safe mode: the ticket of the frame's binning half, whose counters the host has already read
 
     def ready(self) -> bool:
         return self.event.query()
@@ -138,6 +140,11 @@ class FrameTicket:
         return {"num_rendered": int(c[0]), "overflow": int(c[1]), "max_tile": int(c[2]), "trapped": int(c[3]),
                 "num_visible": int(c[4]), "foot_total": int(c[5]) & 0xffffffff, "exact_redos": int(c[6]),
                 "capacity": int(self.capacity)}
+
+    def num_rendered(self) -> int:
+        """Instances the frame rendered.  In safe mode it comes from the counters the forward already read, so it does not wait
+        for the rest of the frame."""
+        return (self.binned if self.binned is not None else self).stats()["num_rendered"]
 
     def ok(self) -> bool:
         s = self.stats()
@@ -446,6 +453,8 @@ def forward_raw(means3D, shs, colors_precomp, opacities, scales, rotations, cov3
                 if s["trapped"]:
                     raise RuntimeError("Point is filtered although prefiltered is set. This shouldn't happen!")  # auxiliary.h:158
                 if not s["overflow"]:
+                    if check is not ticket:
+                        ticket.binned = check
                     break
                 st.grow(needed_capacity(s))  # rare: first frames of a new scene; re-run with a larger binning buffer
                 st.grow_slab(s["max_tile"])
@@ -557,6 +566,18 @@ class PreparedForward:
         return st.issue_ticket(self._counters, stream, self._capacity_instances)
 
 
+def _scratch_bytes(nbytes: int, device: torch.device) -> torch.Tensor:
+    """A byte buffer from the caching allocator, without the NaN fill torch gives every torch.empty under
+    use_deterministic_algorithms: gsr_backward_det writes every scratch byte it reads, and a fill of gigabytes would cost about
+    as much as the backward itself."""
+    fill = torch.utils.deterministic.fill_uninitialized_memory
+    torch.utils.deterministic.fill_uninitialized_memory = False
+    try:
+        return torch.empty(nbytes, dtype=torch.uint8, device=device)
+    finally:
+        torch.utils.deterministic.fill_uninitialized_memory = fill
+
+
 def _cpu_copy(items):
     """CPU clones of the tensors in ``items`` (the reference's cpu_deep_copy_tuple, __init__.py:16-18)."""
     return tuple(x.detach().cpu().clone() if isinstance(x, torch.Tensor) else x for x in items)
@@ -639,7 +660,9 @@ class _RasterizeGaussians(torch.autograd.Function):
     def backward(ctx, grad_out_color, grad_out_depth, grad_out_alpha, *grad_out_rest):
         """gsr_backward, or gsr_backward_multi when the extra image has a gradient.  Returns the gradients in the reference's order
         (__init__.py:146-156): means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp (None for an
-        absent input), None for raster_settings and need_bw, then dL/dextra_colors (None without an extra-image gradient)."""
+        absent input), None for raster_settings and need_bw, then dL/dextra_colors (None without an extra-image gradient).
+        Under ``torch.use_deterministic_algorithms(True)`` both go through gsr_backward_det instead: every gradient is then
+        bit-identical from call to call (INTEGRATION.md, "Deterministic gradients")."""
         if not ctx.needs:
             return (None,) * 11
         grad_out_extra = grad_out_rest[0] if len(grad_out_rest) == 2 else None  # (extra image's, radii's) or (radii's,)
@@ -681,21 +704,29 @@ class _RasterizeGaussians(torch.autograd.Function):
             gr = _lib.gsr_grads(_ptr(dL_dmeans2D), _ptr(dL_dconic), _ptr(dL_dopacity), _ptr(dL_dcolors), _ptr(dL_ddepths),
                                 _ptr(dL_dmeans3D), _ptr(dL_dcov3D), _ptr(dL_dsh), _ptr(dL_dscales), _ptr(dL_drotations))
             stream = _lib.stream_ptr(device)
-            if multi:
-                extra = ctx.saved_tensors[15]
-                g_extra = _dev_f32(grad_out_extra, device)
-                dL_dextra = torch.empty((P, 3), **f32)
+            extra = ctx.saved_tensors[15] if multi else None
+            g_extra = _dev_f32(grad_out_extra, device) if multi else None
+            dL_dextra = torch.empty((P, 3), **f32) if multi else None
+            if torch.are_deterministic_algorithms_enabled():
+                nbytes = _L.gsr_backward_det_bytes(ctx.ticket.num_rendered(), W, H, int(multi))
+                scratch = _scratch_bytes(nbytes, device)
+                rc = _L.gsr_backward_det(C.byref(fr), C.byref(ws), _ptr(radii), _ptr(alpha), _ptr(g_color), _ptr(g_depth), _ptr(g_alpha),
+                                         _ptr(extra), _ptr(g_extra), _ptr(dL_dextra), C.byref(gr), scratch.data_ptr(), nbytes, stream)
+                what = "gsr_backward_det"
+            elif multi:
                 rc = _L.gsr_backward_multi(C.byref(fr), C.byref(ws), _ptr(radii), _ptr(alpha), _ptr(g_color), _ptr(g_depth), _ptr(g_alpha),
                                            _ptr(extra), _ptr(g_extra), _ptr(dL_dextra), C.byref(gr), stream)
+                what = "gsr_backward_multi"
             else:
                 rc = _L.gsr_backward(C.byref(fr), C.byref(ws), _ptr(radii), _ptr(alpha), _ptr(g_color), _ptr(g_depth), _ptr(g_alpha),
                                      C.byref(gr), stream)
+                what = "gsr_backward"
             if rc != 0 and s.debug:  # reference debug behaviour (__init__.py:135-142)
                 torch.save(_cpu_copy((bg, means3D, radii, colors_precomp, scales, rotations, s.scale_modifier, cov3Ds_precomp, view, proj,
                                       s.tanfovx, s.tanfovy, g_color, g_depth, g_alpha, sh, s.sh_degree, campos, alpha, s.debug)
                                      + ((extra, g_extra) if multi else ())), "snapshot_bw.dump")
                 print("\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
-            _lib.check(rc, "gsr_backward_multi" if multi else "gsr_backward")
+            _lib.check(rc, what)
         return (dL_dmeans3D, dL_dmeans2D, dL_dsh if has_sh else None, dL_dcolors if has_col else None, dL_dopacity,
                 dL_dscales if has_scale else None, dL_drotations if has_scale else None, dL_dcov3D if has_cov else None,
                 None, None, dL_dextra if multi else None)

@@ -298,6 +298,23 @@ int gsr_backward_multi(const gsr_frame* frame, const gsr_workspace* ws, const in
                        const float* extra_colors, const float* dL_dout_extra, float* dL_dextra,
                        const gsr_grads* grads, void* stream);
 
+/* Deterministic backward: the arguments of gsr_backward_multi (the three extra pointers all NULL or all given, as there) plus a
+ * device scratch (16-byte aligned) of at least gsr_backward_det_bytes(num_rendered, W, H, extra_colors != NULL) bytes, where
+ * num_rendered is the forward's gsr_counters.num_rendered.  Every gradient is bit-identical from call to call, whatever the CTA
+ * scheduling, the concurrent streams or the blend backward's register budget: each component of dL_dmeans2D, dL_dconic,
+ * dL_dopacity, dL_dcolors, dL_ddepths and dL_dextra is a sequential fp32 sum from +0.0 of the per-(footprint, splat) partials in
+ * a fixed order (tiles of the Gaussian's tile rectangle row-major, then footprints 0..7; DESIGN.md §4), and the rest of the
+ * backward is per Gaussian.  The values agree with gsr_backward's to rounding, not bit for bit.  The library writes every row of
+ * the gradient buffers itself (no zero-fill is needed) and never reads a scratch byte it has not written in the same call.
+ * A NULL or misaligned scratch is GSR_ERR_INVALID; one smaller than gsr_backward_det_bytes(0, W, H, with_extra) is
+ * GSR_ERR_WORKSPACE.  Both are reported before anything is enqueued.  A scratch sized for fewer instances than the frame rendered
+ * is never written beyond its end; the Gaussians whose partials did not fit get NaN gradients. */
+size_t gsr_backward_det_bytes(size_t num_rendered, int32_t W, int32_t H, int with_extra);
+int gsr_backward_det(const gsr_frame* frame, const gsr_workspace* ws, const int32_t* radii, const float* out_alpha,
+                     const float* dL_dout_color, const float* dL_dout_depth, const float* dL_dout_alpha,
+                     const float* extra_colors, const float* dL_dout_extra, float* dL_dextra,
+                     const gsr_grads* grads, void* scratch, size_t scratch_bytes, void* stream);
+
 /* present[i] = (view-space z of means3D[i] > 0.2)  — checkFrustum, rasterizer_impl.cu:54-66. */
 int gsr_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,
                      uint8_t* present, void* stream);
