@@ -9,6 +9,7 @@ import ctypes as C
 import os
 
 import torch
+import torch.utils.deterministic
 
 from . import build as _build
 
@@ -87,7 +88,9 @@ EXPORTS = ("gsr_abi_version", "gsr_last_error", "gsr_geom_bytes", "gsr_binning_b
            "gsr_sugar_sdf_normal_backward", "gsr_densify_stats", "gsr_densify_plan_bytes", "gsr_densify_plan", "gsr_densify_apply",
            "gsr_sugar_sample_bytes", "gsr_sugar_sample", "gsr_sugar_sample_backward", "gsr_binning_bytes_slab", "gsr_binning_capacity_slab",
            "gsr_adam_step", "gsr_photometric_loss_bytes", "gsr_photometric_loss", "gsr_photometric_loss_backward", "gsr_normal_loss",
-           "gsr_normal_loss_backward", "gsr_anisotropic_loss", "gsr_anisotropic_loss_backward", "gsr_backward_det_bytes", "gsr_backward_det")
+           "gsr_normal_loss_backward", "gsr_anisotropic_loss", "gsr_anisotropic_loss_backward", "gsr_backward_det_bytes", "gsr_backward_det",
+           "gsr_sugar_field_backward_det_bytes", "gsr_sugar_field_backward_det", "gsr_sugar_sdf_normal_backward_det_bytes",
+           "gsr_sugar_sdf_normal_backward_det", "gsr_sugar_sample_backward_det_bytes", "gsr_sugar_sample_backward_det")
 
 
 def _load() -> C.CDLL:
@@ -169,11 +172,19 @@ def _load() -> C.CDLL:
     lib.gsr_sugar_field_backward.restype = C.c_int
     lib.gsr_sugar_field_backward.argtypes = ([C.c_int32] * 4 + [C.c_void_p] * 7 + [C.c_float] * 3 + [C.c_void_p] * 10 +
                                              [C.c_size_t, C.c_void_p])
+    lib.gsr_sugar_field_backward_det_bytes.restype = C.c_size_t
+    lib.gsr_sugar_field_backward_det_bytes.argtypes = [C.c_int32] * 3
+    lib.gsr_sugar_field_backward_det.restype = C.c_int
+    lib.gsr_sugar_field_backward_det.argtypes = lib.gsr_sugar_field_backward.argtypes
     lib.gsr_sugar_sdf_normal_bytes.argtypes = [C.c_int32]
     lib.gsr_sugar_sdf_normal.restype = C.c_int
     lib.gsr_sugar_sdf_normal.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 9 + [C.c_void_p, C.c_size_t, C.c_void_p]
     lib.gsr_sugar_sdf_normal_backward.restype = C.c_int
     lib.gsr_sugar_sdf_normal_backward.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 12 + [C.c_void_p, C.c_size_t, C.c_void_p]
+    lib.gsr_sugar_sdf_normal_backward_det_bytes.restype = C.c_size_t
+    lib.gsr_sugar_sdf_normal_backward_det_bytes.argtypes = [C.c_int32] * 3 + [C.c_int]
+    lib.gsr_sugar_sdf_normal_backward_det.restype = C.c_int
+    lib.gsr_sugar_sdf_normal_backward_det.argtypes = lib.gsr_sugar_sdf_normal_backward.argtypes
     lib.gsr_densify_stats.restype = C.c_int
     lib.gsr_densify_stats.argtypes = [C.c_int32] * 2 + [C.c_void_p] * 7
     lib.gsr_densify_plan_bytes.argtypes = [C.c_int32]
@@ -187,6 +198,10 @@ def _load() -> C.CDLL:
     lib.gsr_sugar_sample.argtypes = ([C.c_int32] * 2 + [C.c_float, C.c_int32] + [C.c_void_p] * 10 + [C.c_void_p, C.c_size_t, C.c_void_p])
     lib.gsr_sugar_sample_backward.restype = C.c_int
     lib.gsr_sugar_sample_backward.argtypes = [C.c_int32] * 2 + [C.c_float] + [C.c_void_p] * 10
+    lib.gsr_sugar_sample_backward_det_bytes.restype = C.c_size_t
+    lib.gsr_sugar_sample_backward_det_bytes.argtypes = [C.c_int32] * 2
+    lib.gsr_sugar_sample_backward_det.restype = C.c_int
+    lib.gsr_sugar_sample_backward_det.argtypes = [C.c_int32] * 2 + [C.c_float] + [C.c_void_p] * 9 + [C.c_void_p, C.c_size_t, C.c_void_p]
     lib.gsr_adam_step.restype = C.c_int
     lib.gsr_adam_step.argtypes = [C.c_int32, C.POINTER(gsr_adam_tensor), C.c_void_p]
     lib.gsr_photometric_loss_bytes.restype = C.c_size_t
@@ -229,6 +244,18 @@ for _kv in filter(None, os.environ.get("GSR_OPTIONS", "").split(",")):
 def check(rc: int, what: str) -> None:
     if rc != 0:
         raise RuntimeError("%s failed (%d): %s" % (what, rc, lib.gsr_last_error().decode("utf-8", "replace")))
+
+
+def scratch_bytes(nbytes: int, device: torch.device) -> torch.Tensor:
+    """A byte buffer from the caching allocator, without the NaN fill torch gives every torch.empty under
+    use_deterministic_algorithms: the library's deterministic backwards (gsr_backward_det, gsr_sugar_*_backward_det) write every
+    scratch byte they read, and a fill of gigabytes would cost about as much as the backward itself."""
+    fill = torch.utils.deterministic.fill_uninitialized_memory
+    torch.utils.deterministic.fill_uninitialized_memory = False
+    try:
+        return torch.empty(nbytes, dtype=torch.uint8, device=device)
+    finally:
+        torch.utils.deterministic.fill_uninitialized_memory = fill
 
 
 def stream_ptr(device) -> C.c_void_p:

@@ -54,7 +54,8 @@ int sugar_field_backward_impl(int N, int K, int P, int R, const float* x, const 
                               const float* points, const float* scaling, const float* quaternions, const float* strengths,
                               float density_factor, float opacity_min_clamp, float sdf_offset, const float* g_density, const float* g_opac,
                               const float* g_beta, const float* g_sdf, float* dx, float* d_points, float* d_scaling, float* d_quaternions,
-                              float* d_strengths, void* ws, size_t ws_bytes, cudaStream_t st);
+                              float* d_strengths, void* ws, size_t ws_bytes, bool det, cudaStream_t st);
+size_t sugar_field_backward_det_bytes(int N, int K, int P);
 size_t sugar_sdf_normal_bytes(int P);
 int sugar_sdf_normal_impl(int N, int K, int P, const float* x, const int64_t* gidx, const int64_t* knn, const float* points,
                           const float* scaling, const float* quaternions, const float* opac, float* out_loss, float* out_est, void* ws,
@@ -62,7 +63,8 @@ int sugar_sdf_normal_impl(int N, int K, int P, const float* x, const int64_t* gi
 int sugar_sdf_normal_backward_impl(int N, int K, int P, const float* x, const int64_t* gidx, const int64_t* knn, const float* points,
                                    const float* scaling, const float* quaternions, const float* opac, const float* g_loss,
                                    const float* g_est, float* dx, float* d_points, float* d_quaternions, void* ws, size_t ws_bytes,
-                                   cudaStream_t st);
+                                   bool det, cudaStream_t st);
+size_t sugar_sdf_normal_backward_det_bytes(int N, int K, int P, bool with_loss);
 int densify_stats_impl(int P, int C, const float* grad, const uint8_t* mask, const int32_t* radii, float* accum, float* denom,
                        float* max_radii, cudaStream_t st);
 size_t densify_plan_bytes(int P);
@@ -92,7 +94,8 @@ int sugar_sample_impl(int N, int P, float f, int volume, const uint8_t* mask, co
                       double* out_total, void* ws, size_t ws_bytes, cudaStream_t st);
 int sugar_sample_backward_impl(int N, int P, float f, const int64_t* idx, const float* z, const float* scaling, const float* quaternions,
                                const double* total, const float* dL_dsamples, float* d_points, float* d_scaling, float* d_quaternions,
-                               cudaStream_t st);
+                               bool det, void* scratch, size_t scratch_bytes, cudaStream_t st);
+size_t sugar_sample_backward_det_bytes(int N, int P);
 int profile_begin(int max_frames, int stride);
 int set_option(const char* name, int value);
 int profile_end(float* ms, int* frames);
@@ -276,7 +279,20 @@ int gsr_sugar_field_backward(int32_t N, int32_t K, int32_t P, int32_t R, const f
     NvtxRange nvtx_("gsr_sugar_field_backward");
     return gsr::sugar_field_backward_impl(N, K, P, R, x, rows, row_idx, points, scaling, quaternions, strengths, density_factor,
                                           opacity_min_clamp, sdf_offset, dL_ddensity, dL_dopacities, dL_dbeta, dL_dsdf, dL_dx, dL_dpoints,
-                                          dL_dscaling, dL_dquaternions, dL_dstrengths, workspace, workspace_bytes, (cudaStream_t)stream);
+                                          dL_dscaling, dL_dquaternions, dL_dstrengths, workspace, workspace_bytes, false, (cudaStream_t)stream);
+}
+
+size_t gsr_sugar_field_backward_det_bytes(int32_t N, int32_t K, int32_t P) { return gsr::sugar_field_backward_det_bytes(N, K, P); }
+int gsr_sugar_field_backward_det(int32_t N, int32_t K, int32_t P, int32_t R, const float* x, const int64_t* rows, const int64_t* row_idx,
+                                 const float* points, const float* scaling, const float* quaternions, const float* strengths,
+                                 float density_factor, float opacity_min_clamp, float sdf_offset, const float* dL_ddensity,
+                                 const float* dL_dopacities, const float* dL_dbeta, const float* dL_dsdf, float* dL_dx, float* dL_dpoints,
+                                 float* dL_dscaling, float* dL_dquaternions, float* dL_dstrengths, void* scratch, size_t scratch_bytes,
+                                 void* stream) {
+    NvtxRange nvtx_("gsr_sugar_field_backward_det");
+    return gsr::sugar_field_backward_impl(N, K, P, R, x, rows, row_idx, points, scaling, quaternions, strengths, density_factor,
+                                          opacity_min_clamp, sdf_offset, dL_ddensity, dL_dopacities, dL_dbeta, dL_dsdf, dL_dx, dL_dpoints,
+                                          dL_dscaling, dL_dquaternions, dL_dstrengths, scratch, scratch_bytes, true, (cudaStream_t)stream);
 }
 
 size_t gsr_sugar_sdf_normal_bytes(int32_t P) { return gsr::sugar_sdf_normal_bytes(P); }
@@ -293,7 +309,19 @@ int gsr_sugar_sdf_normal_backward(int32_t N, int32_t K, int32_t P, const float* 
                                   float* dL_dquaternions, void* workspace, size_t workspace_bytes, void* stream) {
     NvtxRange nvtx_("gsr_sugar_sdf_normal_backward");
     return gsr::sugar_sdf_normal_backward_impl(N, K, P, x, gidx, knn_idx, points, scaling, quaternions, opacities, dL_dloss, dL_destimate,
-                                               dL_dx, dL_dpoints, dL_dquaternions, workspace, workspace_bytes, (cudaStream_t)stream);
+                                               dL_dx, dL_dpoints, dL_dquaternions, workspace, workspace_bytes, false, (cudaStream_t)stream);
+}
+
+size_t gsr_sugar_sdf_normal_backward_det_bytes(int32_t N, int32_t K, int32_t P, int with_loss) {
+    return gsr::sugar_sdf_normal_backward_det_bytes(N, K, P, with_loss != 0);
+}
+int gsr_sugar_sdf_normal_backward_det(int32_t N, int32_t K, int32_t P, const float* x, const int64_t* gidx, const int64_t* knn_idx,
+                                      const float* points, const float* scaling, const float* quaternions, const float* opacities,
+                                      const float* dL_dloss, const float* dL_destimate, float* dL_dx, float* dL_dpoints,
+                                      float* dL_dquaternions, void* scratch, size_t scratch_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_sugar_sdf_normal_backward_det");
+    return gsr::sugar_sdf_normal_backward_impl(N, K, P, x, gidx, knn_idx, points, scaling, quaternions, opacities, dL_dloss, dL_destimate,
+                                               dL_dx, dL_dpoints, dL_dquaternions, scratch, scratch_bytes, true, (cudaStream_t)stream);
 }
 
 int gsr_densify_stats(int32_t P, int32_t C, const float* grad, const uint8_t* mask, const int32_t* radii, float* accum, float* denom,
@@ -329,7 +357,17 @@ int gsr_sugar_sample_backward(int32_t N, int32_t P, float sampling_scale_factor,
                               float* dL_dscaling, float* dL_dquaternions, void* stream) {
     NvtxRange nvtx_("gsr_sugar_sample_backward");
     return gsr::sugar_sample_backward_impl(N, P, sampling_scale_factor, idx, z, scaling, quaternions, total, dL_dsamples, dL_dpoints,
-                                           dL_dscaling, dL_dquaternions, (cudaStream_t)stream);
+                                           dL_dscaling, dL_dquaternions, false, nullptr, 0, (cudaStream_t)stream);
+}
+
+size_t gsr_sugar_sample_backward_det_bytes(int32_t N, int32_t P) { return gsr::sugar_sample_backward_det_bytes(N, P); }
+int gsr_sugar_sample_backward_det(int32_t N, int32_t P, float sampling_scale_factor, const int64_t* idx, const float* z,
+                                  const float* scaling, const float* quaternions, const double* total, const float* dL_dsamples,
+                                  float* dL_dpoints, float* dL_dscaling, float* dL_dquaternions, void* scratch, size_t scratch_bytes,
+                                  void* stream) {
+    NvtxRange nvtx_("gsr_sugar_sample_backward_det");
+    return gsr::sugar_sample_backward_impl(N, P, sampling_scale_factor, idx, z, scaling, quaternions, total, dL_dsamples, dL_dpoints,
+                                           dL_dscaling, dL_dquaternions, true, scratch, scratch_bytes, (cudaStream_t)stream);
 }
 
 int gsr_adam_step(int32_t n, const gsr_adam_tensor* tensors, void* stream) {

@@ -12,12 +12,12 @@
 //     bound or than the current third-best) is applied to the box and then to its sub-boxes, and only surviving 64-point
 //     sub-boxes are scanned.  Pruning is conservative at every level, so the three smallest distances are exact.
 // No host round trip (the reference makes two blocking cudaMemcpy's of the bounding box, :197,:200), no cudaMalloc/cudaFree, no
-// Thrust/CUB: the bounding box stays on the device, and the (morton, index) sort is a small hand-written stable LSD radix sort
+// Thrust/CUB: the bounding box stays on the device, and the (morton, index) sort is the library's stable LSD radix sort (gsr_radix.cuh)
 // (one warp per 2048-key chunk, warp match_any ranking).  Init-time only (gaussian_model.py:144).
 //
 // gsr_knn (below k_knn_search) runs the same pipeline for pytorch3d.ops.knn_points as SuGaR calls it: the K <= 32 nearest points
 // of every query, the query set being the points themselves or a second cloud.
-#include "gsr_common.cuh"
+#include "gsr_radix.cuh"
 #include <cfloat>
 
 namespace gsr {
@@ -26,7 +26,7 @@ constexpr int KNN_BOX = 1024;
 constexpr int KNN_SUB = 64;      // points per sub-box (16 per box)
 constexpr int KNN_QCTA = 256;    // queries per CTA of the search kernel
 constexpr int KNN_MAXC = 1024;   // candidate boxes a CTA can list; beyond that it falls back to testing every box
-constexpr int KNN_CHUNK = 2048;  // keys per warp in the radix sort
+constexpr int KNN_CHUNK = RS_CHUNK;  // keys per warp in the radix sort (gsr_radix.cuh)
 
 struct KnnLayout {
     size_t bbox, codes0, codes1, idx0, idx1, hist, boxes, subboxes, sorted, total;
@@ -105,54 +105,6 @@ __global__ void __launch_bounds__(256) k_morton(int P, const float* __restrict__
     const uint32_t z = prep_morton(((c.z - mnz) / (mxz - mnz)) * ((1 << 10) - 1));
     codes[i] = x | (y << 1) | (z << 2);
     idx[i] = (uint32_t)i;
-}
-
-// ---- stable LSD radix sort, 8-bit digits, one warp per chunk of KNN_CHUNK consecutive keys ----
-constexpr int RS_WARPS = 4;
-__global__ void __launch_bounds__(RS_WARPS * 32) k_rs_hist(int P, const uint32_t* __restrict__ keys, int shift, int nchunks,
-                                                           uint32_t* __restrict__ hist) {
-    __shared__ uint32_t cnt[RS_WARPS][256];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int chunk = blockIdx.x * RS_WARPS + warp;
-    for (int d = lane; d < 256; d += 32) cnt[warp][d] = 0;
-    __syncwarp();
-    if (chunk < nchunks) {
-        const int b = chunk * KNN_CHUNK, e = min(P, b + KNN_CHUNK);
-        for (int i = b + lane; i < e; i += 32) atomicAdd(&cnt[warp][(keys[i] >> shift) & 255u], 1u);
-        __syncwarp();
-        for (int d = lane; d < 256; d += 32) hist[(size_t)d * nchunks + chunk] = cnt[warp][d];
-    }
-}
-__global__ void __launch_bounds__(RS_WARPS * 32) k_rs_scatter(int P, const uint32_t* __restrict__ keys, const uint32_t* __restrict__ vals,
-                                                              int shift, int nchunks, const uint32_t* __restrict__ hist,
-                                                              uint32_t* __restrict__ keys_out, uint32_t* __restrict__ vals_out) {
-    __shared__ uint32_t off[RS_WARPS][256];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int chunk = blockIdx.x * RS_WARPS + warp;
-    if (chunk >= nchunks) return;
-    for (int d = lane; d < 256; d += 32) off[warp][d] = hist[(size_t)d * nchunks + chunk];
-    __syncwarp();
-    const int b = chunk * KNN_CHUNK, e = min(P, b + KNN_CHUNK);
-    for (int i0 = b; i0 < e; i0 += 32) {
-        const int i = i0 + lane;
-        const bool act = i < e;
-        const uint32_t k = act ? keys[i] : 0u, v = act ? vals[i] : 0u;
-        const uint32_t d = act ? ((k >> shift) & 255u) : 256u + lane;  // inactive lanes get unique pseudo-digits
-        const unsigned peers = __match_any_sync(GSR_FULL, d);
-        const int leader = __ffs(peers) - 1;
-        const uint32_t rank = __popc(peers & ((1u << lane) - 1u));
-        uint32_t basepos = 0;
-        if (act && lane == leader) {
-            basepos = off[warp][d];
-            off[warp][d] = basepos + __popc(peers);
-        }
-        basepos = __shfl_sync(GSR_FULL, basepos, leader);
-        if (act) {
-            keys_out[basepos + rank] = k;
-            vals_out[basepos + rank] = v;
-        }
-        __syncwarp();
-    }
 }
 
 // ---- points in Morton order, box and sub-box AABBs ----

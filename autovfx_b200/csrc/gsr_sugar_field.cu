@@ -11,11 +11,14 @@
 //                     accumulates the record gradients of every pair into a per-Gaussian 64-byte scratch with 16-byte RED.ADDs
 //   k_field_chain     one thread per Gaussian: record gradients -> dL/dpoints, dL/dscaling (through 1 / clamp(s, 1e-8) and the
 //                     min), dL/dquaternions (through pytorch3d's quaternion_to_matrix), dL/dstrengths
+//   Under torch.use_deterministic_algorithms (gsr_sugar_field_backward_det) k_field_backward<W, true> emits one key per pair
+//   instead of the RED.ADDs, group_ids (gsr_radix.cuh) sorts the pair ids by Gaussian, and k_field_reduce sums each Gaussian's
+//   partials in ascending pair id before the same chain.  The better-normal kernels below do the same (DESIGN.md §4).
 //
 // Every elementwise torch op is one IEEE rounding here (explicit _rn intrinsics, accurate expf / logf / sqrtf, no FMA
 // contraction) in the order SuGaR writes it.  torch's batched 3x3 matmul and its K-sum have no fixed order on the GPU, so the
 // results are not claimed bit-identical to torch; the contract is the tolerance of tests/test_gpu_sugar_field.py.
-#include "gsr_common.cuh"
+#include "gsr_radix.cuh"
 
 namespace gsr {
 
@@ -137,8 +140,55 @@ struct FieldGrad {
     float4* grec;            // [P] x 4 float4: (dc0, dc1, dc2, dfs), (dA00..dA10), (dA11..dA21), (dA22, dsmin, 0, 0)
 };
 
-template <int W>
-__global__ void __launch_bounds__(256) k_field_backward(FieldIn a, FieldGrad b) {
+// The gradient reaching o_nk through every output of sample n but the opacities: the density's, and the sdf chain's (sqrt: g / (2
+// result); -2 *: g * -2; log: g / x; clamp: where(x >= min); normalisation: g / (d + 1e-12)).  gbeta is dL/dbeta in, beta's
+// sdf term added.  d is the segment's density sum, bsum its min-scale sum.
+__device__ __forceinline__ float field_sample_grad(const FieldIn& a, const FieldGrad& b, int64_t n, float d, float bsum, float& gbeta) {
+    float G = b.g_density ? b.g_density[n] : 0.0f;
+    gbeta = b.g_beta ? b.g_beta[n] : 0.0f;
+    if (b.g_sdf) {
+        const float gs = b.g_sdf[n];
+        const float beta = __fdiv_rn(bsum, (float)a.K);
+        const float dh = field_dhat(d), cd = field_clampmin(dh, a.opacity_min_clamp);
+        const float sq = sqrtf(__fmul_rn(-2.0f, logf(cd)));
+        gbeta = __fadd_rn(gbeta, __fmul_rn(gs, __fsub_rn(sq, a.sdf_offset)));
+        const float gm = __fdiv_rn(__fmul_rn(gs, beta), __fmul_rn(2.0f, sq));
+        const float gcd = __fdiv_rn(__fmul_rn(gm, -2.0f), cd);
+        const float gdh = dh >= a.opacity_min_clamp ? gcd : 0.0f;
+        G = __fadd_rn(G, d >= 1.0f ? __fdiv_rn(gdh, __fadd_rn(d, 1e-12f)) : gdh);
+    }
+    return G;
+}
+
+// One pair's partials: dL/dshift ds and the record gradient r[0..12] = (-ds0, -ds1, -ds2, dfs, dA00, dA01, dA02, dA10, dA11, dA12,
+// dA20, dA21, dA22), given G of its sample.  k_field_backward adds them with atomics, k_field_reduce in id order: one formula.
+__device__ __forceinline__ void field_partial(const FieldIn& a, const FieldGrad& b, int64_t n, int k, const FieldPair& f, float G,
+                                              float& ds0, float& ds1, float& ds2, float r[13]) {
+    const float go = b.g_opac ? __fadd_rn(G, b.g_opac[n * a.K + k]) : G;
+    const float dfs = __fmul_rn(go, f.e);
+    const float dqc = __fmul_rn(__fmul_rn(__fmul_rn(go, f.fs), f.e), -0.5f);
+    const float dq = (f.q <= 1e8f) ? dqc : 0.0f;  // clamp(0, 1e8) passes where 0 <= q <= 1e8
+    const float dw0 = __fmul_rn(2.0f, __fmul_rn(dq, f.w0)), dw1 = __fmul_rn(2.0f, __fmul_rn(dq, f.w1)),
+                dw2 = __fmul_rn(2.0f, __fmul_rn(dq, f.w2));
+    ds0 = __fadd_rn(__fadd_rn(__fmul_rn(f.A[0], dw0), __fmul_rn(f.A[1], dw1)), __fmul_rn(f.A[2], dw2));
+    ds1 = __fadd_rn(__fadd_rn(__fmul_rn(f.A[3], dw0), __fmul_rn(f.A[4], dw1)), __fmul_rn(f.A[5], dw2));
+    ds2 = __fadd_rn(__fadd_rn(__fmul_rn(f.A[6], dw0), __fmul_rn(f.A[7], dw1)), __fmul_rn(f.A[8], dw2));
+    r[0] = -ds0; r[1] = -ds1; r[2] = -ds2; r[3] = dfs;
+    r[4] = __fmul_rn(dw0, f.sx); r[5] = __fmul_rn(dw1, f.sx); r[6] = __fmul_rn(dw2, f.sx);
+    r[7] = __fmul_rn(dw0, f.sy); r[8] = __fmul_rn(dw1, f.sy); r[9] = __fmul_rn(dw2, f.sy);
+    r[10] = __fmul_rn(dw0, f.sz); r[11] = __fmul_rn(dw1, f.sz); r[12] = __fmul_rn(dw2, f.sz);
+}
+
+// What DET adds to the default backward: per-sample scalars the partials need and one key per pair id n * K + k.
+struct FieldDet {
+    float* G;       // [N] field_sample_grad
+    float* dmin;    // [N] the min scale's gradient, dL/dbeta / K
+    uint32_t* key;  // [N*K] target Gaussian, P where the pair adds nothing
+    uint32_t* id;   // [N*K] = the position
+};
+
+template <int W, bool DET>
+__global__ void __launch_bounds__(256) k_field_backward(FieldIn a, FieldGrad b, FieldDet det) {
     const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int64_t n = (int64_t)(t / W);
     const int k = (int)(t % W);
@@ -155,39 +205,28 @@ __global__ void __launch_bounds__(256) k_field_backward(FieldIn a, FieldGrad b) 
     const unsigned seg = W == 32 ? 0xffffffffu : ((1u << W) - 1u) << ((threadIdx.x & 31u) & ~(unsigned)(W - 1));
     const bool bad = (__ballot_sync(0xffffffffu, active && !f.ok) & seg) != 0u;
     float ds0 = 0.0f, ds1 = 0.0f, ds2 = 0.0f;  // dL/dshift of this pair
+    if (DET && active) {
+        const size_t pid = (size_t)n * a.K + k;
+        det.key[pid] = bad ? (uint32_t)a.P : (uint32_t)f.g;
+        det.id[pid] = (uint32_t)pid;
+    }
     if (active && bad) {
         ds0 = ds1 = ds2 = __int_as_float(0x7fc00000);
     } else if (active) {  // every lane of the segment is inside its arrays
-        // per-sample gradient reaching every o_nk through densities.sum(dim=-1)
-        float G = b.g_density ? b.g_density[n] : 0.0f;
-        float gbeta = b.g_beta ? b.g_beta[n] : 0.0f;
-        if (b.g_sdf) {
-            const float gs = b.g_sdf[n];
-            const float beta = __fdiv_rn(bsum, (float)a.K);
-            const float dh = field_dhat(d), cd = field_clampmin(dh, a.opacity_min_clamp);
-            const float sq = sqrtf(__fmul_rn(-2.0f, logf(cd)));
-            gbeta = __fadd_rn(gbeta, __fmul_rn(gs, __fsub_rn(sq, a.sdf_offset)));
-            // sqrt: g / (2 result); -2 *: g * -2; log: g / x; clamp: where(x >= min); normalisation: g / (d + 1e-12)
-            const float gm = __fdiv_rn(__fmul_rn(gs, beta), __fmul_rn(2.0f, sq));
-            const float gcd = __fdiv_rn(__fmul_rn(gm, -2.0f), cd);
-            const float gdh = dh >= a.opacity_min_clamp ? gcd : 0.0f;
-            G = __fadd_rn(G, d >= 1.0f ? __fdiv_rn(gdh, __fadd_rn(d, 1e-12f)) : gdh);
-        }
-        const float go = b.g_opac ? __fadd_rn(G, b.g_opac[n * a.K + k]) : G;
-        const float dfs = __fmul_rn(go, f.e);
-        const float dqc = __fmul_rn(__fmul_rn(__fmul_rn(go, f.fs), f.e), -0.5f);
-        const float dq = (f.q <= 1e8f) ? dqc : 0.0f;  // clamp(0, 1e8) passes where 0 <= q <= 1e8
-        const float dw0 = __fmul_rn(2.0f, __fmul_rn(dq, f.w0)), dw1 = __fmul_rn(2.0f, __fmul_rn(dq, f.w1)),
-                    dw2 = __fmul_rn(2.0f, __fmul_rn(dq, f.w2));
-        ds0 = __fadd_rn(__fadd_rn(__fmul_rn(f.A[0], dw0), __fmul_rn(f.A[1], dw1)), __fmul_rn(f.A[2], dw2));
-        ds1 = __fadd_rn(__fadd_rn(__fmul_rn(f.A[3], dw0), __fmul_rn(f.A[4], dw1)), __fmul_rn(f.A[5], dw2));
-        ds2 = __fadd_rn(__fadd_rn(__fmul_rn(f.A[6], dw0), __fmul_rn(f.A[7], dw1)), __fmul_rn(f.A[8], dw2));
+        float gbeta;
+        const float G = field_sample_grad(a, b, n, d, bsum, gbeta);
         const float dmin = (b.g_beta || b.g_sdf) ? __fdiv_rn(gbeta, (float)a.K) : 0.0f;
-        float4* gr = b.grec + 4 * f.g;
-        atomicAdd(gr, make_float4(-ds0, -ds1, -ds2, dfs));
-        atomicAdd(gr + 1, make_float4(__fmul_rn(dw0, f.sx), __fmul_rn(dw1, f.sx), __fmul_rn(dw2, f.sx), __fmul_rn(dw0, f.sy)));
-        atomicAdd(gr + 2, make_float4(__fmul_rn(dw1, f.sy), __fmul_rn(dw2, f.sy), __fmul_rn(dw0, f.sz), __fmul_rn(dw1, f.sz)));
-        atomicAdd(gr + 3, make_float4(__fmul_rn(dw2, f.sz), dmin, 0.0f, 0.0f));
+        float r[13];
+        field_partial(a, b, n, k, f, G, ds0, ds1, ds2, r);
+        if (DET) {
+            if (k == 0) { det.G[n] = G; det.dmin[n] = dmin; }
+        } else {
+            float4* gr = b.grec + 4 * f.g;
+            atomicAdd(gr, make_float4(r[0], r[1], r[2], r[3]));
+            atomicAdd(gr + 1, make_float4(r[4], r[5], r[6], r[7]));
+            atomicAdd(gr + 2, make_float4(r[8], r[9], r[10], r[11]));
+            atomicAdd(gr + 3, make_float4(r[12], dmin, 0.0f, 0.0f));
+        }
     }
     ds0 = seg_sum<W>(ds0);
     ds1 = seg_sum<W>(ds1);
@@ -195,6 +234,35 @@ __global__ void __launch_bounds__(256) k_field_backward(FieldIn a, FieldGrad b) 
     if (active && k == 0 && b.dx) {
         b.dx[3 * n] = ds0; b.dx[3 * n + 1] = ds1; b.dx[3 * n + 2] = ds2;
     }
+}
+
+// DET: one thread per Gaussian g sums the partials of its pairs, recomputed with field_partial, in ascending pair id from +0.0, and
+// writes g's record gradient for the unchanged k_field_chain.
+__global__ void __launch_bounds__(256) k_field_reduce(FieldIn a, FieldGrad b, const float* __restrict__ G, const float* __restrict__ dmin,
+                                                      const uint32_t* __restrict__ ids, const uint32_t* __restrict__ seg) {
+    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= a.P) return;
+    float acc[14];
+#pragma unroll
+    for (int c = 0; c < 14; c++) acc[c] = 0.0f;
+    const uint32_t e = seg[g + 1];
+    for (uint32_t s = seg[g]; s < e; s++) {
+        const uint32_t pid = ids[s];
+        const int64_t n = pid / (uint32_t)a.K;
+        const int k = (int)(pid - (uint32_t)n * (uint32_t)a.K);
+        FieldPair f;
+        field_pair(a, n, k, f);
+        float ds0, ds1, ds2, r[13];
+        field_partial(a, b, n, k, f, G[n], ds0, ds1, ds2, r);
+#pragma unroll
+        for (int c = 0; c < 13; c++) acc[c] = __fadd_rn(acc[c], r[c]);
+        acc[13] = __fadd_rn(acc[13], dmin[n]);
+    }
+    float4* gr = b.grec + 4 * (size_t)g;
+    gr[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
+    gr[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
+    gr[2] = make_float4(acc[8], acc[9], acc[10], acc[11]);
+    gr[3] = make_float4(acc[12], acc[13], 0.0f, 0.0f);
 }
 
 __global__ void __launch_bounds__(256) k_field_chain(int P, const float* __restrict__ scaling, const float* __restrict__ quaternions,
@@ -263,9 +331,10 @@ static void launch_field(const FieldIn& a, float* d, float* o, float* b, float* 
     k_field<W><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(a, d, o, b, s);
 }
 template <int W>
-static void launch_field_backward(const FieldIn& a, const FieldGrad& g, cudaStream_t st) {
+static void launch_field_backward(const FieldIn& a, const FieldGrad& g, const FieldDet* det, cudaStream_t st) {
     const size_t threads = (size_t)a.N * W;
-    k_field_backward<W><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(a, g);
+    if (det) k_field_backward<W, true><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(a, g, *det);
+    else k_field_backward<W, false><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(a, g, FieldDet{});
 }
 static int seg_width(int K) { int w = 1; while (w < K) w <<= 1; return w; }
 
@@ -291,38 +360,81 @@ int sugar_field_impl(int N, int K, int P, int R, const float* x, const int64_t* 
     return check_launch("gsr_sugar_field", false, st);
 }
 
+// det: the deterministic backward (gsr_sugar_field_backward_det); the workspace is then its scratch, laid out by FieldDetLayout.
+struct FieldDetLayout {
+    size_t G, dmin, group, total;
+    GroupLayout gl;
+    FieldDetLayout(int N, int K, int P) : gl((size_t)(N < 0 ? 0 : N) * (size_t)(K < 0 ? 0 : K), P < 0 ? 0 : P) {
+        const size_t n = N < 0 ? 0 : N;
+        size_t o = align_up(2 * sugar_field_bytes(P), 256);  // rec, grec: the default backward's workspace
+        G = o;     o = align_up(o + 4 * n, 256);
+        dmin = o;  o = align_up(o + 4 * n, 256);
+        group = o;
+        total = o + gl.total;
+    }
+};
+size_t sugar_field_backward_det_bytes(int N, int K, int P) { return FieldDetLayout(N, K, P).total; }
+
+static int det_scratch_check(const char* who, const void* scratch) {
+    if (!scratch) { set_error("%s: scratch is NULL", who); return GSR_ERR_INVALID; }
+    if ((uintptr_t)scratch & 15) { set_error("%s: scratch is not 16-byte aligned", who); return GSR_ERR_INVALID; }
+    return GSR_OK;
+}
+
+static int det_ids_check(const char* who, int N, int K, int per_sample) {
+    if (N > 0 && K >= 1 && K <= FIELD_KMAX && (uint64_t)N * (uint64_t)(K + per_sample) >= (1ull << 32)) {
+        set_error("%s: %llu partial ids, at or above 2^32", who, (unsigned long long)((uint64_t)N * (uint64_t)(K + per_sample)));
+        return GSR_ERR_INVALID;
+    }
+    return GSR_OK;
+}
+
 int sugar_field_backward_impl(int N, int K, int P, int R, const float* x, const int64_t* rows, const int64_t* row_idx,
                               const float* points, const float* scaling, const float* quaternions, const float* strengths,
                               float density_factor, float opacity_min_clamp, float sdf_offset, const float* g_density, const float* g_opac,
                               const float* g_beta, const float* g_sdf, float* dx, float* d_points, float* d_scaling, float* d_quaternions,
-                              float* d_strengths, void* ws, size_t ws_bytes, cudaStream_t st) {
-    int rc = field_check("gsr_sugar_field_backward", N, K, P, R, x, rows, row_idx, points, scaling, quaternions, strengths,
-                         g_sdf != nullptr, ws, ws_bytes, 2 * sugar_field_bytes(P));
+                              float* d_strengths, void* ws, size_t ws_bytes, bool det, cudaStream_t st) {
+    const char* who = det ? "gsr_sugar_field_backward_det" : "gsr_sugar_field_backward";
+    if (det) {
+        int rc = det_ids_check(who, N, K, 0);
+        if (rc == GSR_OK && N > 0) rc = det_scratch_check(who, ws);
+        if (rc != GSR_OK) return rc;
+    }
+    int rc = field_check(who, N, K, P, R, x, rows, row_idx, points, scaling, quaternions, strengths, g_sdf != nullptr, ws, ws_bytes,
+                         det ? sugar_field_backward_det_bytes(N, K, P) : 2 * sugar_field_bytes(P));
     if (rc != GSR_OK || N == 0) return rc;
     if (P > 0 && (!d_points || !d_scaling || !d_quaternions || !d_strengths)) {
-        set_error("gsr_sugar_field_backward: dL_dpoints, dL_dscaling, dL_dquaternions and dL_dstrengths are required");
+        set_error("%s: dL_dpoints, dL_dscaling, dL_dquaternions and dL_dstrengths are required", who);
         return GSR_ERR_INVALID;
     }
     float4* rec = (float4*)ws;
     float4* grec = rec + 4 * (size_t)P;
     if (P > 0) {
         k_field_prepare<<<(P + 255) / 256, 256, 0, st>>>(P, points, scaling, quaternions, strengths, density_factor, rec);
-        cudaMemsetAsync(grec, 0, sugar_field_bytes(P), st);
+        if (!det) cudaMemsetAsync(grec, 0, sugar_field_bytes(P), st);
     }
     const FieldIn a{N, K, P, R, x, rows, row_idx, rec, opacity_min_clamp, sdf_offset};
     const FieldGrad g{g_density, g_opac, g_beta, g_sdf, dx, grec};
+    const FieldDetLayout L(N, K, P);
+    char* w = (char*)ws;
+    const FieldDet fd{(float*)(w + L.G), (float*)(w + L.dmin), (uint32_t*)(w + L.group + L.gl.keys0), (uint32_t*)(w + L.group + L.gl.vals0)};
+    const FieldDet* dp = det ? &fd : nullptr;
     switch (seg_width(K)) {
-        case 1: launch_field_backward<1>(a, g, st); break;
-        case 2: launch_field_backward<2>(a, g, st); break;
-        case 4: launch_field_backward<4>(a, g, st); break;
-        case 8: launch_field_backward<8>(a, g, st); break;
-        case 16: launch_field_backward<16>(a, g, st); break;
-        default: launch_field_backward<32>(a, g, st); break;
+        case 1: launch_field_backward<1>(a, g, dp, st); break;
+        case 2: launch_field_backward<2>(a, g, dp, st); break;
+        case 4: launch_field_backward<4>(a, g, dp, st); break;
+        case 8: launch_field_backward<8>(a, g, dp, st); break;
+        case 16: launch_field_backward<16>(a, g, dp, st); break;
+        default: launch_field_backward<32>(a, g, dp, st); break;
+    }
+    if (det && P > 0) {
+        const uint32_t* ids = group_ids((size_t)N * K, P, w + L.group, L.gl, st);
+        k_field_reduce<<<(P + 255) / 256, 256, 0, st>>>(a, g, fd.G, fd.dmin, ids, (const uint32_t*)(w + L.group + L.gl.seg));
     }
     if (P > 0)
         k_field_chain<<<(P + 255) / 256, 256, 0, st>>>(P, scaling, quaternions, density_factor, grec, d_points, d_scaling, d_quaternions,
                                                         d_strengths);
-    return check_launch("gsr_sugar_field_backward", false, st);
+    return check_launch(who, false, st);
 }
 
 // ================================================================================================================================
@@ -411,11 +523,13 @@ __device__ __forceinline__ void normal_pair(const NormalIn& a, int64_t n, int k,
     f.w = __fdiv_rn(__fmul_rn(a.opac[n * a.K + k], d), pc.w);
 }
 
-// The loss's segment reductions: w_hat of this lane and T = sum_j w_hat_j n'_j (every lane gets T).
+__device__ __forceinline__ float normal_what(float w, float S) { return __fdiv_rn(w, S < 1e-6f ? 1e-6f : S); }  // clamp(min=1e-6), NaN passes
+
+// The loss's segment reductions: w_hat of this lane and T = sum_j w_hat_j n'_j (every lane gets T); S = sum_j w_j.
 template <int W>
-__device__ __forceinline__ float normal_sums(const NormalPair& f, float& T0, float& T1, float& T2) {
-    const float S = seg_sum<W>(f.w);
-    const float wh = __fdiv_rn(f.w, S < 1e-6f ? 1e-6f : S);  // clamp(min=1e-6), NaN passes
+__device__ __forceinline__ float normal_sums(const NormalPair& f, float& T0, float& T1, float& T2, float& S) {
+    S = seg_sum<W>(f.w);
+    const float wh = normal_what(f.w, S);
     T0 = seg_sum<W>(__fmul_rn(wh, f.m0));
     T1 = seg_sum<W>(__fmul_rn(wh, f.m1));
     T2 = seg_sum<W>(__fmul_rn(wh, f.m2));
@@ -434,8 +548,8 @@ __global__ void __launch_bounds__(256) k_normal(NormalIn a, float* __restrict__ 
         NormalPair f;
         f.w = f.m0 = f.m1 = f.m2 = 0.0f;
         if (active) normal_pair(a, n, k, s, f);
-        float T0, T1, T2;
-        normal_sums<W>(f, T0, T1, T2);
+        float T0, T1, T2, S;
+        normal_sums<W>(f, T0, T1, T2, S);
         if (active && k == 0) {
             const float r0 = __fsub_rn(s.nz.x, T0), r1 = __fsub_rn(s.nz.y, T1), r2 = __fsub_rn(s.nz.z, T2);
             out_loss[n] = dot3_rn(r0, r1, r2, r0, r1, r2);
@@ -452,12 +566,29 @@ struct NormalGrad {
     float4* grec;         // [P] x 2 float4: (dp.xyz, 0), (dn.xyz, 0)
 };
 
-template <int W>
-__global__ void __launch_bounds__(256) k_normal_backward(NormalIn a, NormalGrad b) {
+// The loss's neighbour term, dL/dn_j of pair (n, j): -dn_i w_hat_j sigma_j, dn_i = dL/dloss * 2 r.  k_normal_backward adds it with
+// atomics, k_normal_reduce in id order: one formula.
+__device__ __forceinline__ float4 normal_neighbour_term(float dn0, float dn1, float dn2, float wh, float sg) {
+    return make_float4(__fmul_rn(__fmul_rn(-dn0, wh), sg), __fmul_rn(__fmul_rn(-dn1, wh), sg), __fmul_rn(__fmul_rn(-dn2, wh), sg), 0.0f);
+}
+
+// What DET adds to the default backward: per-sample values the partials need and one key per partial id n * (KS + 1) + slot, KS
+// = K neighbour slots with the loss, none without.
+struct NormalDet {
+    float4* sc;     // [N]   (the loss's dn_i, S = sum_j w_j)
+    float4* own;    // [N,2] the sample's own term: (dn_i, 0), (-dx, 0)
+    uint32_t* key;  // [N*(KS+1)] slot k < KS: knn[i, k], slot KS: i; P where the slot adds nothing
+    uint32_t* id;   // [N*(KS+1)] = the position
+    int KS;
+};
+
+template <int W, bool DET>
+__global__ void __launch_bounds__(256) k_normal_backward(NormalIn a, NormalGrad b, NormalDet det) {
     const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int64_t n = (int64_t)(t / W);
     const int k = (int)(t % W);
     const bool active = n < a.N && k < a.K;
+    const size_t pid0 = (size_t)n * (det.KS + 1);  // DET: the sample's first partial id
     NormalSample s;
     s.ok = true;
     if (active) normal_sample(a, n, s);
@@ -468,8 +599,8 @@ __global__ void __launch_bounds__(256) k_normal_backward(NormalIn a, NormalGrad 
         f.w = f.m0 = f.m1 = f.m2 = 0.0f;
         f.ok = true;
         if (active) normal_pair(a, n, k, s, f);
-        float T0, T1, T2;
-        const float wh = normal_sums<W>(f, T0, T1, T2);
+        float T0, T1, T2, S;
+        const float wh = normal_sums<W>(f, T0, T1, T2, S);
         if (seg_sum<W>(f.ok ? 0.0f : 1.0f) != 0.0f) bad = active;
         if (active && !bad) {
             // loss = sum_c r_c^2: dr = g * (2 r); r = n_i - T: dn_i = dr, dT = -dr; T = sum_j w_hat_j (sigma_j n_j)
@@ -477,9 +608,15 @@ __global__ void __launch_bounds__(256) k_normal_backward(NormalIn a, NormalGrad 
             dn0 = __fmul_rn(gl, __fmul_rn(2.0f, __fsub_rn(s.nz.x, T0)));
             dn1 = __fmul_rn(gl, __fmul_rn(2.0f, __fsub_rn(s.nz.y, T1)));
             dn2 = __fmul_rn(gl, __fmul_rn(2.0f, __fsub_rn(s.nz.z, T2)));
-            if (f.ok)
-                atomicAdd(b.grec + 2 * f.j + 1, make_float4(__fmul_rn(__fmul_rn(-dn0, wh), f.sg), __fmul_rn(__fmul_rn(-dn1, wh), f.sg),
-                                                            __fmul_rn(__fmul_rn(-dn2, wh), f.sg), 0.0f));
+            if (DET) {
+                if (k == 0) det.sc[n] = make_float4(dn0, dn1, dn2, S);
+            } else if (f.ok) {
+                atomicAdd(b.grec + 2 * f.j + 1, normal_neighbour_term(dn0, dn1, dn2, wh, f.sg));
+            }
+        }
+        if (DET && active) {
+            det.key[pid0 + k] = bad || !f.ok ? (uint32_t)a.P : (uint32_t)f.j;
+            det.id[pid0 + k] = (uint32_t)(pid0 + k);
         }
     }
     if (!active || k != 0) return;
@@ -491,12 +628,55 @@ __global__ void __launch_bounds__(256) k_normal_backward(NormalIn a, NormalGrad 
         dn0 = __fadd_rn(dn0, __fmul_rn(ge, __fsub_rn(s.x0, s.pc.x)));
         dn1 = __fadd_rn(dn1, __fmul_rn(ge, __fsub_rn(s.x1, s.pc.y)));
         dn2 = __fadd_rn(dn2, __fmul_rn(ge, __fsub_rn(s.x2, s.pc.z)));
-        atomicAdd(b.grec + 2 * s.i, make_float4(-dx0, -dx1, -dx2, 0.0f));
+        if (!DET) atomicAdd(b.grec + 2 * s.i, make_float4(-dx0, -dx1, -dx2, 0.0f));
     }
-    if (!bad && (b.g_loss || b.g_est)) atomicAdd(b.grec + 2 * s.i + 1, make_float4(dn0, dn1, dn2, 0.0f));
+    if (DET) {
+        const bool adds = !bad && (b.g_loss || b.g_est);
+        det.key[pid0 + det.KS] = adds ? (uint32_t)s.i : (uint32_t)a.P;
+        det.id[pid0 + det.KS] = (uint32_t)(pid0 + det.KS);
+        if (adds) {
+            det.own[2 * n] = make_float4(dn0, dn1, dn2, 0.0f);
+            det.own[2 * n + 1] = b.g_est ? make_float4(-dx0, -dx1, -dx2, 0.0f) : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        }
+    } else if (!bad && (b.g_loss || b.g_est)) {
+        atomicAdd(b.grec + 2 * s.i + 1, make_float4(dn0, dn1, dn2, 0.0f));
+    }
     // an index outside its array: this sample adds nothing and its dL/dx is NaN
     if (bad) dx0 = dx1 = dx2 = __int_as_float(0x7fc00000);
     if (b.dx) { b.dx[3 * n] = dx0; b.dx[3 * n + 1] = dx1; b.dx[3 * n + 2] = dx2; }
+}
+
+// DET: one thread per Gaussian g sums its partials in ascending id from +0.0: a neighbour slot adds normal_neighbour_term
+// (recomputed) to the normal, an own slot its stored (dn_i, -dx) to the normal and the centre.  Writes g's gradient record for
+// the unchanged k_normal_chain.
+__global__ void __launch_bounds__(256) k_normal_reduce(NormalIn a, float4* __restrict__ grec, const float4* __restrict__ sc,
+                                                       const float4* __restrict__ own, int KS, const uint32_t* __restrict__ ids,
+                                                       const uint32_t* __restrict__ seg) {
+    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= a.P) return;
+    float p0 = 0.0f, p1 = 0.0f, p2 = 0.0f, n0 = 0.0f, n1 = 0.0f, n2 = 0.0f;
+    const uint32_t e = seg[g + 1], K1 = (uint32_t)KS + 1;
+    for (uint32_t q = seg[g]; q < e; q++) {
+        const uint32_t pid = ids[q];
+        const int64_t n = pid / K1;
+        const int k = (int)(pid - (uint32_t)n * K1);
+        float4 v;
+        if (k == KS) {
+            const float4 op = own[2 * n + 1];
+            p0 = __fadd_rn(p0, op.x); p1 = __fadd_rn(p1, op.y); p2 = __fadd_rn(p2, op.z);
+            v = own[2 * n];
+        } else {
+            NormalSample s;
+            normal_sample(a, n, s);
+            NormalPair f;
+            normal_pair(a, n, k, s, f);
+            const float4 c = sc[n];
+            v = normal_neighbour_term(c.x, c.y, c.z, normal_what(f.w, c.w), f.sg);
+        }
+        n0 = __fadd_rn(n0, v.x); n1 = __fadd_rn(n1, v.y); n2 = __fadd_rn(n2, v.z);
+    }
+    grec[2 * (size_t)g] = make_float4(p0, p1, p2, 0.0f);
+    grec[2 * (size_t)g + 1] = make_float4(n0, n1, n2, 0.0f);
 }
 
 __global__ void __launch_bounds__(256) k_normal_chain(int P, const float* __restrict__ scaling, const float* __restrict__ quaternions,
@@ -553,9 +733,10 @@ static void launch_normal(const NormalIn& a, float* l, float* e, cudaStream_t st
     k_normal<W><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(a, l, e);
 }
 template <int W>
-static void launch_normal_backward(const NormalIn& a, const NormalGrad& g, cudaStream_t st) {
+static void launch_normal_backward(const NormalIn& a, const NormalGrad& g, const NormalDet* det, cudaStream_t st) {
     const size_t threads = (size_t)a.N * W;
-    k_normal_backward<W><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(a, g);
+    if (det) k_normal_backward<W, true><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(a, g, *det);
+    else k_normal_backward<W, false><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(a, g, NormalDet{});
 }
 
 int sugar_sdf_normal_impl(int N, int K, int P, const float* x, const int64_t* gidx, const int64_t* knn, const float* points,
@@ -579,35 +760,67 @@ int sugar_sdf_normal_impl(int N, int K, int P, const float* x, const int64_t* gi
     return check_launch("gsr_sugar_sdf_normal", false, st);
 }
 
+// det: the deterministic backward (gsr_sugar_sdf_normal_backward_det); the workspace is then its scratch, laid out by NormalDetLayout
+// for KS = K neighbour slots per sample with the loss, 0 without.
+struct NormalDetLayout {
+    size_t sc, own, group, total;
+    GroupLayout gl;
+    NormalDetLayout(int N, int KS, int P) : gl((size_t)(N < 0 ? 0 : N) * (size_t)(KS < 0 ? 1 : KS + 1), P < 0 ? 0 : P) {
+        const size_t n = N < 0 ? 0 : N;
+        size_t o = align_up(2 * sugar_sdf_normal_bytes(P), 256);  // rec, grec: the default backward's workspace
+        sc = o;   o = align_up(o + 16 * n, 256);
+        own = o;  o = align_up(o + 32 * n, 256);
+        group = o;
+        total = o + gl.total;
+    }
+};
+size_t sugar_sdf_normal_backward_det_bytes(int N, int K, int P, bool with_loss) { return NormalDetLayout(N, with_loss ? K : 0, P).total; }
+
 int sugar_sdf_normal_backward_impl(int N, int K, int P, const float* x, const int64_t* gidx, const int64_t* knn, const float* points,
                                    const float* scaling, const float* quaternions, const float* opac, const float* g_loss,
                                    const float* g_est, float* dx, float* d_points, float* d_quaternions, void* ws, size_t ws_bytes,
-                                   cudaStream_t st) {
-    int rc = normal_check("gsr_sugar_sdf_normal_backward", N, K, P, x, gidx, knn, points, scaling, quaternions, opac, g_loss != nullptr,
-                          ws, ws_bytes, 2 * sugar_sdf_normal_bytes(P));
+                                   bool det, cudaStream_t st) {
+    const char* who = det ? "gsr_sugar_sdf_normal_backward_det" : "gsr_sugar_sdf_normal_backward";
+    if (det) {
+        int rc = g_loss ? det_ids_check(who, N, K, 1) : GSR_OK;
+        if (rc == GSR_OK && N > 0) rc = det_scratch_check(who, ws);
+        if (rc != GSR_OK) return rc;
+    }
+    int rc = normal_check(who, N, K, P, x, gidx, knn, points, scaling, quaternions, opac, g_loss != nullptr, ws, ws_bytes,
+                          det ? sugar_sdf_normal_backward_det_bytes(N, K, P, g_loss != nullptr) : 2 * sugar_sdf_normal_bytes(P));
     if (rc != GSR_OK || N == 0) return rc;
     if (P > 0 && (!d_points || !d_quaternions)) {
-        set_error("gsr_sugar_sdf_normal_backward: dL_dpoints and dL_dquaternions are required");
+        set_error("%s: dL_dpoints and dL_dquaternions are required", who);
         return GSR_ERR_INVALID;
     }
     float4* rec = (float4*)ws;
     float4* grec = rec + 2 * (size_t)P;
     if (P > 0) {
         k_normal_prepare<<<(P + 255) / 256, 256, 0, st>>>(P, points, scaling, quaternions, rec);
-        cudaMemsetAsync(grec, 0, sugar_sdf_normal_bytes(P), st);
+        if (!det) cudaMemsetAsync(grec, 0, sugar_sdf_normal_bytes(P), st);
     }
     const NormalIn a{N, K, P, x, gidx, knn, opac, rec};
     const NormalGrad g{g_loss, g_est, dx, grec};
+    const int KS = g_loss ? K : 0;
+    const NormalDetLayout L(N, KS, P);
+    char* w = (char*)ws;
+    const NormalDet nd{(float4*)(w + L.sc), (float4*)(w + L.own), (uint32_t*)(w + L.group + L.gl.keys0),
+                       (uint32_t*)(w + L.group + L.gl.vals0), KS};
+    const NormalDet* dp = det ? &nd : nullptr;
     switch (normal_width(K, g_loss != nullptr)) {
-        case 1: launch_normal_backward<1>(a, g, st); break;
-        case 2: launch_normal_backward<2>(a, g, st); break;
-        case 4: launch_normal_backward<4>(a, g, st); break;
-        case 8: launch_normal_backward<8>(a, g, st); break;
-        case 16: launch_normal_backward<16>(a, g, st); break;
-        default: launch_normal_backward<32>(a, g, st); break;
+        case 1: launch_normal_backward<1>(a, g, dp, st); break;
+        case 2: launch_normal_backward<2>(a, g, dp, st); break;
+        case 4: launch_normal_backward<4>(a, g, dp, st); break;
+        case 8: launch_normal_backward<8>(a, g, dp, st); break;
+        case 16: launch_normal_backward<16>(a, g, dp, st); break;
+        default: launch_normal_backward<32>(a, g, dp, st); break;
+    }
+    if (det && P > 0) {
+        const uint32_t* ids = group_ids((size_t)N * (KS + 1), P, w + L.group, L.gl, st);
+        k_normal_reduce<<<(P + 255) / 256, 256, 0, st>>>(a, grec, nd.sc, nd.own, KS, ids, (const uint32_t*)(w + L.group + L.gl.seg));
     }
     if (P > 0) k_normal_chain<<<(P + 255) / 256, 256, 0, st>>>(P, scaling, quaternions, grec, d_points, d_quaternions);
-    return check_launch("gsr_sugar_sdf_normal_backward", false, st);
+    return check_launch(who, false, st);
 }
 
 }  // namespace gsr

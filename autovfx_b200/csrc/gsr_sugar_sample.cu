@@ -14,7 +14,7 @@
 // float64 and in a fixed order, so a call is deterministic.  The float64 roundings of a parallel scan can leave a row with t = 0
 // one ulp above its predecessor; the sign of T marks those rows, and a search that lands on one steps back to the last row of
 // positive weight (a zero-weight row is never drawn; leading zero rows have T = 0 exactly and can never be landed on).
-#include "gsr_common.cuh"
+#include "gsr_radix.cuh"
 #include <cfloat>
 
 namespace gsr {
@@ -161,12 +161,10 @@ struct SampleGradArgs {
     float *d_points, *d_scaling, *d_quaternions;
 };
 
-// out = p + q (0, v) q* = p + (w^2 - u.u) v + 2 (u.v) u + 2 w (u x v), q = (w, u), v = (f s) z: any q, unit or not
-__global__ void __launch_bounds__(256) k_sample_backward(SampleGradArgs a) {
-    const int n = blockIdx.x * blockDim.x + threadIdx.x;
-    if (n >= a.N || !total_ok(*a.total)) return;
-    const int64_t i = a.idx[n];
-    if (i < 0 || i >= a.P) return;
+// out = p + q (0, v) q* = p + (w^2 - u.u) v + 2 (u.v) u + 2 w (u x v), q = (w, u), v = (f s) z: any q, unit or not.  Sample n's
+// partials to its Gaussian i: r = (dL/dpoints (3), dL/dscaling (3), dL/dquaternions (4)).  k_sample_backward adds them with atomics,
+// k_sample_reduce in ascending n: one formula.
+__device__ __forceinline__ void sample_partial(const SampleGradArgs& a, int n, int64_t i, float r[10]) {
     const float3 g = {a.g[3 * (size_t)n], a.g[3 * (size_t)n + 1], a.g[3 * (size_t)n + 2]};
     const float3 z = {a.z[3 * (size_t)n], a.z[3 * (size_t)n + 1], a.z[3 * (size_t)n + 2]};
     const float3 v = {a.f * a.scaling[3 * i] * z.x, a.f * a.scaling[3 * i + 1] * z.y, a.f * a.scaling[3 * i + 2] * z.z};
@@ -182,20 +180,61 @@ __global__ void __launch_bounds__(256) k_sample_backward(SampleGradArgs a) {
     // dL/dw = 2 w (g.v) + 2 g.(u x v);  dL/du = -2 (g.v) u + 2 (u.g) v + 2 (u.v) g + 2 w (v x g)
     const float3 uxv = {u.y * v.z - u.z * v.y, u.z * v.x - u.x * v.z, u.x * v.y - u.y * v.x};
     const float3 vxg = {v.y * g.z - v.z * g.y, v.z * g.x - v.x * g.z, v.x * g.y - v.y * g.x};
-    const float dw = 2.0f * (w * gv + (g.x * uxv.x + g.y * uxv.y + g.z * uxv.z));
-    const float dux = 2.0f * (ug * v.x + uv * g.x + w * vxg.x - gv * u.x);
-    const float duy = 2.0f * (ug * v.y + uv * g.y + w * vxg.y - gv * u.y);
-    const float duz = 2.0f * (ug * v.z + uv * g.z + w * vxg.z - gv * u.z);
-    atomicAdd(a.d_points + 3 * i, g.x);
-    atomicAdd(a.d_points + 3 * i + 1, g.y);
-    atomicAdd(a.d_points + 3 * i + 2, g.z);
-    atomicAdd(a.d_scaling + 3 * i, a.f * z.x * dvx);
-    atomicAdd(a.d_scaling + 3 * i + 1, a.f * z.y * dvy);
-    atomicAdd(a.d_scaling + 3 * i + 2, a.f * z.z * dvz);
-    atomicAdd(a.d_quaternions + 4 * i, dw);
-    atomicAdd(a.d_quaternions + 4 * i + 1, dux);
-    atomicAdd(a.d_quaternions + 4 * i + 2, duy);
-    atomicAdd(a.d_quaternions + 4 * i + 3, duz);
+    r[0] = g.x; r[1] = g.y; r[2] = g.z;
+    r[3] = a.f * z.x * dvx; r[4] = a.f * z.y * dvy; r[5] = a.f * z.z * dvz;
+    r[6] = 2.0f * (w * gv + (g.x * uxv.x + g.y * uxv.y + g.z * uxv.z));
+    r[7] = 2.0f * (ug * v.x + uv * g.x + w * vxg.x - gv * u.x);
+    r[8] = 2.0f * (ug * v.y + uv * g.y + w * vxg.y - gv * u.y);
+    r[9] = 2.0f * (ug * v.z + uv * g.z + w * vxg.z - gv * u.z);
+}
+
+// DET: no atomics; key[n] = the sample's Gaussian, or P where it adds nothing (an index outside [0, P), a zero or non-finite
+// total), id[n] = n.
+template <bool DET>
+__global__ void __launch_bounds__(256) k_sample_backward(SampleGradArgs a, uint32_t* __restrict__ key, uint32_t* __restrict__ id) {
+    const int n = blockIdx.x * blockDim.x + threadIdx.x;
+    if (DET) {
+        if (n >= a.N) return;
+        const int64_t i = a.idx[n];
+        key[n] = total_ok(*a.total) && i >= 0 && i < a.P ? (uint32_t)i : (uint32_t)a.P;
+        id[n] = (uint32_t)n;
+        return;
+    }
+    if (n >= a.N || !total_ok(*a.total)) return;
+    const int64_t i = a.idx[n];
+    if (i < 0 || i >= a.P) return;
+    float r[10];
+    sample_partial(a, n, i, r);
+    atomicAdd(a.d_points + 3 * i, r[0]);
+    atomicAdd(a.d_points + 3 * i + 1, r[1]);
+    atomicAdd(a.d_points + 3 * i + 2, r[2]);
+    atomicAdd(a.d_scaling + 3 * i, r[3]);
+    atomicAdd(a.d_scaling + 3 * i + 1, r[4]);
+    atomicAdd(a.d_scaling + 3 * i + 2, r[5]);
+    atomicAdd(a.d_quaternions + 4 * i, r[6]);
+    atomicAdd(a.d_quaternions + 4 * i + 1, r[7]);
+    atomicAdd(a.d_quaternions + 4 * i + 2, r[8]);
+    atomicAdd(a.d_quaternions + 4 * i + 3, r[9]);
+}
+
+// DET: one thread per Gaussian g sums sample_partial over its samples in ascending n from +0.0 and writes g's three rows.
+__global__ void __launch_bounds__(256) k_sample_reduce(SampleGradArgs a, const uint32_t* __restrict__ ids, const uint32_t* __restrict__ seg) {
+    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= a.P) return;
+    float acc[10];
+#pragma unroll
+    for (int c = 0; c < 10; c++) acc[c] = 0.0f;
+    const uint32_t e = seg[g + 1];
+    for (uint32_t q = seg[g]; q < e; q++) {
+        float r[10];
+        sample_partial(a, (int)ids[q], g, r);
+#pragma unroll
+        for (int c = 0; c < 10; c++) acc[c] = __fadd_rn(acc[c], r[c]);
+    }
+    const size_t g3 = 3 * (size_t)g, g4 = 4 * (size_t)g;
+    a.d_points[g3] = acc[0]; a.d_points[g3 + 1] = acc[1]; a.d_points[g3 + 2] = acc[2];
+    a.d_scaling[g3] = acc[3]; a.d_scaling[g3 + 1] = acc[4]; a.d_scaling[g3 + 2] = acc[5];
+    a.d_quaternions[g4] = acc[6]; a.d_quaternions[g4 + 1] = acc[7]; a.d_quaternions[g4 + 2] = acc[8]; a.d_quaternions[g4 + 3] = acc[9];
 }
 
 inline int nblocks_prefix(int P) { return (P + PREFIX_BLOCK - 1) / PREFIX_BLOCK; }
@@ -239,25 +278,41 @@ int sugar_sample_impl(int N, int P, float f, int volume, const uint8_t* mask, co
     return check_launch("gsr_sugar_sample", false, st);
 }
 
+size_t sugar_sample_backward_det_bytes(int N, int P) { return GroupLayout((size_t)(N < 0 ? 0 : N), P < 0 ? 0 : P).total; }
+
+// det: the deterministic backward (gsr_sugar_sample_backward_det) with `scratch` of scratch_bytes; otherwise scratch is unused.
 int sugar_sample_backward_impl(int N, int P, float f, const int64_t* idx, const float* z, const float* scaling, const float* quaternions,
                                const double* total, const float* dL_dsamples, float* d_points, float* d_scaling, float* d_quaternions,
-                               cudaStream_t st) {
+                               bool det, void* scratch, size_t scratch_bytes, cudaStream_t st) {
+    const char* who = det ? "gsr_sugar_sample_backward_det" : "gsr_sugar_sample_backward";
     if (N < 0 || P < 1) {
-        set_error("gsr_sugar_sample_backward: N = %d and P = %d (need N >= 0, P >= 1)", N, P);
+        set_error("%s: N = %d and P = %d (need N >= 0, P >= 1)", who, N, P);
         return GSR_ERR_INVALID;
     }
     if (!d_points || !d_scaling || !d_quaternions || (N > 0 && (!idx || !z || !scaling || !quaternions || !total || !dL_dsamples))) {
-        set_error("gsr_sugar_sample_backward: missing input or output");
+        set_error("%s: missing input or output", who);
         return GSR_ERR_INVALID;
+    }
+    const SampleGradArgs a{N, P, f, idx, z, scaling, quaternions, dL_dsamples, total, d_points, d_scaling, d_quaternions};
+    if (det && N > 0) {
+        if (!scratch) { set_error("%s: scratch is NULL", who); return GSR_ERR_INVALID; }
+        if ((uintptr_t)scratch & 15) { set_error("%s: scratch is not 16-byte aligned", who); return GSR_ERR_INVALID; }
+        const GroupLayout L((size_t)N, P);
+        if (scratch_bytes < L.total) {
+            set_error("%s: scratch too small (%zu < %zu)", who, scratch_bytes, L.total);
+            return GSR_ERR_WORKSPACE;
+        }
+        char* w = (char*)scratch;
+        k_sample_backward<true><<<(N + 255) / 256, 256, 0, st>>>(a, (uint32_t*)(w + L.keys0), (uint32_t*)(w + L.vals0));
+        const uint32_t* ids = group_ids((size_t)N, P, w, L, st);
+        k_sample_reduce<<<(P + 255) / 256, 256, 0, st>>>(a, ids, (const uint32_t*)(w + L.seg));
+        return check_launch(who, false, st);
     }
     cudaMemsetAsync(d_points, 0, 12 * (size_t)P, st);
     cudaMemsetAsync(d_scaling, 0, 12 * (size_t)P, st);
     cudaMemsetAsync(d_quaternions, 0, 16 * (size_t)P, st);
-    if (N > 0) {
-        const SampleGradArgs a{N, P, f, idx, z, scaling, quaternions, dL_dsamples, total, d_points, d_scaling, d_quaternions};
-        k_sample_backward<<<(N + 255) / 256, 256, 0, st>>>(a);
-    }
-    return check_launch("gsr_sugar_sample_backward", false, st);
+    if (N > 0) k_sample_backward<false><<<(N + 255) / 256, 256, 0, st>>>(a, nullptr, nullptr);
+    return check_launch(who, false, st);
 }
 
 }  // namespace gsr

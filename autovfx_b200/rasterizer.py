@@ -27,7 +27,6 @@ from typing import Dict, NamedTuple, Optional, Tuple
 
 import torch
 import torch.nn as nn
-import torch.utils.deterministic
 
 from . import _lib
 from ._lib import lib as _L
@@ -566,18 +565,6 @@ class PreparedForward:
         return st.issue_ticket(self._counters, stream, self._capacity_instances)
 
 
-def _scratch_bytes(nbytes: int, device: torch.device) -> torch.Tensor:
-    """A byte buffer from the caching allocator, without the NaN fill torch gives every torch.empty under
-    use_deterministic_algorithms: gsr_backward_det writes every scratch byte it reads, and a fill of gigabytes would cost about
-    as much as the backward itself."""
-    fill = torch.utils.deterministic.fill_uninitialized_memory
-    torch.utils.deterministic.fill_uninitialized_memory = False
-    try:
-        return torch.empty(nbytes, dtype=torch.uint8, device=device)
-    finally:
-        torch.utils.deterministic.fill_uninitialized_memory = fill
-
-
 def _cpu_copy(items):
     """CPU clones of the tensors in ``items`` (the reference's cpu_deep_copy_tuple, __init__.py:16-18)."""
     return tuple(x.detach().cpu().clone() if isinstance(x, torch.Tensor) else x for x in items)
@@ -709,7 +696,7 @@ class _RasterizeGaussians(torch.autograd.Function):
             dL_dextra = torch.empty((P, 3), **f32) if multi else None
             if torch.are_deterministic_algorithms_enabled():
                 nbytes = _L.gsr_backward_det_bytes(ctx.ticket.num_rendered(), W, H, int(multi))
-                scratch = _scratch_bytes(nbytes, device)
+                scratch = _lib.scratch_bytes(nbytes, device)
                 rc = _L.gsr_backward_det(C.byref(fr), C.byref(ws), _ptr(radii), _ptr(alpha), _ptr(g_color), _ptr(g_depth), _ptr(g_alpha),
                                          _ptr(extra), _ptr(g_extra), _ptr(dL_dextra), C.byref(gr), scratch.data_ptr(), nbytes, stream)
                 what = "gsr_backward_det"

@@ -135,14 +135,19 @@ class _SugarField(torch.autograd.Function):
         d_strengths = torch.zeros_like(strengths)
         if N > 0 and any(t is not None for t in g):
             L = _lib_handle()
-            nbytes = 2 * L.gsr_sugar_field_bytes(P)
-            ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
-            rc = L.gsr_sugar_field_backward(N, cfg.K, P, cfg.R, x.data_ptr(), rows.data_ptr(), _ptr(row_idx), points.data_ptr(),
-                                            scaling.data_ptr(), quaternions.data_ptr(), strengths.data_ptr(), cfg.df, cfg.omc,
-                                            cfg.offset, *[_ptr(t) for t in g], _ptr(dx), d_points.data_ptr(), d_scaling.data_ptr(),
-                                            d_quaternions.data_ptr(), d_strengths.data_ptr(), ws.data_ptr(), nbytes,
-                                            _lib.stream_ptr(dev))
-            _lib.check(rc, "gsr_sugar_field_backward")
+            if torch.are_deterministic_algorithms_enabled():  # fixed-order sums (DESIGN §4), no atomics
+                fn, what = L.gsr_sugar_field_backward_det, "gsr_sugar_field_backward_det"
+                nbytes = L.gsr_sugar_field_backward_det_bytes(N, cfg.K, P)
+                ws = _lib.scratch_bytes(nbytes, dev)
+            else:
+                fn, what = L.gsr_sugar_field_backward, "gsr_sugar_field_backward"
+                nbytes = 2 * L.gsr_sugar_field_bytes(P)
+                ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
+            rc = fn(N, cfg.K, P, cfg.R, x.data_ptr(), rows.data_ptr(), _ptr(row_idx), points.data_ptr(), scaling.data_ptr(),
+                    quaternions.data_ptr(), strengths.data_ptr(), cfg.df, cfg.omc, cfg.offset, *[_ptr(t) for t in g], _ptr(dx),
+                    d_points.data_ptr(), d_scaling.data_ptr(), d_quaternions.data_ptr(), d_strengths.data_ptr(), ws.data_ptr(), nbytes,
+                    _lib.stream_ptr(dev))
+            _lib.check(rc, what)
         need = ctx.needs_input_grad
         return (dx, d_points if need[1] else None, d_scaling if need[2] else None, d_quaternions if need[3] else None,
                 d_strengths if need[4] else None, None, None, None)
@@ -271,14 +276,18 @@ class _SugarSdfNormal(torch.autograd.Function):
         if N > 0 and g is not None:
             g = g.contiguous()
             L = _lib_handle()
-            nbytes = 2 * L.gsr_sugar_sdf_normal_bytes(P)
-            ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=x.device)
-            rc = L.gsr_sugar_sdf_normal_backward(N, ctx.K, P, x.data_ptr(), gidx.data_ptr(), _ptr(knn), points.data_ptr(),
-                                                 scaling.data_ptr(), quaternions.data_ptr(), _ptr(opac),
-                                                 g.data_ptr() if ctx.want_loss else None, None if ctx.want_loss else g.data_ptr(),
-                                                 _ptr(dx), d_points.data_ptr(), d_quaternions.data_ptr(), ws.data_ptr(), nbytes,
-                                                 _lib.stream_ptr(x.device))
-            _lib.check(rc, "gsr_sugar_sdf_normal_backward")
+            if torch.are_deterministic_algorithms_enabled():  # fixed-order sums (DESIGN §4), no atomics
+                fn, what = L.gsr_sugar_sdf_normal_backward_det, "gsr_sugar_sdf_normal_backward_det"
+                nbytes = L.gsr_sugar_sdf_normal_backward_det_bytes(N, ctx.K, P, int(ctx.want_loss))
+                ws = _lib.scratch_bytes(nbytes, x.device)
+            else:
+                fn, what = L.gsr_sugar_sdf_normal_backward, "gsr_sugar_sdf_normal_backward"
+                nbytes = 2 * L.gsr_sugar_sdf_normal_bytes(P)
+                ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=x.device)
+            rc = fn(N, ctx.K, P, x.data_ptr(), gidx.data_ptr(), _ptr(knn), points.data_ptr(), scaling.data_ptr(), quaternions.data_ptr(),
+                    _ptr(opac), g.data_ptr() if ctx.want_loss else None, None if ctx.want_loss else g.data_ptr(), _ptr(dx),
+                    d_points.data_ptr(), d_quaternions.data_ptr(), ws.data_ptr(), nbytes, _lib.stream_ptr(x.device))
+            _lib.check(rc, what)
         return (dx, d_points if need[1] else None, d_quaternions if need[2] else None, None, None, None, None, None, None)
 
 
@@ -375,10 +384,17 @@ class _SugarSample(torch.autograd.Function):
         d_points = torch.empty((P, 3), dtype=torch.float32, device=g.device)
         d_scaling = torch.empty((P, 3), dtype=torch.float32, device=g.device)
         d_quaternions = torch.empty((P, 4), dtype=torch.float32, device=g.device)
-        rc = _lib_handle().gsr_sugar_sample_backward(N, P, ctx.f, idx.data_ptr(), z.data_ptr(), scaling.data_ptr(),
-                                                     quaternions.data_ptr(), total.data_ptr(), g.data_ptr(), d_points.data_ptr(),
-                                                     d_scaling.data_ptr(), d_quaternions.data_ptr(), _lib.stream_ptr(g.device))
-        _lib.check(rc, "gsr_sugar_sample_backward")
+        L = _lib_handle()
+        args = (N, P, ctx.f, idx.data_ptr(), z.data_ptr(), scaling.data_ptr(), quaternions.data_ptr(), total.data_ptr(), g.data_ptr(),
+                d_points.data_ptr(), d_scaling.data_ptr(), d_quaternions.data_ptr())
+        if torch.are_deterministic_algorithms_enabled():  # fixed-order sums (DESIGN §4), no atomics
+            nbytes = L.gsr_sugar_sample_backward_det_bytes(N, P)
+            scratch = _lib.scratch_bytes(nbytes, g.device)
+            rc = L.gsr_sugar_sample_backward_det(*args, scratch.data_ptr(), nbytes, _lib.stream_ptr(g.device))
+            _lib.check(rc, "gsr_sugar_sample_backward_det")
+        else:
+            rc = L.gsr_sugar_sample_backward(*args, _lib.stream_ptr(g.device))
+            _lib.check(rc, "gsr_sugar_sample_backward")
         return (d_points if need[0] else None, d_scaling if need[1] else None, d_quaternions if need[2] else None,
                 None, None, None, None, None, None, None)
 

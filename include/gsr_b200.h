@@ -366,6 +366,27 @@ int gsr_sugar_field_backward(int32_t N, int32_t K, int32_t P, int32_t R, const f
                              float* dL_dscaling, float* dL_dquaternions, float* dL_dstrengths, void* workspace, size_t workspace_bytes,
                              void* stream);
 
+/* Deterministic backward of gsr_sugar_field: gsr_sugar_field_backward's arguments, with a device scratch (16-byte aligned) of at
+ * least gsr_sugar_field_backward_det_bytes(N, K, P) bytes in place of its workspace (the scratch includes it).  Every output is
+ * bit-identical from call to call, whatever the scheduling or the concurrent streams.  Pair (n, k) has the id n*K + k and goes to
+ * Gaussian g = rows[row_idx[n], k]; for every g each of the 14 record gradient components (-dL/dshift, dL/d(density_factor *
+ * strength), the 9 of dL/dA, dL/d(min scale)) is a sequential fp32 sum from +0.0 of g's pair partials in ascending id, and the
+ * per-Gaussian chain to dL_dpoints, dL_dscaling, dL_dquaternions and dL_dstrengths follows as in gsr_sugar_field_backward (DESIGN.md
+ * §4).  dL_dx is per sample, as there.  The values agree with gsr_sugar_field_backward's to rounding, not bit for bit.  The exclusion
+ * rules are the same: a sample with an index outside its array adds nothing through any pair and its dL_dx is NaN.  Every row of the
+ * gradients is written; no scratch byte is read before it is written in the same call.  N*K at or above 2^32, and a NULL or
+ * misaligned scratch (when N > 0), are GSR_ERR_INVALID; a scratch smaller than the query is GSR_ERR_WORKSPACE.  All are reported
+ * before anything is enqueued.  With A(x) = x rounded up to a multiple of 256 and G(M, P), the grouping of M ids over P Gaussians,
+ *   G(M, P) = 4 A(4M) + A(1024 c) + A(4 ceil(max(256 c, P + 1) / 1024)) + A(4 (P + 1)),  c = ceil(M / 2048),
+ * the query is A(128 P) + 2 A(4 N) + G(N K, P). */
+size_t gsr_sugar_field_backward_det_bytes(int32_t N, int32_t K, int32_t P);
+int gsr_sugar_field_backward_det(int32_t N, int32_t K, int32_t P, int32_t R, const float* x, const int64_t* rows, const int64_t* row_idx,
+                                 const float* points, const float* scaling, const float* quaternions, const float* strengths,
+                                 float density_factor, float opacity_min_clamp, float sdf_offset, const float* dL_ddensity,
+                                 const float* dL_dopacities, const float* dL_dbeta, const float* dL_dsdf, float* dL_dx, float* dL_dpoints,
+                                 float* dL_dscaling, float* dL_dquaternions, float* dL_dstrengths, void* scratch, size_t scratch_bytes,
+                                 void* stream);
+
 /* The coarse trainers' better-normal loss and projection estimate (sugar_trainers/coarse_density.py:704-707, :756-780) at N samples
  * x [N,3], each in the Gaussian gidx[n] of P given by SuGaR's getters (points [P,3], scaling [P,3], quaternions [P,4]), with the K
  * neighbours knn_idx[gidx[n], 0..K-1] of the int64 table knn_idx [P,K] (1 <= K <= 32) and their opacities [N,K].  n_g is column
@@ -391,6 +412,21 @@ int gsr_sugar_sdf_normal_backward(int32_t N, int32_t K, int32_t P, const float* 
                                   const float* dL_dloss, const float* dL_destimate, float* dL_dx, float* dL_dpoints,
                                   float* dL_dquaternions, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Deterministic backward of gsr_sugar_sdf_normal: gsr_sugar_sdf_normal_backward's arguments, with a device scratch (16-byte aligned)
+ * of at least gsr_sugar_sdf_normal_backward_det_bytes(N, K, P, dL_dloss != NULL) bytes in place of its workspace.  With the loss,
+ * sample n has K + 1 partial ids: slot k < K (id n*(K+1) + k) is the loss's neighbour term, to knn_idx[gidx[n], k]; slot K (id
+ * n*(K+1) + K) is the sample's own term, to gidx[n]: its dL/dn and, with dL_destimate, -dL/dx for the centre.  Without the loss,
+ * sample n has only its own slot, id n.  For every Gaussian each component of the normal and centre gradients is a sequential fp32
+ * sum from +0.0 of its partials in ascending id (the centre's over own terms only, so in ascending n); the chain to
+ * dL_dquaternions follows as in gsr_sugar_sdf_normal_backward.  The rules for a bad index, the full writes, the unread scratch and
+ * the errors are those of gsr_sugar_field_backward_det, the id limit being N*(K+1) (with the loss).  With A and G as there, the query
+ * is A(64 P) + A(16 N) + A(32 N) + G(N (K + 1), P) with the loss and A(64 P) + A(16 N) + A(32 N) + G(N, P) without. */
+size_t gsr_sugar_sdf_normal_backward_det_bytes(int32_t N, int32_t K, int32_t P, int with_loss);
+int gsr_sugar_sdf_normal_backward_det(int32_t N, int32_t K, int32_t P, const float* x, const int64_t* gidx, const int64_t* knn_idx,
+                                      const float* points, const float* scaling, const float* quaternions, const float* opacities,
+                                      const float* dL_dloss, const float* dL_destimate, float* dL_dx, float* dL_dpoints,
+                                      float* dL_dquaternions, void* scratch, size_t scratch_bytes, void* stream);
+
 /* SuGaR.sample_points_in_gaussians (sugar_model.py:757-799) given its random draws: N samples among P >= 1 Gaussians given by
  * SuGaR's getters, points [P,3], scaling [P,3], quaternions [P,4] (as the getters return them).  A row is selected where mask [P]
  * (bool bytes) is non-zero, every row when mask is NULL.  A selected row's weight is w = |s0 * s1 * s2| (float32, left to right) when
@@ -413,12 +449,24 @@ int gsr_sugar_sample(int32_t N, int32_t P, float sampling_scale_factor, int32_t 
                      size_t workspace_bytes, void* stream);
 
 /* Backward of gsr_sugar_sample (same N, P, factor, z, scaling and quaternions; idx and total as it wrote them): the gradient of the
- * samples dL_dsamples [N,3] in, dL_dpoints [P,3], dL_dscaling [P,3] and dL_dquaternions [P,4] out (required, written in full; the
- * per-sample terms are added with atomics, so the summation order is not fixed).  The weights get no gradient, as through
+ * samples dL_dsamples [N,3] in, dL_dpoints [P,3], dL_dscaling [P,3] and dL_dquaternions [P,4] out (required, written in full;
+ * gsr_sugar_sample_backward_det below sums the per-sample terms in a fixed order).  The weights get no gradient, as through
  * torch.multinomial.  When the total is zero, infinite or NaN the gradients are zero. */
 int gsr_sugar_sample_backward(int32_t N, int32_t P, float sampling_scale_factor, const int64_t* idx, const float* z, const float* scaling,
                               const float* quaternions, const double* total, const float* dL_dsamples, float* dL_dpoints,
                               float* dL_dscaling, float* dL_dquaternions, void* stream);
+
+/* Deterministic backward of gsr_sugar_sample: gsr_sugar_sample_backward's arguments plus a device scratch (16-byte aligned) of at
+ * least gsr_sugar_sample_backward_det_bytes(N, P) = G(N, P) bytes (G as for gsr_sugar_field_backward_det).  Sample n (id n) goes to
+ * Gaussian idx[n]; for every Gaussian each of its 10 gradient components is a sequential fp32 sum from +0.0 of its samples' terms in
+ * ascending n.  A sample whose index is outside [0, P), or every sample when the total is zero or not finite, adds nothing; every
+ * row is written (+0.0 where no sample adds).  A NULL or misaligned scratch (when N > 0) is GSR_ERR_INVALID, a smaller one
+ * GSR_ERR_WORKSPACE, both before anything is enqueued. */
+size_t gsr_sugar_sample_backward_det_bytes(int32_t N, int32_t P);
+int gsr_sugar_sample_backward_det(int32_t N, int32_t P, float sampling_scale_factor, const int64_t* idx, const float* z,
+                                  const float* scaling, const float* quaternions, const double* total, const float* dL_dsamples,
+                                  float* dL_dpoints, float* dL_dscaling, float* dL_dquaternions, void* scratch, size_t scratch_bytes,
+                                  void* stream);
 
 /* Densification statistics (GaussianModel.add_densification_stats plus the trainers' max-radii line, gaussian_model.py:415-417,
  * train.py:163-164; SuGaRDensifier.update_densification_stats, sugar_densifier.py:156-164).  For every row i < P with mask[i] != 0:

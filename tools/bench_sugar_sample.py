@@ -6,6 +6,8 @@ coarse trainer's SDF-regularisation block with and without it, all arms alternat
   block          coarse_density's block on the library (field, projection estimate, better-normal loss), called as
                  tools/bench_sugar_sdf_block.py calls it, on samples drawn before timing
   sample_block   the library's sampler, then that block: the samples carry their gradient back to the model
+  sample_block_det  sample_block under torch.use_deterministic_algorithms(True): the sampler's, the field's and the normal
+                 terms' backwards sum in a fixed order (gsr_sugar_*_backward_det)
 
 Scene: config-3 at 3M Gaussians, knn_idx = knn_points(K = 16) (built before timing), a mask with about 70 % of the rows set,
 1M samples, sampling_scale_factor 1.5, probabilities proportional to volume (the trainers' default).  Per arm: call time (CUDA
@@ -79,9 +81,13 @@ def main():
         elif arm == "block":
             block(x0, gidx0).backward()
         else:
-            block(*sugar_field.sample_points_in_gaussians(model, N, f, mask=mask)).backward()
+            torch.use_deterministic_algorithms(arm == "sample_block_det")
+            try:
+                block(*sugar_field.sample_points_in_gaussians(model, N, f, mask=mask)).backward()
+            finally:
+                torch.use_deterministic_algorithms(False)
 
-    arms = ("sample_torch", "sample_cuda", "block", "sample_block")
+    arms = ("sample_torch", "sample_cuda", "block", "sample_block", "sample_block_det")
     if args.profile:
         from torch.profiler import ProfilerActivity, profile
         for arm in arms:
