@@ -90,7 +90,8 @@ EXPORTS = ("gsr_abi_version", "gsr_last_error", "gsr_geom_bytes", "gsr_binning_b
            "gsr_adam_step", "gsr_photometric_loss_bytes", "gsr_photometric_loss", "gsr_photometric_loss_backward", "gsr_normal_loss",
            "gsr_normal_loss_backward", "gsr_anisotropic_loss", "gsr_anisotropic_loss_backward", "gsr_backward_det_bytes", "gsr_backward_det",
            "gsr_sugar_field_backward_det_bytes", "gsr_sugar_field_backward_det", "gsr_sugar_sdf_normal_backward_det_bytes",
-           "gsr_sugar_sdf_normal_backward_det", "gsr_sugar_sample_backward_det_bytes", "gsr_sugar_sample_backward_det")
+           "gsr_sugar_sdf_normal_backward_det", "gsr_sugar_sample_backward_det_bytes", "gsr_sugar_sample_backward_det",
+           "gsr_percentile_low", "gsr_composite")
 
 
 def _load() -> C.CDLL:
@@ -219,6 +220,10 @@ def _load() -> C.CDLL:
     lib.gsr_anisotropic_loss.argtypes = [C.c_int64, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     lib.gsr_anisotropic_loss_backward.restype = C.c_int
     lib.gsr_anisotropic_loss_backward.argtypes = [C.c_int64, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.gsr_percentile_low.restype = C.c_int
+    lib.gsr_percentile_low.argtypes = [C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+    lib.gsr_composite.restype = C.c_int
+    lib.gsr_composite.argtypes = [C.c_int32] * 2 + [C.c_void_p] * 14
     lib.gsr_get_views.restype = C.c_int
     lib.gsr_get_views.argtypes = [C.POINTER(gsr_workspace), C.c_int32, C.c_int32, C.c_int32, C.POINTER(gsr_views)]
     lib.gsr_profile_begin.restype = C.c_int

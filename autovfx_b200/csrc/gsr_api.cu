@@ -88,6 +88,10 @@ int normal_loss_backward_impl(int64_t n, const float* pred, const int64_t* ps, c
                               cudaStream_t st);
 int anisotropic_loss_impl(int64_t P, const float* scales, float r, float* out, void* ws, size_t ws_bytes, cudaStream_t st);
 int anisotropic_loss_backward_impl(int64_t P, const float* scales, float r, const float* g_out, float* d_scales, cudaStream_t st);
+int percentile_low_impl(int64_t n, const float* x, float* out, void* ws, size_t ws_bytes, cudaStream_t st);
+int composite_impl(int32_t W, int32_t H, const uint8_t* frame, const uint8_t* obj, const float* obj_d, const uint8_t* shadow,
+                   const float* shadow_d, const uint8_t* all, const uint8_t* gs, const float* gs_d, const uint8_t* smoke,
+                   const float* smoke_d, const float* smoke_pct, const uint8_t* fire, uint8_t* out, cudaStream_t st);
 size_t sugar_sample_bytes(int P);
 int sugar_sample_impl(int N, int P, float f, int volume, const uint8_t* mask, const float* strengths, const double* u, const float* z,
                       const float* points, const float* scaling, const float* quaternions, float* out_points, int64_t* out_idx,
@@ -420,6 +424,19 @@ int gsr_anisotropic_loss(int64_t P, const float* scales, float r, float* out, vo
 int gsr_anisotropic_loss_backward(int64_t P, const float* scales, float r, const float* g_out, float* d_scales, void* stream) {
     NvtxRange nvtx_("gsr_anisotropic_loss_backward");
     return gsr::anisotropic_loss_backward_impl(P, scales, r, g_out, d_scales, (cudaStream_t)stream);
+}
+
+int gsr_percentile_low(int64_t n, const float* x, float* out, void* workspace, size_t workspace_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_percentile_low");
+    return gsr::percentile_low_impl(n, x, out, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int gsr_composite(int32_t W, int32_t H, const uint8_t* frame, const uint8_t* obj, const float* obj_depth, const uint8_t* shadow,
+                  const float* shadow_depth, const uint8_t* all, const uint8_t* obj3dgs, const float* obj3dgs_depth, const uint8_t* smoke,
+                  const float* smoke_depth, const float* smoke_pct, const uint8_t* fire, uint8_t* out, void* stream) {
+    NvtxRange nvtx_("gsr_composite");
+    return gsr::composite_impl(W, H, frame, obj, obj_depth, shadow, shadow_depth, all, obj3dgs, obj3dgs_depth, smoke, smoke_depth, smoke_pct,
+                               fire, out, (cudaStream_t)stream);
 }
 
 int gsr_profile_begin(int max_frames) { return gsr::profile_begin(max_frames, 1); }

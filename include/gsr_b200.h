@@ -25,6 +25,8 @@
  *                               coarse_density.py:550-590, scene_representation.py:513-515); gsr_photometric_loss_backward their autograd
  *   gsr_normal_loss   replaces  normal_loss                                       GS/utils/loss_utils.py:118-132; gsr_normal_loss_backward
  *   gsr_anisotropic_loss replaces anisotropic_loss                                GS/utils/loss_utils.py:159-168; gsr_anisotropic_loss_backward
+ *   gsr_percentile_low replaces np.percentile(smoke_depth, 0.001)                blender/blend_all.py:206-208
+ *   gsr_composite     replaces  the per-frame compositing of blend_frames          blender/blend_all.py:236-342
  *
  * and, for the render() wrapper around the two rasterizer passes ("GR/" = sugar/gaussian_splatting/gaussian_renderer/__init__.py):
  *
@@ -588,6 +590,24 @@ int gsr_anisotropic_loss(int64_t P, const float* scales, float r, float* out, vo
 /* d_scales [P,3] = g_out[0] * d out / d scales: the max's and the min's gradient go to the first extreme index (NaN first), as
  * torch's max(dim) / min(dim) return it; nothing where the ratio is below r (clamp_min passes ratio == r).  One thread per Gaussian. */
 int gsr_anisotropic_loss_backward(int64_t P, const float* scales, float r, const float* g_out, float* d_scales, void* stream);
+
+/* Frame compositing (gsr_composite.cu), bit-identical to blender/blend_all.py:blend_frames on the same decoded arrays. */
+#define GSR_PERCENTILE_BYTES 2048 /* the workspace of gsr_percentile_low */
+/* out[0] = np.percentile(x, 0.001) of n float32 values (numpy's default 'linear' method, in float32 as NumPy >= 2 computes it
+ * for a float32 array); NaN when any value is NaN.  The result stays on the device; nothing synchronises with the host.
+ * 1 <= n < 2^31, else GSR_ERR_INVALID; `workspace` (16-byte aligned) needs GSR_PERCENTILE_BYTES, else GSR_ERR_WORKSPACE. */
+int gsr_percentile_low(int64_t n, const float* x, float* out, void* workspace, size_t workspace_bytes, void* stream);
+/* out [H,W,4] uint8 = the composited frame of blend_frames (:236-342) from:
+ *   frame [H,W,4] uint8 (the 3DGS frame: images/*.png, or rgba8 of gsr_pack_frame);
+ *   obj, shadow, all [H,W,4] uint8 (rgb_obj, rgb_shadow, rgb_all) and obj_depth, shadow_depth [H,W] float (depth_obj, depth_shadow);
+ *   optional pairs obj3dgs + obj3dgs_depth (rgb_obj_3dgs, depth_obj_3dgs) and smoke + smoke_depth (rgb_smoke_fire,
+ *   depth_smoke_fire) with smoke_pct, the device scalar gsr_percentile_low wrote for smoke_depth; optional fire [H,W,4] uint8
+ *   (rgb_smoke_fire_pre), which needs smoke.
+ * The frame's depth, depth_all and depth_smoke_fire_pre never affect the frame and are not arguments.  8-bit layers must be
+ * 4-byte aligned.  A missing required layer, an unpaired optional one or fire without smoke is GSR_ERR_INVALID. */
+int gsr_composite(int32_t W, int32_t H, const uint8_t* frame, const uint8_t* obj, const float* obj_depth, const uint8_t* shadow,
+                  const float* shadow_depth, const uint8_t* all, const uint8_t* obj3dgs, const float* obj3dgs_depth, const uint8_t* smoke,
+                  const float* smoke_depth, const float* smoke_pct, const uint8_t* fire, uint8_t* out, void* stream);
 
 /* Device pointers into the workspaces of the last layout (P, capacity, W, H) — for parity tests that
  * compare per-stage buffers with the reference (SURVEY §4).  Pure pointer arithmetic, no CUDA calls. */
