@@ -79,19 +79,77 @@ GSR_FLAG_RESUME = 64
 GSR_SLAB_SHIFT = 16
 ABI_VERSION = 4
 
-EXPORTS = ("gsr_abi_version", "gsr_last_error", "gsr_geom_bytes", "gsr_binning_bytes", "gsr_binning_capacity", "gsr_image_bytes",
-           "gsr_forward", "gsr_backward", "gsr_mark_visible", "gsr_dist2_bytes", "gsr_dist2", "gsr_get_views",
-           "gsr_profile_begin", "gsr_profile_begin_strided", "gsr_profile_end", "gsr_forward_multi", "gsr_axis_normals", "gsr_normal_maps",
-           "gsr_pack_frame", "gsr_activate_gaussians", "gsr_set_option", "gsr_backward_multi", "gsr_activate_gaussians_backward",
-           "gsr_sugar_normals", "gsr_sugar_normals_backward", "gsr_sugar_colors", "gsr_sugar_colors_backward", "gsr_knn_bytes", "gsr_knn",
-           "gsr_sugar_field_bytes", "gsr_sugar_field", "gsr_sugar_field_backward", "gsr_sugar_sdf_normal_bytes", "gsr_sugar_sdf_normal",
-           "gsr_sugar_sdf_normal_backward", "gsr_densify_stats", "gsr_densify_plan_bytes", "gsr_densify_plan", "gsr_densify_apply",
-           "gsr_sugar_sample_bytes", "gsr_sugar_sample", "gsr_sugar_sample_backward", "gsr_binning_bytes_slab", "gsr_binning_capacity_slab",
-           "gsr_adam_step", "gsr_photometric_loss_bytes", "gsr_photometric_loss", "gsr_photometric_loss_backward", "gsr_normal_loss",
-           "gsr_normal_loss_backward", "gsr_anisotropic_loss", "gsr_anisotropic_loss_backward", "gsr_backward_det_bytes", "gsr_backward_det",
-           "gsr_sugar_field_backward_det_bytes", "gsr_sugar_field_backward_det", "gsr_sugar_sdf_normal_backward_det_bytes",
-           "gsr_sugar_sdf_normal_backward_det", "gsr_sugar_sample_backward_det_bytes", "gsr_sugar_sample_backward_det",
-           "gsr_percentile_low", "gsr_composite")
+_int, _i32, _i64, _f32, _size, _ptr = C.c_int, C.c_int32, C.c_int64, C.c_float, C.c_size_t, C.c_void_p
+_frame, _ws, _grads = C.POINTER(gsr_frame), C.POINTER(gsr_workspace), C.POINTER(gsr_grads)
+_FIELD_BWD = [_i32] * 4 + [_ptr] * 7 + [_f32] * 3 + [_ptr] * 10 + [_size, _ptr]
+_SDF_NORMAL_BWD = [_i32] * 3 + [_ptr] * 13 + [_size, _ptr]
+
+# every export of include/gsr_b200.h: name -> (restype, argtypes)
+SIGNATURES = {
+    "gsr_geom_bytes": (_size, [_i32]),
+    "gsr_binning_bytes": (_size, [_size]),
+    "gsr_image_bytes": (_size, [_i32, _i32]),
+    "gsr_binning_capacity": (_size, [_size]),
+    "gsr_binning_bytes_slab": (_size, [_size, _i32, _i32, _i32]),
+    "gsr_binning_capacity_slab": (_size, [_size, _i32, _i32, _i32]),
+    "gsr_forward": (_int, [_frame, _ws] + [_ptr] * 4 + [_int, _ptr]),
+    "gsr_forward_multi": (_int, [_frame, _ws] + [_ptr] * 6 + [_int, _ptr]),
+    "gsr_axis_normals": (_int, [_i32] + [_ptr] * 4 + [_int, _ptr, _ptr]),
+    "gsr_sugar_normals": (_int, [_i32] + [_ptr] * 6),
+    "gsr_sugar_normals_backward": (_int, [_i32] + [_ptr] * 7),
+    "gsr_sugar_colors": (_int, [_i32] * 3 + [_ptr] * 9),
+    "gsr_sugar_colors_backward": (_int, [_i32] * 3 + [_ptr] * 13),
+    "gsr_normal_maps": (_int, [_i32, _i32] + [_ptr] * 3 + [_f32] * 4 + [_ptr] * 3),
+    "gsr_pack_frame": (_int, [_i32, _i32] + [_ptr] * 4 + [_f32] + [_ptr] * 4),
+    "gsr_activate_gaussians": (_int, [_i32, _i32] + [_ptr] * 6 + [C.POINTER(gsr_object_xform)] + [_ptr] * 6),
+    "gsr_activate_gaussians_backward": (_int, [_i32, _i32] + [_ptr] * 17),
+    "gsr_backward": (_int, [_frame, _ws] + [_ptr] * 5 + [_grads, _ptr]),
+    "gsr_backward_multi": (_int, [_frame, _ws] + [_ptr] * 8 + [_grads, _ptr]),
+    "gsr_backward_det_bytes": (_size, [_size, _i32, _i32, _int]),
+    "gsr_backward_det": (_int, [_frame, _ws] + [_ptr] * 8 + [_grads, _ptr, _size, _ptr]),
+    "gsr_mark_visible": (_int, [_i32] + [_ptr] * 5),
+    "gsr_dist2_bytes": (_size, [_i32]),
+    "gsr_dist2": (_int, [_i32] + [_ptr] * 3 + [_size, _ptr]),
+    "gsr_knn_bytes": (_size, [_i32] * 3),
+    "gsr_knn": (_int, [_i32] * 3 + [_ptr] * 5 + [_size, _ptr]),
+    "gsr_sugar_field_bytes": (_size, [_i32]),
+    "gsr_sugar_field": (_int, [_i32] * 4 + [_ptr] * 7 + [_f32] * 3 + [_ptr] * 5 + [_size, _ptr]),
+    "gsr_sugar_field_backward": (_int, _FIELD_BWD),
+    "gsr_sugar_field_backward_det_bytes": (_size, [_i32] * 3),
+    "gsr_sugar_field_backward_det": (_int, _FIELD_BWD),
+    "gsr_sugar_sdf_normal_bytes": (_size, [_i32]),
+    "gsr_sugar_sdf_normal": (_int, [_i32] * 3 + [_ptr] * 10 + [_size, _ptr]),
+    "gsr_sugar_sdf_normal_backward": (_int, _SDF_NORMAL_BWD),
+    "gsr_sugar_sdf_normal_backward_det_bytes": (_size, [_i32] * 3 + [_int]),
+    "gsr_sugar_sdf_normal_backward_det": (_int, _SDF_NORMAL_BWD),
+    "gsr_sugar_sample_bytes": (_size, [_i32]),
+    "gsr_sugar_sample": (_int, [_i32, _i32, _f32, _i32] + [_ptr] * 11 + [_size, _ptr]),
+    "gsr_sugar_sample_backward": (_int, [_i32, _i32, _f32] + [_ptr] * 10),
+    "gsr_sugar_sample_backward_det_bytes": (_size, [_i32] * 2),
+    "gsr_sugar_sample_backward_det": (_int, [_i32, _i32, _f32] + [_ptr] * 10 + [_size, _ptr]),
+    "gsr_densify_stats": (_int, [_i32] * 2 + [_ptr] * 7),
+    "gsr_densify_plan_bytes": (_size, [_i32]),
+    "gsr_densify_plan": (_int, [_i32] + [_ptr] * 4 + [_f32] * 3 + [_i32] + [_f32] * 2 + [_ptr] * 3 + [_size, _ptr]),
+    "gsr_densify_apply": (_int, [_i32] * 3 + [C.POINTER(gsr_densify_group)] + [_ptr] * 5 + [_i32, _ptr]),
+    "gsr_adam_step": (_int, [_i32, C.POINTER(gsr_adam_tensor), _ptr]),
+    "gsr_photometric_loss_bytes": (_size, [_i32] * 5),
+    "gsr_photometric_loss": (_int, [_i32] * 4 + [_ptr] * 5 + [_i32] + [_ptr] * 3 + [_size, _ptr]),
+    "gsr_photometric_loss_backward": (_int, [_i32] * 4 + [_ptr] * 9 + [_size, _ptr]),
+    "gsr_normal_loss": (_int, [_i64] + [_ptr] * 5 + [_i64, _f32, _ptr, _ptr, _size, _ptr]),
+    "gsr_normal_loss_backward": (_int, [_i64] + [_ptr] * 5 + [_i64, _f32] + [_ptr] * 3 + [_size, _ptr]),
+    "gsr_anisotropic_loss": (_int, [_i64, _ptr, _f32, _ptr, _ptr, _size, _ptr]),
+    "gsr_anisotropic_loss_backward": (_int, [_i64, _ptr, _f32] + [_ptr] * 3),
+    "gsr_percentile_low": (_int, [_i64] + [_ptr] * 3 + [_size, _ptr]),
+    "gsr_composite": (_int, [_i32] * 2 + [_ptr] * 14),
+    "gsr_get_views": (_int, [_ws, _i32, _i32, _i32, C.POINTER(gsr_views)]),
+    "gsr_profile_begin": (_int, [_int]),
+    "gsr_profile_begin_strided": (_int, [_int, _int]),
+    "gsr_profile_end": (_int, [C.POINTER(C.c_float), C.POINTER(C.c_int)]),
+    "gsr_set_option": (_int, [C.c_char_p, _int]),
+    "gsr_last_error": (C.c_char_p, []),
+    "gsr_abi_version": (_int, []),
+}
+EXPORTS = tuple(SIGNATURES)
 
 
 def _load() -> C.CDLL:
@@ -105,135 +163,13 @@ def _load() -> C.CDLL:
                 raise ImportError("autovfx_b200: CUDA library %s is missing and cannot be built (%s). "
                                   "There is no CPU fallback." % (path, ex)) from ex
     lib = C.CDLL(path)
-    for name in EXPORTS:
+    for name, (restype, argtypes) in SIGNATURES.items():
         if not hasattr(lib, name):
             raise ImportError("autovfx_b200: %s does not export %s" % (path, name))
-    lib.gsr_abi_version.restype = C.c_int
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
     if lib.gsr_abi_version() != ABI_VERSION:
         raise ImportError("autovfx_b200: ABI mismatch, rebuild with `python -m autovfx_b200.build --force`")
-    lib.gsr_last_error.restype = C.c_char_p
-    for n in ("gsr_geom_bytes", "gsr_image_bytes", "gsr_binning_bytes", "gsr_binning_capacity", "gsr_dist2_bytes", "gsr_knn_bytes",
-              "gsr_sugar_field_bytes", "gsr_sugar_sdf_normal_bytes", "gsr_densify_plan_bytes", "gsr_sugar_sample_bytes"):
-        getattr(lib, n).restype = C.c_size_t
-    lib.gsr_geom_bytes.argtypes = [C.c_int32]
-    lib.gsr_image_bytes.argtypes = [C.c_int32, C.c_int32]
-    lib.gsr_binning_bytes.argtypes = [C.c_size_t]
-    lib.gsr_binning_capacity.argtypes = [C.c_size_t]
-    for n in ("gsr_binning_bytes_slab", "gsr_binning_capacity_slab"):
-        getattr(lib, n).restype = C.c_size_t
-        getattr(lib, n).argtypes = [C.c_size_t, C.c_int32, C.c_int32, C.c_int32]
-    lib.gsr_dist2_bytes.argtypes = [C.c_int32]
-    lib.gsr_forward.restype = C.c_int
-    lib.gsr_forward.argtypes = [C.POINTER(gsr_frame), C.POINTER(gsr_workspace), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                C.c_int, C.c_void_p]
-    lib.gsr_forward_multi.restype = C.c_int
-    lib.gsr_forward_multi.argtypes = [C.POINTER(gsr_frame), C.POINTER(gsr_workspace), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                      C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
-    lib.gsr_axis_normals.restype = C.c_int
-    lib.gsr_axis_normals.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
-    lib.gsr_sugar_normals.restype = C.c_int
-    lib.gsr_sugar_normals.argtypes = [C.c_int32] + [C.c_void_p] * 6
-    lib.gsr_sugar_normals_backward.restype = C.c_int
-    lib.gsr_sugar_normals_backward.argtypes = [C.c_int32] + [C.c_void_p] * 7
-    lib.gsr_sugar_colors.restype = C.c_int
-    lib.gsr_sugar_colors.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 9
-    lib.gsr_sugar_colors_backward.restype = C.c_int
-    lib.gsr_sugar_colors_backward.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 13
-    lib.gsr_normal_maps.restype = C.c_int
-    lib.gsr_normal_maps.argtypes = [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_float,
-                                    C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.gsr_pack_frame.restype = C.c_int
-    lib.gsr_pack_frame.argtypes = [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p,
-                                   C.c_void_p, C.c_void_p]
-    lib.gsr_activate_gaussians.restype = C.c_int
-    lib.gsr_activate_gaussians.argtypes = [C.c_int32, C.c_int32] + [C.c_void_p] * 6 + [C.POINTER(gsr_object_xform)] + [C.c_void_p] * 6
-    lib.gsr_activate_gaussians_backward.restype = C.c_int
-    lib.gsr_activate_gaussians_backward.argtypes = [C.c_int32, C.c_int32] + [C.c_void_p] * 17
-    lib.gsr_backward.restype = C.c_int
-    lib.gsr_backward.argtypes = [C.POINTER(gsr_frame), C.POINTER(gsr_workspace), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                 C.c_void_p, C.POINTER(gsr_grads), C.c_void_p]
-    lib.gsr_backward_multi.restype = C.c_int
-    lib.gsr_backward_multi.argtypes = [C.POINTER(gsr_frame), C.POINTER(gsr_workspace), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(gsr_grads), C.c_void_p]
-    lib.gsr_backward_det_bytes.restype = C.c_size_t
-    lib.gsr_backward_det_bytes.argtypes = [C.c_size_t, C.c_int32, C.c_int32, C.c_int]
-    lib.gsr_backward_det.restype = C.c_int
-    lib.gsr_backward_det.argtypes = [C.POINTER(gsr_frame), C.POINTER(gsr_workspace)] + [C.c_void_p] * 8 + [C.POINTER(gsr_grads), C.c_void_p,
-                                                                                          C.c_size_t, C.c_void_p]
-    lib.gsr_mark_visible.restype = C.c_int
-    lib.gsr_mark_visible.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.gsr_dist2.restype = C.c_int
-    lib.gsr_dist2.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
-    lib.gsr_knn_bytes.argtypes = [C.c_int32] * 3
-    lib.gsr_knn.restype = C.c_int
-    lib.gsr_knn.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 5 + [C.c_size_t, C.c_void_p]
-    lib.gsr_sugar_field_bytes.argtypes = [C.c_int32]
-    lib.gsr_sugar_field.restype = C.c_int
-    lib.gsr_sugar_field.argtypes = [C.c_int32] * 4 + [C.c_void_p] * 7 + [C.c_float] * 3 + [C.c_void_p] * 5 + [C.c_size_t, C.c_void_p]
-    lib.gsr_sugar_field_backward.restype = C.c_int
-    lib.gsr_sugar_field_backward.argtypes = ([C.c_int32] * 4 + [C.c_void_p] * 7 + [C.c_float] * 3 + [C.c_void_p] * 10 +
-                                             [C.c_size_t, C.c_void_p])
-    lib.gsr_sugar_field_backward_det_bytes.restype = C.c_size_t
-    lib.gsr_sugar_field_backward_det_bytes.argtypes = [C.c_int32] * 3
-    lib.gsr_sugar_field_backward_det.restype = C.c_int
-    lib.gsr_sugar_field_backward_det.argtypes = lib.gsr_sugar_field_backward.argtypes
-    lib.gsr_sugar_sdf_normal_bytes.argtypes = [C.c_int32]
-    lib.gsr_sugar_sdf_normal.restype = C.c_int
-    lib.gsr_sugar_sdf_normal.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 9 + [C.c_void_p, C.c_size_t, C.c_void_p]
-    lib.gsr_sugar_sdf_normal_backward.restype = C.c_int
-    lib.gsr_sugar_sdf_normal_backward.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 12 + [C.c_void_p, C.c_size_t, C.c_void_p]
-    lib.gsr_sugar_sdf_normal_backward_det_bytes.restype = C.c_size_t
-    lib.gsr_sugar_sdf_normal_backward_det_bytes.argtypes = [C.c_int32] * 3 + [C.c_int]
-    lib.gsr_sugar_sdf_normal_backward_det.restype = C.c_int
-    lib.gsr_sugar_sdf_normal_backward_det.argtypes = lib.gsr_sugar_sdf_normal_backward.argtypes
-    lib.gsr_densify_stats.restype = C.c_int
-    lib.gsr_densify_stats.argtypes = [C.c_int32] * 2 + [C.c_void_p] * 7
-    lib.gsr_densify_plan_bytes.argtypes = [C.c_int32]
-    lib.gsr_densify_plan.restype = C.c_int
-    lib.gsr_densify_plan.argtypes = ([C.c_int32] + [C.c_void_p] * 4 + [C.c_float] * 3 + [C.c_int32] + [C.c_float] * 2 + [C.c_void_p] * 3 +
-                                     [C.c_size_t, C.c_void_p])
-    lib.gsr_densify_apply.restype = C.c_int
-    lib.gsr_densify_apply.argtypes = ([C.c_int32] * 3 + [C.POINTER(gsr_densify_group)] + [C.c_void_p] * 5 + [C.c_int32, C.c_void_p])
-    lib.gsr_sugar_sample_bytes.argtypes = [C.c_int32]
-    lib.gsr_sugar_sample.restype = C.c_int
-    lib.gsr_sugar_sample.argtypes = ([C.c_int32] * 2 + [C.c_float, C.c_int32] + [C.c_void_p] * 10 + [C.c_void_p, C.c_size_t, C.c_void_p])
-    lib.gsr_sugar_sample_backward.restype = C.c_int
-    lib.gsr_sugar_sample_backward.argtypes = [C.c_int32] * 2 + [C.c_float] + [C.c_void_p] * 10
-    lib.gsr_sugar_sample_backward_det_bytes.restype = C.c_size_t
-    lib.gsr_sugar_sample_backward_det_bytes.argtypes = [C.c_int32] * 2
-    lib.gsr_sugar_sample_backward_det.restype = C.c_int
-    lib.gsr_sugar_sample_backward_det.argtypes = [C.c_int32] * 2 + [C.c_float] + [C.c_void_p] * 9 + [C.c_void_p, C.c_size_t, C.c_void_p]
-    lib.gsr_adam_step.restype = C.c_int
-    lib.gsr_adam_step.argtypes = [C.c_int32, C.POINTER(gsr_adam_tensor), C.c_void_p]
-    lib.gsr_photometric_loss_bytes.restype = C.c_size_t
-    lib.gsr_photometric_loss_bytes.argtypes = [C.c_int32] * 5
-    lib.gsr_photometric_loss.restype = C.c_int
-    lib.gsr_photometric_loss.argtypes = [C.c_int32] * 4 + [C.c_void_p] * 5 + [C.c_int32] + [C.c_void_p] * 3 + [C.c_size_t, C.c_void_p]
-    lib.gsr_photometric_loss_backward.restype = C.c_int
-    lib.gsr_photometric_loss_backward.argtypes = [C.c_int32] * 4 + [C.c_void_p] * 9 + [C.c_size_t, C.c_void_p]
-    lib.gsr_normal_loss.restype = C.c_int
-    lib.gsr_normal_loss.argtypes = [C.c_int64] + [C.c_void_p] * 5 + [C.c_int64, C.c_float, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
-    lib.gsr_normal_loss_backward.restype = C.c_int
-    lib.gsr_normal_loss_backward.argtypes = ([C.c_int64] + [C.c_void_p] * 5 + [C.c_int64, C.c_float] + [C.c_void_p] * 3 +
-                                             [C.c_size_t, C.c_void_p])
-    lib.gsr_anisotropic_loss.restype = C.c_int
-    lib.gsr_anisotropic_loss.argtypes = [C.c_int64, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
-    lib.gsr_anisotropic_loss_backward.restype = C.c_int
-    lib.gsr_anisotropic_loss_backward.argtypes = [C.c_int64, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.gsr_percentile_low.restype = C.c_int
-    lib.gsr_percentile_low.argtypes = [C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
-    lib.gsr_composite.restype = C.c_int
-    lib.gsr_composite.argtypes = [C.c_int32] * 2 + [C.c_void_p] * 14
-    lib.gsr_get_views.restype = C.c_int
-    lib.gsr_get_views.argtypes = [C.POINTER(gsr_workspace), C.c_int32, C.c_int32, C.c_int32, C.POINTER(gsr_views)]
-    lib.gsr_profile_begin.restype = C.c_int
-    lib.gsr_profile_begin.argtypes = [C.c_int]
-    lib.gsr_profile_begin_strided.restype = C.c_int
-    lib.gsr_profile_begin_strided.argtypes = [C.c_int, C.c_int]
-    lib.gsr_set_option.restype = C.c_int
-    lib.gsr_set_option.argtypes = [C.c_char_p, C.c_int]
-    lib.gsr_profile_end.restype = C.c_int
-    lib.gsr_profile_end.argtypes = [C.POINTER(C.c_float), C.POINTER(C.c_int)]
     return lib
 
 

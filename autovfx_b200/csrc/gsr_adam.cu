@@ -120,8 +120,13 @@ int adam_grid_cap() {
 }
 
 }  // namespace
+}  // namespace gsr
 
-int adam_step_impl(int n, const gsr_adam_tensor* tensors, cudaStream_t st) {
+using namespace gsr;
+
+int gsr_adam_step(int32_t n, const gsr_adam_tensor* tensors, void* stream) {
+    NvtxRange nvtx_("gsr_adam_step");
+    const cudaStream_t st = (cudaStream_t)stream;
     if (n < 0 || (n > 0 && !tensors)) {
         set_error("gsr_adam_step: %d tensors", n);
         return GSR_ERR_INVALID;
@@ -156,5 +161,3 @@ int adam_step_impl(int n, const gsr_adam_tensor* tensors, cudaStream_t st) {
     }
     return GSR_OK;
 }
-
-}  // namespace gsr

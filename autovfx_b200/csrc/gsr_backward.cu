@@ -546,7 +546,6 @@ struct DetLayout {
     }
     __host__ __device__ static size_t slot_bytes(bool extra) { return (size_t)GSR_FOOTS * det_nv(extra ? 3 : 0) * sizeof(float); }
 };
-size_t backward_det_bytes(size_t R, int W, int H, bool extra) { return DetLayout(R, ImageLayout(W < 1 ? 1 : W, H < 1 ? 1 : H).tiles, extra).total; }
 
 // =====================================================================================================
 // per-Gaussian backward (fused computeCov2DCUDA + preprocessCUDA backward)
@@ -869,10 +868,18 @@ static void launch_blend_backward(const BwdArgs& ba, dim3 grid, cudaStream_t st)
     else k_blend_backward<NX, 6, DET><<<grid, BWL_WARPS * 32, 0, st>>>(ba);
 }
 
+}  // namespace gsr
+
+using namespace gsr;
+
+size_t gsr_backward_det_bytes(size_t num_rendered, int32_t W, int32_t H, int with_extra) {
+    return DetLayout(num_rendered, ImageLayout(W < 1 ? 1 : W, H < 1 ? 1 : H).tiles, with_extra != 0).total;
+}
+
 // det: the deterministic backward (gsr_backward_det) with `scratch` of scratch_bytes; otherwise scratch is unused.
-int backward_impl(const gsr_frame* f, const gsr_workspace* ws, const int32_t* radii, const float* out_alpha, const float* dL_dc,
-                  const float* dL_dd, const float* dL_da, const float* extra_colors, const float* dL_de, float* dL_dextra,
-                  const gsr_grads* g, bool det, void* scratch, size_t scratch_bytes, cudaStream_t st) {
+static int backward_impl(const gsr_frame* f, const gsr_workspace* ws, const int32_t* radii, const float* out_alpha, const float* dL_dc,
+                         const float* dL_dd, const float* dL_da, const float* extra_colors, const float* dL_de, float* dL_dextra,
+                         const gsr_grads* g, bool det, void* scratch, size_t scratch_bytes, cudaStream_t st) {
     if (!f || !ws || !g) { set_error("gsr_backward: null argument"); return GSR_ERR_INVALID; }
     const int n_extra = (extra_colors != nullptr) + (dL_de != nullptr) + (dL_dextra != nullptr);
     if (n_extra != 0 && n_extra != 3) {
@@ -892,9 +899,9 @@ int backward_impl(const gsr_frame* f, const gsr_workspace* ws, const int32_t* ra
         if (!scratch) { set_error("gsr_backward_det: scratch is NULL"); return GSR_ERR_INVALID; }
         if ((uintptr_t)scratch & 15) { set_error("gsr_backward_det: scratch is not 16-byte aligned"); return GSR_ERR_INVALID; }
         if (f->P > 0 && (!radii || !out_alpha || !dL_dc || !dL_dd || !dL_da)) { set_error("gsr_backward_det: null input"); return GSR_ERR_INVALID; }
-        if (scratch_bytes < backward_det_bytes(0, f->W, f->H, multi)) {
+        if (scratch_bytes < gsr_backward_det_bytes(0, f->W, f->H, multi)) {
             set_error("gsr_backward_det: scratch of %zu bytes is too small: gsr_backward_det_bytes(num_rendered, W, H, with_extra) = "
-                      "%zu + %zu per rendered instance", scratch_bytes, backward_det_bytes(0, f->W, f->H, multi), DetLayout::slot_bytes(multi));
+                      "%zu + %zu per rendered instance", scratch_bytes, gsr_backward_det_bytes(0, f->W, f->H, multi), DetLayout::slot_bytes(multi));
             return GSR_ERR_WORKSPACE;
         }
     }
@@ -976,4 +983,27 @@ int backward_impl(const gsr_frame* f, const gsr_workspace* ws, const int32_t* ra
     return check_launch("gsr_backward/gaussian", debug, st);
 }
 
-}  // namespace gsr
+int gsr_backward(const gsr_frame* frame, const gsr_workspace* ws, const int32_t* radii, const float* out_alpha,
+                 const float* dL_dout_color, const float* dL_dout_depth, const float* dL_dout_alpha, const gsr_grads* grads,
+                 void* stream) {
+    NvtxRange nvtx_("gsr_backward");
+    return backward_impl(frame, ws, radii, out_alpha, dL_dout_color, dL_dout_depth, dL_dout_alpha, nullptr, nullptr, nullptr, grads, false,
+                         nullptr, 0, (cudaStream_t)stream);
+}
+
+int gsr_backward_multi(const gsr_frame* frame, const gsr_workspace* ws, const int32_t* radii, const float* out_alpha,
+                       const float* dL_dout_color, const float* dL_dout_depth, const float* dL_dout_alpha, const float* extra_colors,
+                       const float* dL_dout_extra, float* dL_dextra, const gsr_grads* grads, void* stream) {
+    NvtxRange nvtx_("gsr_backward_multi");
+    return backward_impl(frame, ws, radii, out_alpha, dL_dout_color, dL_dout_depth, dL_dout_alpha, extra_colors, dL_dout_extra, dL_dextra,
+                         grads, false, nullptr, 0, (cudaStream_t)stream);
+}
+
+int gsr_backward_det(const gsr_frame* frame, const gsr_workspace* ws, const int32_t* radii, const float* out_alpha,
+                     const float* dL_dout_color, const float* dL_dout_depth, const float* dL_dout_alpha, const float* extra_colors,
+                     const float* dL_dout_extra, float* dL_dextra, const gsr_grads* grads, void* scratch, size_t scratch_bytes,
+                     void* stream) {
+    NvtxRange nvtx_("gsr_backward_det");
+    return backward_impl(frame, ws, radii, out_alpha, dL_dout_color, dL_dout_depth, dL_dout_alpha, extra_colors, dL_dout_extra, dL_dextra,
+                         grads, true, scratch, scratch_bytes, (cudaStream_t)stream);
+}

@@ -8,6 +8,7 @@
 // memory access pattern, staging and parallel decomposition are ours.
 #pragma once
 #include <cuda_runtime.h>
+#include <nvtx3/nvToolsExt.h>  // header-only NVTX v3: the ranges cost nothing unless a profiler is attached
 #include <stdint.h>
 #include "../../include/gsr_b200.h"
 
@@ -539,7 +540,11 @@ __global__ void __launch_bounds__(1024) k_rs_scan(T* hist, int n) {
 }  // namespace
 
 void set_error(const char* fmt, ...);
-const char* last_error();
 int check_launch(const char* what, bool debug, cudaStream_t stream);
+
+struct NvtxRange {  // one named range per C-ABI call (SURVEY §5: the reference has no instrumentation; this build adds NVTX)
+    explicit NvtxRange(const char* name) { nvtxRangePushA(name); }
+    ~NvtxRange() { nvtxRangePop(); }
+};
 
 }  // namespace gsr

@@ -82,24 +82,6 @@ __global__ void __launch_bounds__(256) k_compose(const ComposeParams p) {
     }
 }
 
-int compose_impl(int N, int M, const float* xyz, const float* f_dc, const float* f_rest, const float* opacity_raw, const float* scaling_raw,
-                 const float* rotation_raw, const gsr_object_xform* xform, float* means3D, float* shs, float* opacities, float* scales,
-                 float* rotations, cudaStream_t st) {
-    if (N < 0 || M < 1) { set_error("gsr_activate_gaussians: bad sizes N=%d M=%d", N, M); return GSR_ERR_INVALID; }
-    if (N == 0) return GSR_OK;
-    if (!xyz || !f_dc || (M > 1 && !f_rest) || !opacity_raw || !scaling_raw || !rotation_raw || !means3D || !shs || !opacities || !scales || !rotations) {
-        set_error("gsr_activate_gaussians: null pointer");
-        return GSR_ERR_INVALID;
-    }
-    ComposeParams p{};
-    p.N = N; p.M = M; p.xyz = xyz; p.f_dc = f_dc; p.f_rest = f_rest; p.opacity_raw = opacity_raw; p.scaling_raw = scaling_raw;
-    p.rotation_raw = rotation_raw; p.means3D = means3D; p.shs = shs; p.opacities = opacities; p.scales = scales; p.rotations = rotations;
-    p.has_xform = xform != nullptr;
-    if (xform) p.x = *xform;
-    k_compose<<<(N + 255) / 256, 256, 0, st>>>(p);
-    return check_launch("gsr_activate_gaussians", false, st);
-}
-
 // ---- backward of the activation (xform = NULL) and of the remapped shading normal (gsr_axis_normals(..., remap01 = 1)) ----------
 // Gradients with respect to the activated tensors in, gradients with respect to the raw parameters out.  With s = exp(sigma),
 // r = rho / max(||rho||, 1e-12), o = sigmoid(omega) and e = n * 0.5 + 0.5 the shading normal of the smallest axis:
@@ -177,10 +159,36 @@ __global__ void __launch_bounds__(256) k_activate_backward(const ActivateBwdPara
     }
 }
 
-int activate_backward_impl(int N, int M, const float* xyz, const float* campos, const float* opacities, const float* scales,
-                           const float* rotations, const float* rotation_raw, const float* g_o, const float* g_s, const float* g_r,
-                           const float* g_sh, const float* g_e, float* d_opacity, float* d_scaling, float* d_rotation, float* d_fdc,
-                           float* d_frest, cudaStream_t st) {
+}  // namespace gsr
+
+using namespace gsr;
+
+int gsr_activate_gaussians(int32_t N, int32_t M, const float* xyz, const float* f_dc, const float* f_rest, const float* opacity_raw,
+                           const float* scaling_raw, const float* rotation_raw, const gsr_object_xform* xform, float* means3D, float* shs,
+                           float* opacities, float* scales, float* rotations, void* stream) {
+    NvtxRange nvtx_("gsr_activate_gaussians");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (N < 0 || M < 1) { set_error("gsr_activate_gaussians: bad sizes N=%d M=%d", N, M); return GSR_ERR_INVALID; }
+    if (N == 0) return GSR_OK;
+    if (!xyz || !f_dc || (M > 1 && !f_rest) || !opacity_raw || !scaling_raw || !rotation_raw || !means3D || !shs || !opacities || !scales || !rotations) {
+        set_error("gsr_activate_gaussians: null pointer");
+        return GSR_ERR_INVALID;
+    }
+    ComposeParams p{};
+    p.N = N; p.M = M; p.xyz = xyz; p.f_dc = f_dc; p.f_rest = f_rest; p.opacity_raw = opacity_raw; p.scaling_raw = scaling_raw;
+    p.rotation_raw = rotation_raw; p.means3D = means3D; p.shs = shs; p.opacities = opacities; p.scales = scales; p.rotations = rotations;
+    p.has_xform = xform != nullptr;
+    if (xform) p.x = *xform;
+    k_compose<<<(N + 255) / 256, 256, 0, st>>>(p);
+    return check_launch("gsr_activate_gaussians", false, st);
+}
+
+int gsr_activate_gaussians_backward(int32_t N, int32_t M, const float* xyz, const float* campos, const float* opacities,
+                                    const float* scales, const float* rotations, const float* rotation_raw, const float* g_o,
+                                    const float* g_s, const float* g_r, const float* g_sh, const float* g_e, float* d_opacity,
+                                    float* d_scaling, float* d_rotation, float* d_fdc, float* d_frest, void* stream) {
+    NvtxRange nvtx_("gsr_activate_gaussians_backward");
+    const cudaStream_t st = (cudaStream_t)stream;
     if (N < 0 || M < 1) { set_error("gsr_activate_gaussians_backward: bad sizes N=%d M=%d", N, M); return GSR_ERR_INVALID; }
     if (N == 0) return GSR_OK;
     if (!opacities || !scales || !rotations || !rotation_raw || !g_o || !g_s || !g_r || !d_opacity || !d_scaling || !d_rotation ||
@@ -195,5 +203,3 @@ int activate_backward_impl(int N, int M, const float* xyz, const float* campos, 
     k_activate_backward<<<(N + 255) / 256, 256, 0, st>>>(p);
     return check_launch("gsr_activate_gaussians_backward", false, st);
 }
-
-}  // namespace gsr

@@ -115,32 +115,6 @@ __global__ void k_pct_final(float t, int same, const PctState* __restrict__ st, 
     out[0] = st->nan ? __int_as_float(0x7fc00000) : r;
 }
 
-int percentile_low_impl(int64_t n, const float* x, float* out, void* ws, size_t ws_bytes, cudaStream_t s) {
-    if (n <= 0 || n > 0x7fffffffLL || !x || !out) { set_error("gsr_percentile_low: bad arguments (n %lld)", (long long)n); return GSR_ERR_INVALID; }
-    if (!ws || ((uintptr_t)ws & 15) || ws_bytes < GSR_PERCENTILE_BYTES) {
-        set_error("gsr_percentile_low: workspace of %zu bytes, GSR_PERCENTILE_BYTES (%d) needed (16-byte aligned)", ws_bytes, GSR_PERCENTILE_BYTES);
-        return GSR_ERR_WORKSPACE;
-    }
-    // numpy's index arithmetic, in float32 as NumPy >= 2 does it for a float32 array
-    const float q = 0.001f / 100.0f;
-    const float v = (float)(n - 1) * q;
-    const float fi = floorf(v);
-    const bool top = v >= (float)(n - 1);  // only n = 1: both statistics are the maximum (index -1)
-    const float t = top ? 1.0f : v - fi;   // numpy's gamma is v - (-1) there
-    const uint32_t rank = top ? (uint32_t)(n - 1) : (uint32_t)fi;
-    PctState* st = (PctState*)ws;
-    k_pct_init<<<1, 256, 0, s>>>(rank, st);
-    const int64_t tiles = (n + PCT_THREADS * PCT_ITEMS - 1) / (PCT_THREADS * PCT_ITEMS);
-    const unsigned grid = (unsigned)(tiles < 2048 ? tiles : 2048);
-    for (int pass = 0; pass < 4; pass++) {
-        k_pct_hist<<<grid, PCT_THREADS, 0, s>>>(n, x, pass, st);
-        k_pct_pick<<<1, 256, 0, s>>>(pass, st);
-    }
-    if (!top) k_pct_above<<<grid, PCT_THREADS, 0, s>>>(n, x, st);
-    k_pct_final<<<1, 1, 0, s>>>(t, top ? 1 : 0, st, out);
-    return check_launch("gsr_percentile_low", false, s);
-}
-
 // ------------------------------------------------------------------------------------------------------------- the composite
 __device__ __forceinline__ float byte_f(uint32_t px, int c) { return (float)((px >> (8 * c)) & 255u); }
 __device__ __forceinline__ float alpha_f(uint32_t px) { return __fdiv_rn((float)(px >> 24), 255.0f); }  // rgb[..., 3] / 255.
@@ -217,9 +191,43 @@ __global__ void __launch_bounds__(256) k_composite(int64_t HW, const uint32_t* _
     out[p] = to_u8(f[0]) | (to_u8(f[1]) << 8) | (to_u8(f[2]) << 16) | (to_u8(f[3]) << 24);
 }
 
-int composite_impl(int32_t W, int32_t H, const uint8_t* frame, const uint8_t* obj, const float* obj_d, const uint8_t* shadow,
-                   const float* shadow_d, const uint8_t* all, const uint8_t* gs, const float* gs_d, const uint8_t* smoke,
-                   const float* smoke_d, const float* smoke_pct, const uint8_t* fire, uint8_t* out, cudaStream_t s) {
+}  // namespace gsr
+
+using namespace gsr;
+
+int gsr_percentile_low(int64_t n, const float* x, float* out, void* ws, size_t ws_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_percentile_low");
+    const cudaStream_t s = (cudaStream_t)stream;
+    if (n <= 0 || n > 0x7fffffffLL || !x || !out) { set_error("gsr_percentile_low: bad arguments (n %lld)", (long long)n); return GSR_ERR_INVALID; }
+    if (!ws || ((uintptr_t)ws & 15) || ws_bytes < GSR_PERCENTILE_BYTES) {
+        set_error("gsr_percentile_low: workspace of %zu bytes, GSR_PERCENTILE_BYTES (%d) needed (16-byte aligned)", ws_bytes, GSR_PERCENTILE_BYTES);
+        return GSR_ERR_WORKSPACE;
+    }
+    // numpy's index arithmetic, in float32 as NumPy >= 2 does it for a float32 array
+    const float q = 0.001f / 100.0f;
+    const float v = (float)(n - 1) * q;
+    const float fi = floorf(v);
+    const bool top = v >= (float)(n - 1);  // only n = 1: both statistics are the maximum (index -1)
+    const float t = top ? 1.0f : v - fi;   // numpy's gamma is v - (-1) there
+    const uint32_t rank = top ? (uint32_t)(n - 1) : (uint32_t)fi;
+    PctState* st = (PctState*)ws;
+    k_pct_init<<<1, 256, 0, s>>>(rank, st);
+    const int64_t tiles = (n + PCT_THREADS * PCT_ITEMS - 1) / (PCT_THREADS * PCT_ITEMS);
+    const unsigned grid = (unsigned)(tiles < 2048 ? tiles : 2048);
+    for (int pass = 0; pass < 4; pass++) {
+        k_pct_hist<<<grid, PCT_THREADS, 0, s>>>(n, x, pass, st);
+        k_pct_pick<<<1, 256, 0, s>>>(pass, st);
+    }
+    if (!top) k_pct_above<<<grid, PCT_THREADS, 0, s>>>(n, x, st);
+    k_pct_final<<<1, 1, 0, s>>>(t, top ? 1 : 0, st, out);
+    return check_launch("gsr_percentile_low", false, s);
+}
+
+int gsr_composite(int32_t W, int32_t H, const uint8_t* frame, const uint8_t* obj, const float* obj_d, const uint8_t* shadow,
+                  const float* shadow_d, const uint8_t* all, const uint8_t* gs, const float* gs_d, const uint8_t* smoke,
+                  const float* smoke_d, const float* smoke_pct, const uint8_t* fire, uint8_t* out, void* stream) {
+    NvtxRange nvtx_("gsr_composite");
+    const cudaStream_t s = (cudaStream_t)stream;
     if (W <= 0 || H <= 0) { set_error("gsr_composite: bad size (%d x %d)", W, H); return GSR_ERR_INVALID; }
     if (!frame || !obj || !obj_d || !shadow || !shadow_d || !all || !out) { set_error("gsr_composite: a required layer is NULL"); return GSR_ERR_INVALID; }
     if (!gs != !gs_d || !smoke != !smoke_d || !smoke != !smoke_pct || (fire && !smoke)) {
@@ -249,5 +257,3 @@ int composite_impl(int32_t W, int32_t H, const uint8_t* frame, const uint8_t* ob
 #undef GSR_COMPOSITE
     return check_launch("gsr_composite", false, s);
 }
-
-}  // namespace gsr

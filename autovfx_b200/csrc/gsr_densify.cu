@@ -220,8 +220,14 @@ inline int nblocks_plan(int P) { return (P + PLAN_BLOCK - 1) / PLAN_BLOCK; }
 
 }  // namespace
 
-int densify_stats_impl(int P, int C, const float* grad, const uint8_t* mask, const int32_t* radii, float* accum, float* denom,
-                       float* max_radii, cudaStream_t st) {
+}  // namespace gsr
+
+using namespace gsr;
+
+int gsr_densify_stats(int32_t P, int32_t C, const float* grad, const uint8_t* mask, const int32_t* radii, float* accum, float* denom,
+                      float* max_radii, void* stream) {
+    NvtxRange nvtx_("gsr_densify_stats");
+    const cudaStream_t st = (cudaStream_t)stream;
     if (P < 0 || C < 2) {
         set_error("gsr_densify_stats: P = %d and C = %d (need P >= 0, C >= 2)", P, C);
         return GSR_ERR_INVALID;
@@ -235,14 +241,16 @@ int densify_stats_impl(int P, int C, const float* grad, const uint8_t* mask, con
     return check_launch("gsr_densify_stats", false, st);
 }
 
-size_t densify_plan_bytes(int P) {
+size_t gsr_densify_plan_bytes(int32_t P) {
     const size_t nb = P > 0 ? (size_t)nblocks_plan(P) : 0;
     return align_up((size_t)(P > 0 ? P : 0), 16) + 4 * (N_STREAMS * nb + 1);
 }
 
-int densify_plan_impl(int P, const float* accum, const float* denom, const float* scaling, const float* opacity, float max_grad,
-                      float dense_thr, float min_opacity, int use_screen, float max_screen_size, float big_thr, int32_t* dst,
-                      int32_t* totals, void* ws, size_t ws_bytes, cudaStream_t st) {
+int gsr_densify_plan(int32_t P, const float* accum, const float* denom, const float* scaling, const float* opacity, float max_grad,
+                     float dense_thr, float min_opacity, int32_t use_screen, float max_screen_size, float big_thr, int32_t* dst,
+                     int32_t* totals, void* ws, size_t ws_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_densify_plan");
+    const cudaStream_t st = (cudaStream_t)stream;
     if (P < 0 || P > INT32_MAX / 3) {
         set_error("gsr_densify_plan: P = %d outside 0..%d", P, INT32_MAX / 3);
         return GSR_ERR_INVALID;
@@ -251,8 +259,8 @@ int densify_plan_impl(int P, const float* accum, const float* denom, const float
         set_error("gsr_densify_plan: missing input or output");
         return GSR_ERR_INVALID;
     }
-    if (ws_bytes < densify_plan_bytes(P) || (P > 0 && !ws) || ((uintptr_t)ws & 15)) {
-        set_error("gsr_densify_plan: workspace of %zu bytes (need %zu, 16-byte aligned)", ws_bytes, densify_plan_bytes(P));
+    if (ws_bytes < gsr_densify_plan_bytes(P) || (P > 0 && !ws) || ((uintptr_t)ws & 15)) {
+        set_error("gsr_densify_plan: workspace of %zu bytes (need %zu, 16-byte aligned)", ws_bytes, gsr_densify_plan_bytes(P));
         return GSR_ERR_WORKSPACE;
     }
     if (P == 0) {
@@ -270,8 +278,10 @@ int densify_plan_impl(int P, const float* accum, const float* denom, const float
     return check_launch("gsr_densify_plan", false, st);
 }
 
-int densify_apply_impl(int P, int S, int n_groups, const gsr_densify_group* groups, const int32_t* dst, const float* xyz,
-                       const float* scaling, const float* rotation, const float* eps, int rotation_mode, cudaStream_t st) {
+int gsr_densify_apply(int32_t P, int32_t S, int32_t n_groups, const gsr_densify_group* groups, const int32_t* dst, const float* xyz,
+                      const float* scaling, const float* rotation, const float* eps, int32_t rotation_mode, void* stream) {
+    NvtxRange nvtx_("gsr_densify_apply");
+    const cudaStream_t st = (cudaStream_t)stream;
     if (P < 0 || S < 0 || S > P || n_groups < 0 || n_groups > GSR_DENSIFY_MAX_GROUPS || (n_groups > 0 && !groups) ||
         (rotation_mode != GSR_DENSIFY_ROTATION_3DGS && rotation_mode != GSR_DENSIFY_ROTATION_SUGAR)) {
         set_error("gsr_densify_apply: P = %d, S = %d, %d groups (at most %d), rotation mode %d", P, S, n_groups, GSR_DENSIFY_MAX_GROUPS,
@@ -302,5 +312,3 @@ int densify_apply_impl(int P, int S, int n_groups, const gsr_densify_group* grou
     k_densify_apply<<<grid, 256, 0, st>>>(a);
     return check_launch("gsr_densify_apply", false, st);
 }
-
-}  // namespace gsr

@@ -34,7 +34,6 @@ void set_error(const char* fmt, ...) {
     vsnprintf(g_err, sizeof g_err, fmt, ap);
     va_end(ap);
 }
-const char* last_error() { return g_err; }
 int check_launch(const char* what, bool debug, cudaStream_t stream) {
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess && debug) e = cudaStreamSynchronize(stream);
@@ -1195,6 +1194,15 @@ __global__ void __launch_bounds__(256) k_recolor(int P, const int* __restrict__ 
     c[2] = colors_precomp[3 * (size_t)idx + 2];
 }
 
+// checkFrustum (rasterizer_impl.cu:54-66): in_frustum() only tests view-space z (auxiliary.h:154)
+__global__ void k_mark_visible(int P, const float* __restrict__ means3D, const float* __restrict__ view, uint8_t* __restrict__ present) {
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= P) return;
+    const float3 p = {means3D[3 * (size_t)idx], means3D[3 * (size_t)idx + 1], means3D[3 * (size_t)idx + 2]};
+    const float3 pv = xform4x3(p, view);
+    present[idx] = !(pv.z <= 0.2f);
+}
+
 // =====================================================================================================
 // optional per-kernel timing (bench.py roofline): CUDA events recorded around each forward kernel on the
 // launching stream; no effect unless gsr_profile_begin() was called.  Not thread safe (one profiled stream).
@@ -1209,40 +1217,6 @@ struct ProfileState {
 static ProfileState g_prof;
 static inline void prof_mark(int k, cudaStream_t st) {
     if (g_prof.on && g_prof.frames < g_prof.max_frames && g_prof.seen % g_prof.stride == 0) cudaEventRecord(g_prof.ev[g_prof.frames * 6 + k], st);
-}
-int profile_begin(int max_frames, int stride) {
-    if (max_frames <= 0 || stride <= 0) { set_error("gsr_profile_begin: max_frames and stride must be > 0"); return GSR_ERR_INVALID; }
-    if (g_prof.allocated < max_frames * 6) {
-        cudaEvent_t* ne = new cudaEvent_t[max_frames * 6];
-        for (int i = 0; i < max_frames * 6; i++) {
-            if (i < g_prof.allocated) ne[i] = g_prof.ev[i];
-            else if (cudaEventCreate(&ne[i]) != cudaSuccess) { set_error("gsr_profile_begin: cudaEventCreate failed"); return GSR_ERR_CUDA; }
-        }
-        delete[] g_prof.ev;
-        g_prof.ev = ne;
-        g_prof.allocated = max_frames * 6;
-    }
-    g_prof.max_frames = max_frames;
-    g_prof.frames = 0;
-    g_prof.stride = stride;
-    g_prof.seen = 0;
-    g_prof.on = true;
-    return GSR_OK;
-}
-int profile_end(float* ms, int* frames) {
-    g_prof.on = false;
-    double acc[5] = {0, 0, 0, 0, 0};
-    for (int f = 0; f < g_prof.frames; f++) {
-        if (cudaEventSynchronize(g_prof.ev[f * 6 + 5]) != cudaSuccess) { set_error("gsr_profile_end: event sync failed"); return GSR_ERR_CUDA; }
-        for (int k = 0; k < 5; k++) {
-            float t = 0;
-            cudaEventElapsedTime(&t, g_prof.ev[f * 6 + k], g_prof.ev[f * 6 + k + 1]);
-            acc[k] += t;
-        }
-    }
-    for (int k = 0; k < 5; k++) ms[k] = g_prof.frames ? (float)(acc[k] / g_prof.frames) : 0.f;
-    if (frames) *frames = g_prof.frames;
-    return GSR_OK;
 }
 
 // =====================================================================================================
@@ -1279,14 +1253,95 @@ struct ForwardOptions {
 };
 static ForwardOptions g_opt;
 int set_blend_persist(int k);
-int set_option(const char* name, int value) {
-    if (strcmp(name, "blend_persist") == 0) return set_blend_persist(value);
-    if (strcmp(name, "sort_single_pass") == 0) { g_opt.sort_single_pass = value ? 1 : 0; return GSR_OK; }
-    return GSR_ERR_INVALID;
+
+}  // namespace gsr
+
+using namespace gsr;
+
+int gsr_abi_version(void) { return GSR_ABI_VERSION; }
+const char* gsr_last_error(void) { return g_err; }
+
+size_t gsr_geom_bytes(int32_t P) { return GeomLayout((size_t)(P < 0 ? 0 : P)).total; }
+size_t gsr_binning_bytes(size_t capacity) { return BinLayout(capacity < 1 ? 1 : capacity).total; }
+size_t gsr_binning_capacity(size_t bytes) { return BinLayout::capacity_of(bytes); }
+size_t gsr_binning_bytes_slab(size_t capacity, int32_t W, int32_t H, int32_t slab_stride) {
+    if (slab_stride <= 0) return gsr_binning_bytes(capacity);
+    const ImageLayout il(W < 1 ? 1 : W, H < 1 ? 1 : H);
+    return BinLayout::bytes_with_slab(capacity < 1 ? 1 : capacity, (size_t)il.tiles * (size_t)slab_stride);
+}
+size_t gsr_binning_capacity_slab(size_t bytes, int32_t W, int32_t H, int32_t slab_stride) {
+    if (slab_stride <= 0) return gsr_binning_capacity(bytes);
+    const ImageLayout il(W < 1 ? 1 : W, H < 1 ? 1 : H);
+    return BinLayout::slab_offset(BinLayout::capacity_of(bytes), (size_t)il.tiles * (size_t)slab_stride) / 8;
+}
+size_t gsr_image_bytes(int32_t W, int32_t H) { return ImageLayout(W < 1 ? 1 : W, H < 1 ? 1 : H).total; }
+
+int gsr_get_views(const gsr_workspace* ws, int32_t P, int32_t W, int32_t H, gsr_views* out) {
+    if (!ws || !out) { set_error("gsr_get_views: null argument"); return GSR_ERR_INVALID; }
+    const GeomLayout gl((size_t)P);
+    const ImageLayout il(W, H);
+    const BinLayout bl(BinLayout::capacity_of(ws->binning_bytes));
+    const char* geo = (const char*)ws->geom; const char* img = (const char*)ws->image; const char* bin = (const char*)ws->binning;
+    out->records = (const float*)(geo + gl.records);
+    out->cov3D = (const float*)(geo + gl.cov3D);
+    out->clamped = (const uint8_t*)(geo + gl.clamped);
+    out->point_list = (const uint32_t*)(bin + bl.point_list);
+    out->sorted_keys = (const uint64_t*)(bin + bl.pairs);
+    out->ranges = (const uint32_t*)(img + il.ranges);
+    out->n_contrib = (const uint32_t*)(img + il.n_contrib);
+    out->tile_count = (const uint32_t*)(img + il.tile_count);
+    out->tile_big = (const uint32_t*)(img + il.tile_big);
+    out->counters = (const gsr_counters*)(img + il.counters);
+    return GSR_OK;
 }
 
-int forward_impl(const gsr_frame* f, const gsr_workspace* ws, float* out_color, float* out_depth, float* out_alpha,
-                 int32_t* radii, const float* extra_colors, float* out_extra, int flags, cudaStream_t st) {
+int gsr_profile_begin(int max_frames) { return gsr_profile_begin_strided(max_frames, 1); }
+int gsr_profile_begin_strided(int max_frames, int stride) {
+    if (max_frames <= 0 || stride <= 0) { set_error("gsr_profile_begin: max_frames and stride must be > 0"); return GSR_ERR_INVALID; }
+    if (g_prof.allocated < max_frames * 6) {
+        cudaEvent_t* ne = new cudaEvent_t[max_frames * 6];
+        for (int i = 0; i < max_frames * 6; i++) {
+            if (i < g_prof.allocated) ne[i] = g_prof.ev[i];
+            else if (cudaEventCreate(&ne[i]) != cudaSuccess) { set_error("gsr_profile_begin: cudaEventCreate failed"); return GSR_ERR_CUDA; }
+        }
+        delete[] g_prof.ev;
+        g_prof.ev = ne;
+        g_prof.allocated = max_frames * 6;
+    }
+    g_prof.max_frames = max_frames;
+    g_prof.frames = 0;
+    g_prof.stride = stride;
+    g_prof.seen = 0;
+    g_prof.on = true;
+    return GSR_OK;
+}
+int gsr_profile_end(float* ms, int* frames) {
+    g_prof.on = false;
+    double acc[5] = {0, 0, 0, 0, 0};
+    for (int f = 0; f < g_prof.frames; f++) {
+        if (cudaEventSynchronize(g_prof.ev[f * 6 + 5]) != cudaSuccess) { set_error("gsr_profile_end: event sync failed"); return GSR_ERR_CUDA; }
+        for (int k = 0; k < 5; k++) {
+            float t = 0;
+            cudaEventElapsedTime(&t, g_prof.ev[f * 6 + k], g_prof.ev[f * 6 + k + 1]);
+            acc[k] += t;
+        }
+    }
+    for (int k = 0; k < 5; k++) ms[k] = g_prof.frames ? (float)(acc[k] / g_prof.frames) : 0.f;
+    if (frames) *frames = g_prof.frames;
+    return GSR_OK;
+}
+
+int gsr_set_option(const char* name, int value) {
+    if (!name) { set_error("gsr_set_option: null name"); return GSR_ERR_INVALID; }
+    int rc = GSR_ERR_INVALID;
+    if (strcmp(name, "blend_persist") == 0) rc = set_blend_persist(value);
+    else if (strcmp(name, "sort_single_pass") == 0) { g_opt.sort_single_pass = value ? 1 : 0; rc = GSR_OK; }
+    if (rc != GSR_OK) set_error("gsr_set_option: unknown option or bad value (%s = %d)", name, value);
+    return rc;
+}
+
+static int forward_impl(const gsr_frame* f, const gsr_workspace* ws, float* out_color, float* out_depth, float* out_alpha,
+                        int32_t* radii, const float* extra_colors, float* out_extra, int flags, cudaStream_t st) {
     if (!f || !ws) { set_error("gsr_forward: null frame/workspace"); return GSR_ERR_INVALID; }
     if (f->P < 0 || f->W <= 0 || f->H <= 0) { set_error("gsr_forward: bad sizes P=%d W=%d H=%d", f->P, f->W, f->H); return GSR_ERR_INVALID; }
     if (!out_color || !out_depth || !out_alpha) { set_error("gsr_forward: null output image"); return GSR_ERR_INVALID; }
@@ -1443,4 +1498,24 @@ int forward_impl(const gsr_frame* f, const gsr_workspace* ws, float* out_color, 
     return check_launch("gsr_forward/blend", debug, st);
 }
 
-}  // namespace gsr
+int gsr_forward(const gsr_frame* frame, const gsr_workspace* ws, float* out_color, float* out_depth, float* out_alpha,
+                int32_t* radii, int flags, void* stream) {
+    NvtxRange nvtx_("gsr_forward");
+    return forward_impl(frame, ws, out_color, out_depth, out_alpha, radii, nullptr, nullptr, flags, (cudaStream_t)stream);
+}
+
+int gsr_forward_multi(const gsr_frame* frame, const gsr_workspace* ws, float* out_color, float* out_depth, float* out_alpha,
+                      int32_t* radii, const float* extra_colors, float* out_extra, int flags, void* stream) {
+    NvtxRange nvtx_("gsr_forward_multi");
+    return forward_impl(frame, ws, out_color, out_depth, out_alpha, radii, extra_colors, out_extra, flags, (cudaStream_t)stream);
+}
+
+int gsr_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix, uint8_t* present,
+                     void* stream) {
+    (void)projmatrix;
+    if (P < 0 || (P > 0 && (!means3D || !viewmatrix || !present))) { set_error("gsr_mark_visible: bad arguments"); return GSR_ERR_INVALID; }
+    if (P == 0) return GSR_OK;
+    const cudaStream_t st = (cudaStream_t)stream;
+    k_mark_visible<<<(P + 255) / 256, 256, 0, st>>>(P, means3D, viewmatrix, present);
+    return check_launch("gsr_mark_visible", false, st);
+}

@@ -48,7 +48,6 @@ struct KnnLayout {
         total = o + 256;
     }
 };
-size_t dist2_bytes(int P) { return KnnLayout((size_t)(P < 0 ? 0 : P)).total; }
 
 __device__ __forceinline__ uint32_t f2ord(float f) {
     uint32_t u = __float_as_uint(f);
@@ -247,36 +246,6 @@ __global__ void __launch_bounds__(KNN_QCTA) k_knn_search(int P, const float4* __
     dists[orig] = (b0 + b1 + b2) / 3.0f;
 }
 
-int dist2_impl(int P, const float* points, float* out, void* ws, size_t ws_bytes, cudaStream_t st) {
-    if (P < 0) { set_error("gsr_dist2: negative P"); return GSR_ERR_INVALID; }
-    if (P == 0) return GSR_OK;
-    if (!points || !out) { set_error("gsr_dist2: null pointer"); return GSR_ERR_INVALID; }
-    const KnnLayout L((size_t)P);
-    if (!ws || ws_bytes < L.total) { set_error("gsr_dist2: workspace too small (%zu < %zu)", ws_bytes, L.total); return GSR_ERR_WORKSPACE; }
-    char* w = (char*)ws;
-    uint32_t* bbox = (uint32_t*)(w + L.bbox);
-    uint32_t *k0 = (uint32_t*)(w + L.codes0), *k1 = (uint32_t*)(w + L.codes1), *v0 = (uint32_t*)(w + L.idx0), *v1 = (uint32_t*)(w + L.idx1);
-    uint32_t* hist = (uint32_t*)(w + L.hist);
-    float* boxes = (float*)(w + L.boxes);
-    k_bbox_init<<<1, 32, 0, st>>>(bbox);
-    k_bbox<<<min(132 * 8, (P + 255) / 256), 256, 0, st>>>(P, points, bbox);
-    k_morton<<<(P + 255) / 256, 256, 0, st>>>(P, points, bbox, k0, v0);
-    const int rs_blocks = (L.nchunks + RS_WARPS - 1) / RS_WARPS;
-    for (int pass = 0; pass < 4; pass++) {
-        k_rs_hist<<<rs_blocks, RS_WARPS * 32, 0, st>>>(P, k0, pass * 8, L.nchunks, hist);
-        k_rs_scan<<<1, 1024, 0, st>>>(hist, 256 * L.nchunks);
-        k_rs_scatter<<<rs_blocks, RS_WARPS * 32, 0, st>>>(P, k0, v0, pass * 8, L.nchunks, hist, k1, v1);
-        uint32_t* t = k0; k0 = k1; k1 = t;
-        t = v0; v0 = v1; v1 = t;
-    }
-    float4* sorted = (float4*)(w + L.sorted);
-    float* subboxes = (float*)(w + L.subboxes);
-    k_gather_sorted<<<(P + 255) / 256, 256, 0, st>>>(P, points, v0, sorted);
-    k_box_minmax<<<L.nboxes, 512, 0, st>>>(P, sorted, boxes, subboxes);
-    k_knn_search<<<(P + KNN_QCTA - 1) / KNN_QCTA, KNN_QCTA, 0, st>>>(P, sorted, boxes, subboxes, L.nboxes, out);
-    return check_launch("gsr_dist2", false, st);
-}
-
 // ================================================================================================================================
 // gsr_knn — exact K nearest neighbours (pytorch3d.ops.knn_points for N = 1, D = 3, K <= 32) on the same Morton boxes.
 //
@@ -472,11 +441,54 @@ static void knn_launch(bool self, int P1, int P2, int K, const float4* qsorted, 
         k_knn_topk<KCAP, false><<<grid, KNN_QCTA, 0, st>>>(P1, P2, K, qsorted, qcodes, sorted, pcodes, boxes, subboxes, nboxes, out_d, out_i);
 }
 
-// the points' layout, then (general queries only) the queries' layout
-size_t knn_bytes(int P1, int P2) { return KnnLayout((size_t)max(P2, 0)).total + KnnLayout((size_t)max(P1, 0)).total; }
+}  // namespace gsr
 
-int knn_impl(int P1, int P2, int K, const float* queries, const float* points, float* out_d, int64_t* out_i, void* ws, size_t ws_bytes,
-             cudaStream_t st) {
+using namespace gsr;
+
+size_t gsr_dist2_bytes(int32_t P) { return KnnLayout((size_t)(P < 0 ? 0 : P)).total; }
+
+int gsr_dist2(int32_t P, const float* points, float* out, void* ws, size_t ws_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_dist2");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (P < 0) { set_error("gsr_dist2: negative P"); return GSR_ERR_INVALID; }
+    if (P == 0) return GSR_OK;
+    if (!points || !out) { set_error("gsr_dist2: null pointer"); return GSR_ERR_INVALID; }
+    const KnnLayout L((size_t)P);
+    if (!ws || ws_bytes < L.total) { set_error("gsr_dist2: workspace too small (%zu < %zu)", ws_bytes, L.total); return GSR_ERR_WORKSPACE; }
+    char* w = (char*)ws;
+    uint32_t* bbox = (uint32_t*)(w + L.bbox);
+    uint32_t *k0 = (uint32_t*)(w + L.codes0), *k1 = (uint32_t*)(w + L.codes1), *v0 = (uint32_t*)(w + L.idx0), *v1 = (uint32_t*)(w + L.idx1);
+    uint32_t* hist = (uint32_t*)(w + L.hist);
+    float* boxes = (float*)(w + L.boxes);
+    k_bbox_init<<<1, 32, 0, st>>>(bbox);
+    k_bbox<<<min(132 * 8, (P + 255) / 256), 256, 0, st>>>(P, points, bbox);
+    k_morton<<<(P + 255) / 256, 256, 0, st>>>(P, points, bbox, k0, v0);
+    const int rs_blocks = (L.nchunks + RS_WARPS - 1) / RS_WARPS;
+    for (int pass = 0; pass < 4; pass++) {
+        k_rs_hist<<<rs_blocks, RS_WARPS * 32, 0, st>>>(P, k0, pass * 8, L.nchunks, hist);
+        k_rs_scan<<<1, 1024, 0, st>>>(hist, 256 * L.nchunks);
+        k_rs_scatter<<<rs_blocks, RS_WARPS * 32, 0, st>>>(P, k0, v0, pass * 8, L.nchunks, hist, k1, v1);
+        uint32_t* t = k0; k0 = k1; k1 = t;
+        t = v0; v0 = v1; v1 = t;
+    }
+    float4* sorted = (float4*)(w + L.sorted);
+    float* subboxes = (float*)(w + L.subboxes);
+    k_gather_sorted<<<(P + 255) / 256, 256, 0, st>>>(P, points, v0, sorted);
+    k_box_minmax<<<L.nboxes, 512, 0, st>>>(P, sorted, boxes, subboxes);
+    k_knn_search<<<(P + KNN_QCTA - 1) / KNN_QCTA, KNN_QCTA, 0, st>>>(P, sorted, boxes, subboxes, L.nboxes, out);
+    return check_launch("gsr_dist2", false, st);
+}
+
+// the points' layout, then (general queries only) the queries' layout; the workspace does not depend on K
+size_t gsr_knn_bytes(int32_t P1, int32_t P2, int32_t K) {
+    (void)K;
+    return KnnLayout((size_t)max(P2, 0)).total + KnnLayout((size_t)max(P1, 0)).total;
+}
+
+int gsr_knn(int32_t P1, int32_t P2, int32_t K, const float* queries, const float* points, float* out_d, int64_t* out_i, void* ws,
+            size_t ws_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_knn");
+    const cudaStream_t st = (cudaStream_t)stream;
     if (P1 < 0 || P2 < 0) { set_error("gsr_knn: negative size (P1 = %d, P2 = %d)", P1, P2); return GSR_ERR_INVALID; }
     if (K < 1 || K > KNN_KMAX) { set_error("gsr_knn: K = %d outside 1..%d", K, KNN_KMAX); return GSR_ERR_INVALID; }
     if (K > P2) { set_error("gsr_knn: K = %d > P2 = %d", K, P2); return GSR_ERR_INVALID; }
@@ -514,5 +526,3 @@ int knn_impl(int P1, int P2, int K, const float* queries, const float* points, f
     else knn_launch<32>(self, P1, P2, K, qsorted, qcodes, sorted, pcodes, boxes, subboxes, L.nboxes, out_d, out_i, st);
     return check_launch("gsr_knn", false, st);
 }
-
-}  // namespace gsr

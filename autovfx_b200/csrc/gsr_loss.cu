@@ -369,21 +369,46 @@ Window make_window(const float* w) {
 
 }  // namespace
 
-size_t photometric_loss_bytes(int B, int C, int H, int W, int for_backward) {
+static int normal_args(const char* who, int64_t n, const float* pred, const int64_t* ps, const float* gt, const int64_t* gs,
+                       const float* depth, int64_t d_sp, float scene_scale, NormalArgs& a) {
+    if (n <= 0 || !pred || !ps || !gt || !gs) {
+        set_error("%s: bad arguments (n %lld)", who, (long long)n);
+        return GSR_ERR_INVALID;
+    }
+    a = NormalArgs{n, pred, ps[0], ps[1], gt, gs[0], gs[1], depth, d_sp, scene_scale};
+    return GSR_OK;
+}
+
+static int check_reduce_ws(const char* who, const void* ws, size_t ws_bytes) {
+    if (!ws || ws_bytes < GSR_LOSS_REDUCE_BYTES || ((uintptr_t)ws & 15u)) {
+        set_error("%s: workspace of %zu bytes, GSR_LOSS_REDUCE_BYTES (%d) needed (16-byte aligned)", who, ws_bytes,
+                  GSR_LOSS_REDUCE_BYTES);
+        return GSR_ERR_WORKSPACE;
+    }
+    return GSR_OK;
+}
+
+}  // namespace gsr
+
+using namespace gsr;
+
+size_t gsr_photometric_loss_bytes(int32_t B, int32_t C, int32_t H, int32_t W, int32_t for_backward) {
     if (!photo_dims_ok(B, C, H, W)) return 0;
     const size_t n = (size_t)B * C * H * W;
     return 256 + align256(photo_blocks(B, C, H, W) * 2 * sizeof(float)) + (for_backward ? align256(3 * n * sizeof(float)) : 0);
 }
 
-int photometric_loss_impl(int B, int C, int H, int W, const float* x, const int64_t* xs, const float* y, const int64_t* ys,
-                          const float* window, int for_backward, float* out_l1, float* out_ssim, void* ws, size_t ws_bytes,
-                          cudaStream_t st) {
+int gsr_photometric_loss(int32_t B, int32_t C, int32_t H, int32_t W, const float* x, const int64_t* xs, const float* y,
+                         const int64_t* ys, const float* window, int32_t for_backward, float* out_l1, float* out_ssim, void* ws,
+                         size_t ws_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_photometric_loss");
+    const cudaStream_t st = (cudaStream_t)stream;
     if (!photo_dims_ok(B, C, H, W) || !x || !xs || !y || !ys || !window || !out_ssim) {
         set_error("gsr_photometric_loss: bad arguments (B %d, C %d, H %d, W %d)", B, C, H, W);
         return GSR_ERR_INVALID;
     }
     const bool store = for_backward != 0;
-    const size_t need = photometric_loss_bytes(B, C, H, W, store);
+    const size_t need = gsr_photometric_loss_bytes(B, C, H, W, store);
     if (!ws || ws_bytes < need || ((uintptr_t)ws & 15u)) {
         set_error("gsr_photometric_loss: workspace of %zu bytes, %zu needed (16-byte aligned)", ws_bytes, need);
         return GSR_ERR_WORKSPACE;
@@ -407,14 +432,16 @@ int photometric_loss_impl(int B, int C, int H, int W, const float* x, const int6
     return check_launch("gsr_photometric_loss", false, st);
 }
 
-int photometric_loss_backward_impl(int B, int C, int H, int W, const float* x, const int64_t* xs, const float* y, const int64_t* ys,
-                                   const float* window, const float* g_l1, const float* g_ssim, float* dx, const void* ws,
-                                   size_t ws_bytes, cudaStream_t st) {
+int gsr_photometric_loss_backward(int32_t B, int32_t C, int32_t H, int32_t W, const float* x, const int64_t* xs, const float* y,
+                                  const int64_t* ys, const float* window, const float* g_l1, const float* g_ssim, float* dx,
+                                  const void* ws, size_t ws_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_photometric_loss_backward");
+    const cudaStream_t st = (cudaStream_t)stream;
     if (!photo_dims_ok(B, C, H, W) || !x || !xs || !y || !ys || !window || !dx) {
         set_error("gsr_photometric_loss_backward: bad arguments (B %d, C %d, H %d, W %d)", B, C, H, W);
         return GSR_ERR_INVALID;
     }
-    const size_t need = photometric_loss_bytes(B, C, H, W, 1);
+    const size_t need = gsr_photometric_loss_bytes(B, C, H, W, 1);
     if (!ws || ws_bytes < need || ((uintptr_t)ws & 15u)) {
         set_error("gsr_photometric_loss_backward: workspace of %zu bytes, %zu needed (the forward's, with for_backward)",
                   ws_bytes, need);
@@ -433,27 +460,10 @@ int photometric_loss_backward_impl(int B, int C, int H, int W, const float* x, c
     return check_launch("gsr_photometric_loss_backward", false, st);
 }
 
-static int normal_args(const char* who, int64_t n, const float* pred, const int64_t* ps, const float* gt, const int64_t* gs,
-                       const float* depth, int64_t d_sp, float scene_scale, NormalArgs& a) {
-    if (n <= 0 || !pred || !ps || !gt || !gs) {
-        set_error("%s: bad arguments (n %lld)", who, (long long)n);
-        return GSR_ERR_INVALID;
-    }
-    a = NormalArgs{n, pred, ps[0], ps[1], gt, gs[0], gs[1], depth, d_sp, scene_scale};
-    return GSR_OK;
-}
-
-static int check_reduce_ws(const char* who, const void* ws, size_t ws_bytes) {
-    if (!ws || ws_bytes < GSR_LOSS_REDUCE_BYTES || ((uintptr_t)ws & 15u)) {
-        set_error("%s: workspace of %zu bytes, GSR_LOSS_REDUCE_BYTES (%d) needed (16-byte aligned)", who, ws_bytes,
-                  GSR_LOSS_REDUCE_BYTES);
-        return GSR_ERR_WORKSPACE;
-    }
-    return GSR_OK;
-}
-
-int normal_loss_impl(int64_t n, const float* pred, const int64_t* ps, const float* gt, const int64_t* gs, const float* depth,
-                     int64_t d_sp, float scene_scale, float* out, void* ws, size_t ws_bytes, cudaStream_t st) {
+int gsr_normal_loss(int64_t n, const float* pred, const int64_t* ps, const float* gt, const int64_t* gs, const float* depth,
+                    int64_t d_sp, float scene_scale, float* out, void* ws, size_t ws_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_normal_loss");
+    const cudaStream_t st = (cudaStream_t)stream;
     NormalArgs a;
     int rc = normal_args("gsr_normal_loss", n, pred, ps, gt, gs, depth, d_sp, scene_scale, a);
     if (rc == GSR_OK && !out) { set_error("gsr_normal_loss: null output"); rc = GSR_ERR_INVALID; }
@@ -466,9 +476,11 @@ int normal_loss_impl(int64_t n, const float* pred, const int64_t* ps, const floa
     return check_launch("gsr_normal_loss", false, st);
 }
 
-int normal_loss_backward_impl(int64_t n, const float* pred, const int64_t* ps, const float* gt, const int64_t* gs, const float* depth,
-                              int64_t d_sp, float scene_scale, const float* g_out, float* d_pred, const void* ws, size_t ws_bytes,
-                              cudaStream_t st) {
+int gsr_normal_loss_backward(int64_t n, const float* pred, const int64_t* ps, const float* gt, const int64_t* gs,
+                             const float* depth, int64_t d_sp, float scene_scale, const float* g_out, float* d_pred, const void* ws,
+                             size_t ws_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_normal_loss_backward");
+    const cudaStream_t st = (cudaStream_t)stream;
     NormalArgs a;
     int rc = normal_args("gsr_normal_loss_backward", n, pred, ps, gt, gs, depth, d_sp, scene_scale, a);
     if (rc == GSR_OK && (!g_out || !d_pred)) { set_error("gsr_normal_loss_backward: null gradient"); rc = GSR_ERR_INVALID; }
@@ -478,7 +490,9 @@ int normal_loss_backward_impl(int64_t n, const float* pred, const int64_t* ps, c
     return check_launch("gsr_normal_loss_backward", false, st);
 }
 
-int anisotropic_loss_impl(int64_t P, const float* scales, float r, float* out, void* ws, size_t ws_bytes, cudaStream_t st) {
+int gsr_anisotropic_loss(int64_t P, const float* scales, float r, float* out, void* ws, size_t ws_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_anisotropic_loss");
+    const cudaStream_t st = (cudaStream_t)stream;
     if (P <= 0 || !scales || !out) {
         set_error("gsr_anisotropic_loss: bad arguments (P %lld)", (long long)P);
         return GSR_ERR_INVALID;
@@ -492,7 +506,9 @@ int anisotropic_loss_impl(int64_t P, const float* scales, float r, float* out, v
     return check_launch("gsr_anisotropic_loss", false, st);
 }
 
-int anisotropic_loss_backward_impl(int64_t P, const float* scales, float r, const float* g_out, float* d_scales, cudaStream_t st) {
+int gsr_anisotropic_loss_backward(int64_t P, const float* scales, float r, const float* g_out, float* d_scales, void* stream) {
+    NvtxRange nvtx_("gsr_anisotropic_loss_backward");
+    const cudaStream_t st = (cudaStream_t)stream;
     if (P <= 0 || !scales || !g_out || !d_scales) {
         set_error("gsr_anisotropic_loss_backward: bad arguments (P %lld)", (long long)P);
         return GSR_ERR_INVALID;
@@ -500,5 +516,3 @@ int anisotropic_loss_backward_impl(int64_t P, const float* scales, float r, cons
     k_aniso_bwd<<<reduce_blocks(P), RB, 0, st>>>(P, scales, r, g_out, d_scales);
     return check_launch("gsr_anisotropic_loss_backward", false, st);
 }
-
-}  // namespace gsr

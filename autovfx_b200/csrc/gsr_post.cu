@@ -170,24 +170,34 @@ __global__ void __launch_bounds__(256) k_pack_frame(int W, int H, const float* _
     }
 }
 
-int axis_normals_impl(int P, const float* means3D, const float* scales, const float* rotations, const float* campos, int remap01,
-                      float* out, cudaStream_t st) {
+}  // namespace gsr
+
+using namespace gsr;
+
+int gsr_axis_normals(int32_t P, const float* means3D, const float* scales, const float* rotations, const float* campos, int remap01,
+                     float* out, void* stream) {
+    NvtxRange nvtx_("gsr_axis_normals");
+    const cudaStream_t st = (cudaStream_t)stream;
     if (P < 0 || (P > 0 && (!means3D || !scales || !rotations || !campos || !out))) { set_error("gsr_axis_normals: bad arguments"); return GSR_ERR_INVALID; }
     if (P == 0) return GSR_OK;
     k_axis_normals<<<(P + 255) / 256, 256, 0, st>>>(P, means3D, scales, rotations, campos, remap01, out);
     return check_launch("gsr_axis_normals", false, st);
 }
 
-int sugar_normals_impl(int P, const float* positions, const float* scales, const float* quaternions, const float* campos, float* out,
-                       cudaStream_t st) {
+int gsr_sugar_normals(int32_t P, const float* positions, const float* scales, const float* quaternions, const float* campos, float* out,
+                      void* stream) {
+    NvtxRange nvtx_("gsr_sugar_normals");
+    const cudaStream_t st = (cudaStream_t)stream;
     if (P < 0 || (P > 0 && (!positions || !scales || !quaternions || !campos || !out))) { set_error("gsr_sugar_normals: bad arguments"); return GSR_ERR_INVALID; }
     if (P == 0) return GSR_OK;
     k_sugar_normals<<<(P + 255) / 256, 256, 0, st>>>(P, positions, scales, quaternions, campos, out);
     return check_launch("gsr_sugar_normals", false, st);
 }
 
-int sugar_normals_backward_impl(int P, const float* positions, const float* scales, const float* quaternions, const float* campos,
-                                const float* dL_dnormals, float* dL_dquaternions, cudaStream_t st) {
+int gsr_sugar_normals_backward(int32_t P, const float* positions, const float* scales, const float* quaternions, const float* campos,
+                               const float* dL_dnormals, float* dL_dquaternions, void* stream) {
+    NvtxRange nvtx_("gsr_sugar_normals_backward");
+    const cudaStream_t st = (cudaStream_t)stream;
     if (P < 0 || (P > 0 && (!positions || !scales || !quaternions || !campos || !dL_dnormals || !dL_dquaternions))) {
         set_error("gsr_sugar_normals_backward: bad arguments");
         return GSR_ERR_INVALID;
@@ -197,8 +207,10 @@ int sugar_normals_backward_impl(int P, const float* positions, const float* scal
     return check_launch("gsr_sugar_normals_backward", false, st);
 }
 
-int normal_maps_impl(int W, int H, const float* normal_img, const float* depth, const float* c2w, float fx, float fy, float cx, float cy,
-                     float* out_normal, float* out_pseudo, cudaStream_t st) {
+int gsr_normal_maps(int32_t W, int32_t H, const float* normal_img, const float* depth, const float* c2w, float fx, float fy, float cx,
+                    float cy, float* out_normal, float* out_pseudo, void* stream) {
+    NvtxRange nvtx_("gsr_normal_maps");
+    const cudaStream_t st = (cudaStream_t)stream;
     if (W <= 0 || H <= 0) { set_error("gsr_normal_maps: bad size"); return GSR_ERR_INVALID; }
     if ((normal_img == nullptr) != (out_normal == nullptr) || (depth == nullptr) != (out_pseudo == nullptr) || (depth && !c2w)) {
         set_error("gsr_normal_maps: inputs and outputs must come in pairs");
@@ -208,8 +220,10 @@ int normal_maps_impl(int W, int H, const float* normal_img, const float* depth, 
     return check_launch("gsr_normal_maps", false, st);
 }
 
-int pack_frame_impl(int W, int H, const float* rgb, const float* alpha, const float* depth, const float* normal_hwc, float depth_scale,
-                    uint8_t* rgba8, uint8_t* normal8, uint8_t* depth8, cudaStream_t st) {
+int gsr_pack_frame(int32_t W, int32_t H, const float* rgb, const float* alpha, const float* depth, const float* normal_hwc,
+                   float depth_scale, uint8_t* rgba8, uint8_t* normal8, uint8_t* depth8, void* stream) {
+    NvtxRange nvtx_("gsr_pack_frame");
+    const cudaStream_t st = (cudaStream_t)stream;
     if (W <= 0 || H <= 0) { set_error("gsr_pack_frame: bad size"); return GSR_ERR_INVALID; }
     if ((rgba8 && !rgb) || (normal8 && !normal_hwc) || (depth8 && (!depth || !(depth_scale > 0.0f)))) { set_error("gsr_pack_frame: missing input for a requested output"); return GSR_ERR_INVALID; }
     if (rgba8 && ((uintptr_t)rgba8 & 3)) { set_error("gsr_pack_frame: rgba8 must be 4-byte aligned"); return GSR_ERR_INVALID; }
@@ -217,5 +231,3 @@ int pack_frame_impl(int W, int H, const float* rgb, const float* alpha, const fl
     k_pack_frame<<<(unsigned)((HW + 255) / 256), 256, 0, st>>>(W, H, rgb, alpha, depth, normal_hwc, depth_scale, (uint32_t*)rgba8, normal8, depth8);
     return check_launch("gsr_pack_frame", false, st);
 }
-
-}  // namespace gsr

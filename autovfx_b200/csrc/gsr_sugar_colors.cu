@@ -254,8 +254,14 @@ static bool sugar_color_args_ok(const char* what, int P, int M, int deg, const S
         default: KERNEL<4><<<(P + SC_THREADS - 1) / SC_THREADS, SC_THREADS, 0, st>>>(a); break;                  \
     }
 
-int sugar_colors_impl(int P, int M, int deg, const float* positions, const float* campos, const float* directions, const float* sh_dc,
-                      const float* sh_rest, const float* densities, float* out_colors, float* out_opacities, cudaStream_t st) {
+}  // namespace gsr
+
+using namespace gsr;
+
+int gsr_sugar_colors(int32_t P, int32_t M, int32_t deg, const float* positions, const float* campos, const float* directions,
+                     const float* sh_dc, const float* sh_rest, const float* densities, float* out_colors, float* out_opacities, void* stream) {
+    NvtxRange nvtx_("gsr_sugar_colors");
+    const cudaStream_t st = (cudaStream_t)stream;
     SugarColorArgs a{};
     a.P = P; a.M = M; a.positions = positions; a.campos = campos; a.directions = directions; a.sh_dc = sh_dc; a.sh_rest = sh_rest;
     a.densities = densities; a.colors = out_colors; a.opacities = out_opacities;
@@ -265,10 +271,12 @@ int sugar_colors_impl(int P, int M, int deg, const float* positions, const float
     return check_launch("gsr_sugar_colors", false, st);
 }
 
-int sugar_colors_backward_impl(int P, int M, int deg, const float* positions, const float* campos, const float* directions,
-                               const float* sh_dc, const float* sh_rest, const float* densities, const float* dL_dcolors,
-                               const float* dL_dopacities, float* dL_dsh_dc, float* dL_dsh_rest, float* dL_dpositions, float* dL_ddensities,
-                               cudaStream_t st) {
+int gsr_sugar_colors_backward(int32_t P, int32_t M, int32_t deg, const float* positions, const float* campos, const float* directions,
+                              const float* sh_dc, const float* sh_rest, const float* densities, const float* dL_dcolors,
+                              const float* dL_dopacities, float* dL_dsh_dc, float* dL_dsh_rest, float* dL_dpositions, float* dL_ddensities,
+                              void* stream) {
+    NvtxRange nvtx_("gsr_sugar_colors_backward");
+    const cudaStream_t st = (cudaStream_t)stream;
     SugarColorArgs a{};
     a.P = P; a.M = M; a.positions = positions; a.campos = campos; a.directions = directions; a.sh_dc = sh_dc; a.sh_rest = sh_rest;
     a.densities = densities; a.g_colors = dL_dcolors; a.g_opacities = dL_dopacities; a.d_sh_dc = dL_dsh_dc; a.d_sh_rest = dL_dsh_rest;
@@ -284,5 +292,3 @@ int sugar_colors_backward_impl(int P, int M, int deg, const float* positions, co
 }
 
 #undef GSR_SC_LAUNCH
-
-}  // namespace gsr

@@ -301,8 +301,6 @@ __global__ void __launch_bounds__(256) k_field_chain(int P, const float* __restr
     d_quaternions[p4] = dq[0]; d_quaternions[p4 + 1] = dq[1]; d_quaternions[p4 + 2] = dq[2]; d_quaternions[p4 + 3] = dq[3];
 }
 
-size_t sugar_field_bytes(int P) { return 64 * (size_t)(P < 0 ? 0 : P); }
-
 static int field_check(const char* who, int N, int K, int P, int R, const float* x, const int64_t* rows, const int64_t* row_idx,
                        const float* points, const float* scaling, const float* quaternions, const float* strengths, bool want_sdf,
                        void* ws, size_t ws_bytes, size_t need) {
@@ -338,42 +336,19 @@ static void launch_field_backward(const FieldIn& a, const FieldGrad& g, const Fi
 }
 static int seg_width(int K) { int w = 1; while (w < K) w <<= 1; return w; }
 
-int sugar_field_impl(int N, int K, int P, int R, const float* x, const int64_t* rows, const int64_t* row_idx, const float* points,
-                     const float* scaling, const float* quaternions, const float* strengths, float density_factor,
-                     float opacity_min_clamp, float sdf_offset, float* out_density, float* out_opac, float* out_beta, float* out_sdf,
-                     void* ws, size_t ws_bytes, cudaStream_t st) {
-    int rc = field_check("gsr_sugar_field", N, K, P, R, x, rows, row_idx, points, scaling, quaternions, strengths, out_sdf != nullptr, ws,
-                         ws_bytes, sugar_field_bytes(P));
-    if (rc != GSR_OK || N == 0) return rc;
-    if (!out_density && !out_opac && !out_beta && !out_sdf) return GSR_OK;
-    float4* rec = (float4*)ws;
-    if (P > 0) k_field_prepare<<<(P + 255) / 256, 256, 0, st>>>(P, points, scaling, quaternions, strengths, density_factor, rec);
-    const FieldIn a{N, K, P, R, x, rows, row_idx, rec, opacity_min_clamp, sdf_offset};
-    switch (seg_width(K)) {
-        case 1: launch_field<1>(a, out_density, out_opac, out_beta, out_sdf, st); break;
-        case 2: launch_field<2>(a, out_density, out_opac, out_beta, out_sdf, st); break;
-        case 4: launch_field<4>(a, out_density, out_opac, out_beta, out_sdf, st); break;
-        case 8: launch_field<8>(a, out_density, out_opac, out_beta, out_sdf, st); break;
-        case 16: launch_field<16>(a, out_density, out_opac, out_beta, out_sdf, st); break;
-        default: launch_field<32>(a, out_density, out_opac, out_beta, out_sdf, st); break;
-    }
-    return check_launch("gsr_sugar_field", false, st);
-}
-
 // det: the deterministic backward (gsr_sugar_field_backward_det); the workspace is then its scratch, laid out by FieldDetLayout.
 struct FieldDetLayout {
     size_t G, dmin, group, total;
     GroupLayout gl;
     FieldDetLayout(int N, int K, int P) : gl((size_t)(N < 0 ? 0 : N) * (size_t)(K < 0 ? 0 : K), P < 0 ? 0 : P) {
         const size_t n = N < 0 ? 0 : N;
-        size_t o = align_up(2 * sugar_field_bytes(P), 256);  // rec, grec: the default backward's workspace
+        size_t o = align_up(2 * gsr_sugar_field_bytes(P), 256);  // rec, grec: the default backward's workspace
         G = o;     o = align_up(o + 4 * n, 256);
         dmin = o;  o = align_up(o + 4 * n, 256);
         group = o;
         total = o + gl.total;
     }
 };
-size_t sugar_field_backward_det_bytes(int N, int K, int P) { return FieldDetLayout(N, K, P).total; }
 
 static int det_scratch_check(const char* who, const void* scratch) {
     if (!scratch) { set_error("%s: scratch is NULL", who); return GSR_ERR_INVALID; }
@@ -387,54 +362,6 @@ static int det_ids_check(const char* who, int N, int K, int per_sample) {
         return GSR_ERR_INVALID;
     }
     return GSR_OK;
-}
-
-int sugar_field_backward_impl(int N, int K, int P, int R, const float* x, const int64_t* rows, const int64_t* row_idx,
-                              const float* points, const float* scaling, const float* quaternions, const float* strengths,
-                              float density_factor, float opacity_min_clamp, float sdf_offset, const float* g_density, const float* g_opac,
-                              const float* g_beta, const float* g_sdf, float* dx, float* d_points, float* d_scaling, float* d_quaternions,
-                              float* d_strengths, void* ws, size_t ws_bytes, bool det, cudaStream_t st) {
-    const char* who = det ? "gsr_sugar_field_backward_det" : "gsr_sugar_field_backward";
-    if (det) {
-        int rc = det_ids_check(who, N, K, 0);
-        if (rc == GSR_OK && N > 0) rc = det_scratch_check(who, ws);
-        if (rc != GSR_OK) return rc;
-    }
-    int rc = field_check(who, N, K, P, R, x, rows, row_idx, points, scaling, quaternions, strengths, g_sdf != nullptr, ws, ws_bytes,
-                         det ? sugar_field_backward_det_bytes(N, K, P) : 2 * sugar_field_bytes(P));
-    if (rc != GSR_OK || N == 0) return rc;
-    if (P > 0 && (!d_points || !d_scaling || !d_quaternions || !d_strengths)) {
-        set_error("%s: dL_dpoints, dL_dscaling, dL_dquaternions and dL_dstrengths are required", who);
-        return GSR_ERR_INVALID;
-    }
-    float4* rec = (float4*)ws;
-    float4* grec = rec + 4 * (size_t)P;
-    if (P > 0) {
-        k_field_prepare<<<(P + 255) / 256, 256, 0, st>>>(P, points, scaling, quaternions, strengths, density_factor, rec);
-        if (!det) cudaMemsetAsync(grec, 0, sugar_field_bytes(P), st);
-    }
-    const FieldIn a{N, K, P, R, x, rows, row_idx, rec, opacity_min_clamp, sdf_offset};
-    const FieldGrad g{g_density, g_opac, g_beta, g_sdf, dx, grec};
-    const FieldDetLayout L(N, K, P);
-    char* w = (char*)ws;
-    const FieldDet fd{(float*)(w + L.G), (float*)(w + L.dmin), (uint32_t*)(w + L.group + L.gl.keys0), (uint32_t*)(w + L.group + L.gl.vals0)};
-    const FieldDet* dp = det ? &fd : nullptr;
-    switch (seg_width(K)) {
-        case 1: launch_field_backward<1>(a, g, dp, st); break;
-        case 2: launch_field_backward<2>(a, g, dp, st); break;
-        case 4: launch_field_backward<4>(a, g, dp, st); break;
-        case 8: launch_field_backward<8>(a, g, dp, st); break;
-        case 16: launch_field_backward<16>(a, g, dp, st); break;
-        default: launch_field_backward<32>(a, g, dp, st); break;
-    }
-    if (det && P > 0) {
-        const uint32_t* ids = group_ids((size_t)N * K, P, w + L.group, L.gl, st);
-        k_field_reduce<<<(P + 255) / 256, 256, 0, st>>>(a, g, fd.G, fd.dmin, ids, (const uint32_t*)(w + L.group + L.gl.seg));
-    }
-    if (P > 0)
-        k_field_chain<<<(P + 255) / 256, 256, 0, st>>>(P, scaling, quaternions, density_factor, grec, d_points, d_scaling, d_quaternions,
-                                                        d_strengths);
-    return check_launch(who, false, st);
 }
 
 // ================================================================================================================================
@@ -701,8 +628,6 @@ __global__ void __launch_bounds__(256) k_normal_chain(int P, const float* __rest
     d_quaternions[p4] = dq[0]; d_quaternions[p4 + 1] = dq[1]; d_quaternions[p4 + 2] = dq[2]; d_quaternions[p4 + 3] = dq[3];
 }
 
-size_t sugar_sdf_normal_bytes(int P) { return 32 * (size_t)(P < 0 ? 0 : P); }
-
 static int normal_check(const char* who, int N, int K, int P, const float* x, const int64_t* gidx, const int64_t* knn,
                         const float* points, const float* scaling, const float* quaternions, const float* opac, bool want_loss,
                         void* ws, size_t ws_bytes, size_t need) {
@@ -739,11 +664,135 @@ static void launch_normal_backward(const NormalIn& a, const NormalGrad& g, const
     else k_normal_backward<W, false><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(a, g, NormalDet{});
 }
 
-int sugar_sdf_normal_impl(int N, int K, int P, const float* x, const int64_t* gidx, const int64_t* knn, const float* points,
-                          const float* scaling, const float* quaternions, const float* opac, float* out_loss, float* out_est, void* ws,
-                          size_t ws_bytes, cudaStream_t st) {
+// det: the deterministic backward (gsr_sugar_sdf_normal_backward_det); the workspace is then its scratch, laid out by NormalDetLayout
+// for KS = K neighbour slots per sample with the loss, 0 without.
+struct NormalDetLayout {
+    size_t sc, own, group, total;
+    GroupLayout gl;
+    NormalDetLayout(int N, int KS, int P) : gl((size_t)(N < 0 ? 0 : N) * (size_t)(KS < 0 ? 1 : KS + 1), P < 0 ? 0 : P) {
+        const size_t n = N < 0 ? 0 : N;
+        size_t o = align_up(2 * gsr_sugar_sdf_normal_bytes(P), 256);  // rec, grec: the default backward's workspace
+        sc = o;   o = align_up(o + 16 * n, 256);
+        own = o;  o = align_up(o + 32 * n, 256);
+        group = o;
+        total = o + gl.total;
+    }
+};
+
+}  // namespace gsr
+
+using namespace gsr;
+
+size_t gsr_sugar_field_bytes(int32_t P) { return 64 * (size_t)(P < 0 ? 0 : P); }
+
+int gsr_sugar_field(int32_t N, int32_t K, int32_t P, int32_t R, const float* x, const int64_t* rows, const int64_t* row_idx,
+                    const float* points, const float* scaling, const float* quaternions, const float* strengths, float density_factor,
+                    float opacity_min_clamp, float sdf_offset, float* out_density, float* out_opac, float* out_beta, float* out_sdf,
+                    void* ws, size_t ws_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_sugar_field");
+    const cudaStream_t st = (cudaStream_t)stream;
+    int rc = field_check("gsr_sugar_field", N, K, P, R, x, rows, row_idx, points, scaling, quaternions, strengths, out_sdf != nullptr, ws,
+                         ws_bytes, gsr_sugar_field_bytes(P));
+    if (rc != GSR_OK || N == 0) return rc;
+    if (!out_density && !out_opac && !out_beta && !out_sdf) return GSR_OK;
+    float4* rec = (float4*)ws;
+    if (P > 0) k_field_prepare<<<(P + 255) / 256, 256, 0, st>>>(P, points, scaling, quaternions, strengths, density_factor, rec);
+    const FieldIn a{N, K, P, R, x, rows, row_idx, rec, opacity_min_clamp, sdf_offset};
+    switch (seg_width(K)) {
+        case 1: launch_field<1>(a, out_density, out_opac, out_beta, out_sdf, st); break;
+        case 2: launch_field<2>(a, out_density, out_opac, out_beta, out_sdf, st); break;
+        case 4: launch_field<4>(a, out_density, out_opac, out_beta, out_sdf, st); break;
+        case 8: launch_field<8>(a, out_density, out_opac, out_beta, out_sdf, st); break;
+        case 16: launch_field<16>(a, out_density, out_opac, out_beta, out_sdf, st); break;
+        default: launch_field<32>(a, out_density, out_opac, out_beta, out_sdf, st); break;
+    }
+    return check_launch("gsr_sugar_field", false, st);
+}
+
+size_t gsr_sugar_field_backward_det_bytes(int32_t N, int32_t K, int32_t P) { return FieldDetLayout(N, K, P).total; }
+
+static int sugar_field_backward_impl(int N, int K, int P, int R, const float* x, const int64_t* rows, const int64_t* row_idx,
+                                     const float* points, const float* scaling, const float* quaternions, const float* strengths,
+                                     float density_factor, float opacity_min_clamp, float sdf_offset, const float* g_density,
+                                     const float* g_opac, const float* g_beta, const float* g_sdf, float* dx, float* d_points,
+                                     float* d_scaling, float* d_quaternions, float* d_strengths, void* ws, size_t ws_bytes, bool det,
+                                     cudaStream_t st) {
+    const char* who = det ? "gsr_sugar_field_backward_det" : "gsr_sugar_field_backward";
+    if (det) {
+        int rc = det_ids_check(who, N, K, 0);
+        if (rc == GSR_OK && N > 0) rc = det_scratch_check(who, ws);
+        if (rc != GSR_OK) return rc;
+    }
+    int rc = field_check(who, N, K, P, R, x, rows, row_idx, points, scaling, quaternions, strengths, g_sdf != nullptr, ws, ws_bytes,
+                         det ? gsr_sugar_field_backward_det_bytes(N, K, P) : 2 * gsr_sugar_field_bytes(P));
+    if (rc != GSR_OK || N == 0) return rc;
+    if (P > 0 && (!d_points || !d_scaling || !d_quaternions || !d_strengths)) {
+        set_error("%s: dL_dpoints, dL_dscaling, dL_dquaternions and dL_dstrengths are required", who);
+        return GSR_ERR_INVALID;
+    }
+    float4* rec = (float4*)ws;
+    float4* grec = rec + 4 * (size_t)P;
+    if (P > 0) {
+        k_field_prepare<<<(P + 255) / 256, 256, 0, st>>>(P, points, scaling, quaternions, strengths, density_factor, rec);
+        if (!det) cudaMemsetAsync(grec, 0, gsr_sugar_field_bytes(P), st);
+    }
+    const FieldIn a{N, K, P, R, x, rows, row_idx, rec, opacity_min_clamp, sdf_offset};
+    const FieldGrad g{g_density, g_opac, g_beta, g_sdf, dx, grec};
+    const FieldDetLayout L(N, K, P);
+    char* w = (char*)ws;
+    const FieldDet fd{(float*)(w + L.G), (float*)(w + L.dmin), (uint32_t*)(w + L.group + L.gl.keys0), (uint32_t*)(w + L.group + L.gl.vals0)};
+    const FieldDet* dp = det ? &fd : nullptr;
+    switch (seg_width(K)) {
+        case 1: launch_field_backward<1>(a, g, dp, st); break;
+        case 2: launch_field_backward<2>(a, g, dp, st); break;
+        case 4: launch_field_backward<4>(a, g, dp, st); break;
+        case 8: launch_field_backward<8>(a, g, dp, st); break;
+        case 16: launch_field_backward<16>(a, g, dp, st); break;
+        default: launch_field_backward<32>(a, g, dp, st); break;
+    }
+    if (det && P > 0) {
+        const uint32_t* ids = group_ids((size_t)N * K, P, w + L.group, L.gl, st);
+        k_field_reduce<<<(P + 255) / 256, 256, 0, st>>>(a, g, fd.G, fd.dmin, ids, (const uint32_t*)(w + L.group + L.gl.seg));
+    }
+    if (P > 0)
+        k_field_chain<<<(P + 255) / 256, 256, 0, st>>>(P, scaling, quaternions, density_factor, grec, d_points, d_scaling, d_quaternions,
+                                                        d_strengths);
+    return check_launch(who, false, st);
+}
+
+int gsr_sugar_field_backward(int32_t N, int32_t K, int32_t P, int32_t R, const float* x, const int64_t* rows, const int64_t* row_idx,
+                             const float* points, const float* scaling, const float* quaternions, const float* strengths,
+                             float density_factor, float opacity_min_clamp, float sdf_offset, const float* dL_ddensity,
+                             const float* dL_dopacities, const float* dL_dbeta, const float* dL_dsdf, float* dL_dx, float* dL_dpoints,
+                             float* dL_dscaling, float* dL_dquaternions, float* dL_dstrengths, void* workspace, size_t workspace_bytes,
+                             void* stream) {
+    NvtxRange nvtx_("gsr_sugar_field_backward");
+    return sugar_field_backward_impl(N, K, P, R, x, rows, row_idx, points, scaling, quaternions, strengths, density_factor,
+                                     opacity_min_clamp, sdf_offset, dL_ddensity, dL_dopacities, dL_dbeta, dL_dsdf, dL_dx, dL_dpoints,
+                                     dL_dscaling, dL_dquaternions, dL_dstrengths, workspace, workspace_bytes, false, (cudaStream_t)stream);
+}
+
+int gsr_sugar_field_backward_det(int32_t N, int32_t K, int32_t P, int32_t R, const float* x, const int64_t* rows, const int64_t* row_idx,
+                                 const float* points, const float* scaling, const float* quaternions, const float* strengths,
+                                 float density_factor, float opacity_min_clamp, float sdf_offset, const float* dL_ddensity,
+                                 const float* dL_dopacities, const float* dL_dbeta, const float* dL_dsdf, float* dL_dx, float* dL_dpoints,
+                                 float* dL_dscaling, float* dL_dquaternions, float* dL_dstrengths, void* scratch, size_t scratch_bytes,
+                                 void* stream) {
+    NvtxRange nvtx_("gsr_sugar_field_backward_det");
+    return sugar_field_backward_impl(N, K, P, R, x, rows, row_idx, points, scaling, quaternions, strengths, density_factor,
+                                     opacity_min_clamp, sdf_offset, dL_ddensity, dL_dopacities, dL_dbeta, dL_dsdf, dL_dx, dL_dpoints,
+                                     dL_dscaling, dL_dquaternions, dL_dstrengths, scratch, scratch_bytes, true, (cudaStream_t)stream);
+}
+
+size_t gsr_sugar_sdf_normal_bytes(int32_t P) { return 32 * (size_t)(P < 0 ? 0 : P); }
+
+int gsr_sugar_sdf_normal(int32_t N, int32_t K, int32_t P, const float* x, const int64_t* gidx, const int64_t* knn,
+                         const float* points, const float* scaling, const float* quaternions, const float* opac, float* out_loss,
+                         float* out_est, void* ws, size_t ws_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_sugar_sdf_normal");
+    const cudaStream_t st = (cudaStream_t)stream;
     int rc = normal_check("gsr_sugar_sdf_normal", N, K, P, x, gidx, knn, points, scaling, quaternions, opac, out_loss != nullptr, ws,
-                          ws_bytes, sugar_sdf_normal_bytes(P));
+                          ws_bytes, gsr_sugar_sdf_normal_bytes(P));
     if (rc != GSR_OK || N == 0) return rc;
     if (!out_loss && !out_est) return GSR_OK;
     float4* rec = (float4*)ws;
@@ -760,26 +809,14 @@ int sugar_sdf_normal_impl(int N, int K, int P, const float* x, const int64_t* gi
     return check_launch("gsr_sugar_sdf_normal", false, st);
 }
 
-// det: the deterministic backward (gsr_sugar_sdf_normal_backward_det); the workspace is then its scratch, laid out by NormalDetLayout
-// for KS = K neighbour slots per sample with the loss, 0 without.
-struct NormalDetLayout {
-    size_t sc, own, group, total;
-    GroupLayout gl;
-    NormalDetLayout(int N, int KS, int P) : gl((size_t)(N < 0 ? 0 : N) * (size_t)(KS < 0 ? 1 : KS + 1), P < 0 ? 0 : P) {
-        const size_t n = N < 0 ? 0 : N;
-        size_t o = align_up(2 * sugar_sdf_normal_bytes(P), 256);  // rec, grec: the default backward's workspace
-        sc = o;   o = align_up(o + 16 * n, 256);
-        own = o;  o = align_up(o + 32 * n, 256);
-        group = o;
-        total = o + gl.total;
-    }
-};
-size_t sugar_sdf_normal_backward_det_bytes(int N, int K, int P, bool with_loss) { return NormalDetLayout(N, with_loss ? K : 0, P).total; }
+size_t gsr_sugar_sdf_normal_backward_det_bytes(int32_t N, int32_t K, int32_t P, int with_loss) {
+    return NormalDetLayout(N, with_loss ? K : 0, P).total;
+}
 
-int sugar_sdf_normal_backward_impl(int N, int K, int P, const float* x, const int64_t* gidx, const int64_t* knn, const float* points,
-                                   const float* scaling, const float* quaternions, const float* opac, const float* g_loss,
-                                   const float* g_est, float* dx, float* d_points, float* d_quaternions, void* ws, size_t ws_bytes,
-                                   bool det, cudaStream_t st) {
+static int sugar_sdf_normal_backward_impl(int N, int K, int P, const float* x, const int64_t* gidx, const int64_t* knn,
+                                          const float* points, const float* scaling, const float* quaternions, const float* opac,
+                                          const float* g_loss, const float* g_est, float* dx, float* d_points, float* d_quaternions,
+                                          void* ws, size_t ws_bytes, bool det, cudaStream_t st) {
     const char* who = det ? "gsr_sugar_sdf_normal_backward_det" : "gsr_sugar_sdf_normal_backward";
     if (det) {
         int rc = g_loss ? det_ids_check(who, N, K, 1) : GSR_OK;
@@ -787,7 +824,7 @@ int sugar_sdf_normal_backward_impl(int N, int K, int P, const float* x, const in
         if (rc != GSR_OK) return rc;
     }
     int rc = normal_check(who, N, K, P, x, gidx, knn, points, scaling, quaternions, opac, g_loss != nullptr, ws, ws_bytes,
-                          det ? sugar_sdf_normal_backward_det_bytes(N, K, P, g_loss != nullptr) : 2 * sugar_sdf_normal_bytes(P));
+                          det ? gsr_sugar_sdf_normal_backward_det_bytes(N, K, P, g_loss != nullptr) : 2 * gsr_sugar_sdf_normal_bytes(P));
     if (rc != GSR_OK || N == 0) return rc;
     if (P > 0 && (!d_points || !d_quaternions)) {
         set_error("%s: dL_dpoints and dL_dquaternions are required", who);
@@ -797,7 +834,7 @@ int sugar_sdf_normal_backward_impl(int N, int K, int P, const float* x, const in
     float4* grec = rec + 2 * (size_t)P;
     if (P > 0) {
         k_normal_prepare<<<(P + 255) / 256, 256, 0, st>>>(P, points, scaling, quaternions, rec);
-        if (!det) cudaMemsetAsync(grec, 0, sugar_sdf_normal_bytes(P), st);
+        if (!det) cudaMemsetAsync(grec, 0, gsr_sugar_sdf_normal_bytes(P), st);
     }
     const NormalIn a{N, K, P, x, gidx, knn, opac, rec};
     const NormalGrad g{g_loss, g_est, dx, grec};
@@ -823,4 +860,20 @@ int sugar_sdf_normal_backward_impl(int N, int K, int P, const float* x, const in
     return check_launch(who, false, st);
 }
 
-}  // namespace gsr
+int gsr_sugar_sdf_normal_backward(int32_t N, int32_t K, int32_t P, const float* x, const int64_t* gidx, const int64_t* knn_idx,
+                                  const float* points, const float* scaling, const float* quaternions, const float* opacities,
+                                  const float* dL_dloss, const float* dL_destimate, float* dL_dx, float* dL_dpoints,
+                                  float* dL_dquaternions, void* workspace, size_t workspace_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_sugar_sdf_normal_backward");
+    return sugar_sdf_normal_backward_impl(N, K, P, x, gidx, knn_idx, points, scaling, quaternions, opacities, dL_dloss, dL_destimate,
+                                          dL_dx, dL_dpoints, dL_dquaternions, workspace, workspace_bytes, false, (cudaStream_t)stream);
+}
+
+int gsr_sugar_sdf_normal_backward_det(int32_t N, int32_t K, int32_t P, const float* x, const int64_t* gidx, const int64_t* knn_idx,
+                                      const float* points, const float* scaling, const float* quaternions, const float* opacities,
+                                      const float* dL_dloss, const float* dL_destimate, float* dL_dx, float* dL_dpoints,
+                                      float* dL_dquaternions, void* scratch, size_t scratch_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_sugar_sdf_normal_backward_det");
+    return sugar_sdf_normal_backward_impl(N, K, P, x, gidx, knn_idx, points, scaling, quaternions, opacities, dL_dloss, dL_destimate,
+                                          dL_dx, dL_dpoints, dL_dquaternions, scratch, scratch_bytes, true, (cudaStream_t)stream);
+}

@@ -240,15 +240,20 @@ __global__ void __launch_bounds__(256) k_sample_reduce(SampleGradArgs a, const u
 inline int nblocks_prefix(int P) { return (P + PREFIX_BLOCK - 1) / PREFIX_BLOCK; }
 
 }  // namespace
+}  // namespace gsr
 
-size_t sugar_sample_bytes(int P) {
+using namespace gsr;
+
+size_t gsr_sugar_sample_bytes(int32_t P) {
     if (P < 1) return 16;
     return align_up(8 * (size_t)P, 16) + 2 * align_up(8 * (size_t)nblocks_prefix(P), 16);
 }
 
-int sugar_sample_impl(int N, int P, float f, int volume, const uint8_t* mask, const float* strengths, const double* u, const float* z,
-                      const float* points, const float* scaling, const float* quaternions, float* out_points, int64_t* out_idx,
-                      double* out_total, void* ws, size_t ws_bytes, cudaStream_t st) {
+int gsr_sugar_sample(int32_t N, int32_t P, float f, int32_t volume, const uint8_t* mask, const float* strengths, const double* u,
+                     const float* z, const float* points, const float* scaling, const float* quaternions, float* out_points,
+                     int64_t* out_idx, double* out_total, void* ws, size_t ws_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_sugar_sample");
+    const cudaStream_t st = (cudaStream_t)stream;
     if (N < 0 || P < 1) {
         set_error("gsr_sugar_sample: N = %d and P = %d (need N >= 0, P >= 1)", N, P);
         return GSR_ERR_INVALID;
@@ -258,8 +263,8 @@ int sugar_sample_impl(int N, int P, float f, int volume, const uint8_t* mask, co
         set_error("gsr_sugar_sample: missing input or output (only mask and strengths may be NULL)");
         return GSR_ERR_INVALID;
     }
-    if (ws_bytes < sugar_sample_bytes(P) || !ws || ((uintptr_t)ws & 15)) {
-        set_error("gsr_sugar_sample: workspace of %zu bytes (need %zu, 16-byte aligned)", ws_bytes, sugar_sample_bytes(P));
+    if (ws_bytes < gsr_sugar_sample_bytes(P) || !ws || ((uintptr_t)ws & 15)) {
+        set_error("gsr_sugar_sample: workspace of %zu bytes (need %zu, 16-byte aligned)", ws_bytes, gsr_sugar_sample_bytes(P));
         return GSR_ERR_WORKSPACE;
     }
     const int nb = nblocks_prefix(P);
@@ -278,12 +283,13 @@ int sugar_sample_impl(int N, int P, float f, int volume, const uint8_t* mask, co
     return check_launch("gsr_sugar_sample", false, st);
 }
 
-size_t sugar_sample_backward_det_bytes(int N, int P) { return GroupLayout((size_t)(N < 0 ? 0 : N), P < 0 ? 0 : P).total; }
+size_t gsr_sugar_sample_backward_det_bytes(int32_t N, int32_t P) { return GroupLayout((size_t)(N < 0 ? 0 : N), P < 0 ? 0 : P).total; }
 
 // det: the deterministic backward (gsr_sugar_sample_backward_det) with `scratch` of scratch_bytes; otherwise scratch is unused.
-int sugar_sample_backward_impl(int N, int P, float f, const int64_t* idx, const float* z, const float* scaling, const float* quaternions,
-                               const double* total, const float* dL_dsamples, float* d_points, float* d_scaling, float* d_quaternions,
-                               bool det, void* scratch, size_t scratch_bytes, cudaStream_t st) {
+static int sugar_sample_backward_impl(int N, int P, float f, const int64_t* idx, const float* z, const float* scaling,
+                                      const float* quaternions, const double* total, const float* dL_dsamples, float* d_points,
+                                      float* d_scaling, float* d_quaternions, bool det, void* scratch, size_t scratch_bytes,
+                                      cudaStream_t st) {
     const char* who = det ? "gsr_sugar_sample_backward_det" : "gsr_sugar_sample_backward";
     if (N < 0 || P < 1) {
         set_error("%s: N = %d and P = %d (need N >= 0, P >= 1)", who, N, P);
@@ -315,4 +321,19 @@ int sugar_sample_backward_impl(int N, int P, float f, const int64_t* idx, const 
     return check_launch(who, false, st);
 }
 
-}  // namespace gsr
+int gsr_sugar_sample_backward(int32_t N, int32_t P, float sampling_scale_factor, const int64_t* idx, const float* z, const float* scaling,
+                              const float* quaternions, const double* total, const float* dL_dsamples, float* dL_dpoints,
+                              float* dL_dscaling, float* dL_dquaternions, void* stream) {
+    NvtxRange nvtx_("gsr_sugar_sample_backward");
+    return sugar_sample_backward_impl(N, P, sampling_scale_factor, idx, z, scaling, quaternions, total, dL_dsamples, dL_dpoints,
+                                      dL_dscaling, dL_dquaternions, false, nullptr, 0, (cudaStream_t)stream);
+}
+
+int gsr_sugar_sample_backward_det(int32_t N, int32_t P, float sampling_scale_factor, const int64_t* idx, const float* z,
+                                  const float* scaling, const float* quaternions, const double* total, const float* dL_dsamples,
+                                  float* dL_dpoints, float* dL_dscaling, float* dL_dquaternions, void* scratch, size_t scratch_bytes,
+                                  void* stream) {
+    NvtxRange nvtx_("gsr_sugar_sample_backward_det");
+    return sugar_sample_backward_impl(N, P, sampling_scale_factor, idx, z, scaling, quaternions, total, dL_dsamples, dL_dpoints,
+                                      dL_dscaling, dL_dquaternions, true, scratch, scratch_bytes, (cudaStream_t)stream);
+}
