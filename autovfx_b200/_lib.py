@@ -141,6 +141,10 @@ SIGNATURES = {
     "gsr_anisotropic_loss_backward": (_int, [_i64, _ptr, _f32] + [_ptr] * 3),
     "gsr_percentile_low": (_int, [_i64] + [_ptr] * 3 + [_size, _ptr]),
     "gsr_composite": (_int, [_i32] * 2 + [_ptr] * 14),
+    "gsr_select_rows_bytes": (_size, [_i64]),
+    "gsr_select_rows": (_int, [_i64] + [_ptr] * 11 + [_size, _ptr]),
+    "gsr_pack_masks": (_int, [_i32] * 3 + [_ptr] * 3),
+    "gsr_mask_disagreement": (_int, [_i32] * 2 + [_ptr] * 2 + [_f32, _ptr, _ptr]),
     "gsr_get_views": (_int, [_ws, _i32, _i32, _i32, C.POINTER(gsr_views)]),
     "gsr_profile_begin": (_int, [_int]),
     "gsr_profile_begin_strided": (_int, [_int, _int]),

@@ -487,31 +487,35 @@ class PreparedForward:
     an event (a few microseconds of host time instead of the ~0.3 ms of argument checking in ``forward_raw``).  Used by
     ``render_loop.FrameLoop``; forward-only (no buffers are kept for a backward pass).
 
-    ``cam`` is a contiguous float32 device tensor holding view(16) | proj(16) | campos(3) at its start."""
+    ``cam`` is a contiguous float32 device tensor holding view(16) | proj(16) | campos(3) at its start.  ``shs`` may be None when
+    ``colors_precomp`` [P,3] is given instead."""
 
     def __init__(self, means3D, shs, opacities, scales, rotations, cam: torch.Tensor, W: int, H: int, bg: torch.Tensor, sh_degree: int,
                  scale_modifier: float, out, extra: Optional[torch.Tensor] = None, extra_out: Optional[torch.Tensor] = None,
-                 tight: Optional[bool] = None, exact: Optional[bool] = None):
+                 tight: Optional[bool] = None, exact: Optional[bool] = None, colors_precomp: Optional[torch.Tensor] = None):
         device = means3D.device
         self.device, self.st = device, _state(device)
         self.P, self.W, self.H = int(means3D.shape[0]), int(W), int(H)
-        chk = [means3D, shs, opacities, scales, rotations, cam, bg] + list(out) + ([extra, extra_out] if extra is not None else [])
+        if (shs is None) == (colors_precomp is None):
+            raise ValueError("PreparedForward: provide exactly one of shs / colors_precomp")
+        colors = shs if shs is not None else colors_precomp
+        chk = [means3D, colors, opacities, scales, rotations, cam, bg] + list(out) + ([extra, extra_out] if extra is not None else [])
         for t in chk:
             if not (t.is_cuda and t.device == device and t.is_contiguous()):
                 raise ValueError("PreparedForward: tensors must be contiguous and live on %s" % device)
-        for t in (means3D, shs, opacities, scales, rotations, cam, bg):
+        for t in (means3D, colors, opacities, scales, rotations, cam, bg):
             if t.dtype != torch.float32:
                 raise ValueError("PreparedForward: float32 tensors required")
         if (extra is None) != (extra_out is None):
             raise ValueError("extra and extra_out go together")
-        self.keep = (means3D, shs, opacities, scales, rotations, cam, bg, out, extra, extra_out)
+        self.keep = (means3D, colors, opacities, scales, rotations, cam, bg, out, extra, extra_out)
         color, depth, alpha, radii = out
         self.fr = _lib.gsr_frame()
         fr = self.fr
-        fr.P, fr.D, fr.M, fr.W, fr.H = self.P, int(sh_degree), int(shs.shape[1]), self.W, self.H
+        fr.P, fr.D, fr.M, fr.W, fr.H = self.P, int(sh_degree), int(shs.shape[1]) if shs is not None else 0, self.W, self.H
         fr.scale_modifier = float(scale_modifier)
         fr.prefiltered, fr.debug = 0, 0
-        fr.bg, fr.means3D, fr.shs, fr.colors_precomp = bg.data_ptr(), _ptr(means3D), _ptr(shs), None
+        fr.bg, fr.means3D, fr.shs, fr.colors_precomp = bg.data_ptr(), _ptr(means3D), _ptr(shs), _ptr(colors_precomp)
         fr.opacities, fr.scales, fr.rotations, fr.cov3D_precomp = _ptr(opacities), _ptr(scales), _ptr(rotations), None
         base = cam.data_ptr()
         fr.viewmatrix, fr.projmatrix, fr.campos = base, base + 64, base + 128
@@ -540,8 +544,13 @@ class PreparedForward:
         self._counters = image[:32].view(torch.int32)
         self._capacity_instances = _L.gsr_binning_capacity_slab(binning.numel(), self.W, self.H, S)
 
-    def launch(self, tanfovx: float, tanfovy: float) -> FrameTicket:
-        """Issue the frame on the current stream; never synchronises.  Validate the returned ticket before trusting the images."""
+    def launch(self, tanfovx: float, tanfovy: float, P: Optional[int] = None) -> FrameTicket:
+        """Issue the frame on the current stream; never synchronises.  Validate the returned ticket before trusting the images.
+        ``P``: render only the first P rows of the bound tensors (0 <= P <= the rows they were bound with)."""
+        P = self.P if P is None else int(P)
+        if not 0 <= P <= self.P:
+            raise ValueError("PreparedForward.launch: P = %d outside 0..%d" % (P, self.P))
+        self.fr.P = P
         with torch.cuda.device(self.device):
             return self._launch(tanfovx, tanfovy)
 
@@ -557,7 +566,7 @@ class PreparedForward:
         st.geom_cache.pop(stream.cuda_stream, None)  # the shared workspaces are about to hold this frame
         fr = self.fr
         fr.tanfovx, fr.tanfovy = tanfovx, tanfovy
-        if self.extra_out is not None and self.P == 0:
+        if self.extra_out is not None and fr.P == 0:
             self.extra_out.zero_()
         rc = _L.gsr_forward_multi(C.byref(fr), C.byref(self.ws), self.out_ptrs[0], self.out_ptrs[1], self.out_ptrs[2], self.out_ptrs[3],
                                   self.extra_ptrs[0], self.extra_ptrs[1], self.flags, C.c_void_p(stream.cuda_stream))

@@ -27,6 +27,8 @@
  *   gsr_anisotropic_loss replaces anisotropic_loss                                GS/utils/loss_utils.py:159-168; gsr_anisotropic_loss_backward
  *   gsr_percentile_low replaces np.percentile(smoke_depth, 0.001)                blender/blend_all.py:206-208
  *   gsr_composite     replaces  the per-frame compositing of blend_frames          blender/blend_all.py:236-342
+ *   gsr_select_rows   replaces  the deepcopy + boolean indexing of each candidate subset  extract/extract_object.py:196-202, :315-321
+ *   gsr_pack_masks, gsr_mask_disagreement replace the host readback and numpy XOR count of each tracked view  :215-221, :334-340
  *
  * and, for the render() wrapper around the two rasterizer passes ("GR/" = sugar/gaussian_splatting/gaussian_renderer/__init__.py):
  *
@@ -608,6 +610,22 @@ int gsr_percentile_low(int64_t n, const float* x, float* out, void* workspace, s
 int gsr_composite(int32_t W, int32_t H, const uint8_t* frame, const uint8_t* obj, const float* obj_depth, const uint8_t* shadow,
                   const float* shadow_depth, const uint8_t* all, const uint8_t* obj3dgs, const float* obj3dgs_depth, const uint8_t* smoke,
                   const float* smoke_depth, const float* smoke_pct, const uint8_t* fire, uint8_t* out, void* stream);
+
+/* Candidate-subset scoring of extract_object (gsr_extract.cu).  Nothing here synchronises with the host. */
+/* Bytes of gsr_select_rows' workspace for P rows (0 when P is out of range). */
+size_t gsr_select_rows_bytes(int64_t P);
+/* t_out[:n] = t[keep] for means3D [P,3], opacities [P,1], scales [P,3] and rotations [P,4], with *count = n (device int32): the kept
+ * rows in their original order, bit for bit (sort ties resolve by Gaussian index, so the order decides the image).  keep is a
+ * bool [P] (one byte per row, nonzero = kept); the outputs hold P rows.  0 <= P < 2^31, else GSR_ERR_INVALID. */
+int gsr_select_rows(int64_t P, const uint8_t* keep, const float* means3D, const float* opacities, const float* scales, const float* rotations,
+                    float* means3D_out, float* opacities_out, float* scales_out, float* rotations_out, int32_t* count, void* workspace,
+                    size_t workspace_bytes, void* stream);
+/* bits [V,H,ceil(W/32)] uint32 from masks [V,H,W] uint8: bit x % 32 of word (v, y, x / 32) is masks[v,y,x] == 255; bits past W are 0. */
+int gsr_pack_masks(int32_t V, int32_t W, int32_t H, const uint8_t* masks, uint32_t* bits, void* stream);
+/* *count += the pixels of one [H,W] frame where (alpha >= thr) differs from the packed mask bit (bits [H,ceil(W/32)] of
+ * gsr_pack_masks).  The comparison is float32, and false for a NaN alpha, as numpy's `alpha >= np.float32(thr)` is.  count is an
+ * 8-byte aligned device int64; the sum is exact and the same on every run. */
+int gsr_mask_disagreement(int32_t W, int32_t H, const float* alpha, const uint32_t* bits, float thr, int64_t* count, void* stream);
 
 /* Device pointers into the workspaces of the last layout (P, capacity, W, H) — for parity tests that
  * compare per-stage buffers with the reference (SURVEY §4).  Pure pointer arithmetic, no CUDA calls. */
