@@ -83,6 +83,8 @@ _int, _i32, _i64, _f32, _size, _ptr = C.c_int, C.c_int32, C.c_int64, C.c_float, 
 _frame, _ws, _grads = C.POINTER(gsr_frame), C.POINTER(gsr_workspace), C.POINTER(gsr_grads)
 _FIELD_BWD = [_i32] * 4 + [_ptr] * 7 + [_f32] * 3 + [_ptr] * 10 + [_size, _ptr]
 _SDF_NORMAL_BWD = [_i32] * 3 + [_ptr] * 13 + [_size, _ptr]
+_DEPTH_MAP = [_i32] * 3 + [_i64] * 2 + [_ptr, _f32, _f32, _ptr]  # N or P, H, W, the depth view, sx, sy, camera
+_DEPTH_LOSS_BWD = _DEPTH_MAP + [_ptr] * 2 + [_f32] * 2 + [_ptr] * 5
 
 # every export of include/gsr_b200.h: name -> (restype, argtypes)
 SIGNATURES = {
@@ -127,6 +129,12 @@ SIGNATURES = {
     "gsr_sugar_sample_backward": (_int, [_i32, _i32, _f32] + [_ptr] * 10),
     "gsr_sugar_sample_backward_det_bytes": (_size, [_i32] * 2),
     "gsr_sugar_sample_backward_det": (_int, [_i32, _i32, _f32] + [_ptr] * 10 + [_size, _ptr]),
+    "gsr_sugar_surface_mask": (_int, _DEPTH_MAP + [_ptr] * 3 + [_f32] + [_ptr] * 3),
+    "gsr_sugar_depth_sdf_loss_bytes": (_size, [_i32]),
+    "gsr_sugar_depth_sdf_loss": (_int, _DEPTH_MAP + [_ptr] * 2 + [_f32] * 2 + [_ptr] * 3 + [_size, _ptr]),
+    "gsr_sugar_depth_sdf_loss_backward": (_int, _DEPTH_LOSS_BWD + [_ptr]),
+    "gsr_sugar_depth_sdf_loss_backward_det_bytes": (_size, [_i32] * 3),
+    "gsr_sugar_depth_sdf_loss_backward_det": (_int, _DEPTH_LOSS_BWD + [_ptr, _size, _ptr]),
     "gsr_densify_stats": (_int, [_i32] * 2 + [_ptr] * 7),
     "gsr_densify_plan_bytes": (_size, [_i32]),
     "gsr_densify_plan": (_int, [_i32] + [_ptr] * 4 + [_f32] * 3 + [_i32] + [_f32] * 2 + [_ptr] * 3 + [_size, _ptr]),

@@ -20,6 +20,14 @@ SuGaR's sampler of the SDF-regularisation points (SS/:757-799) runs through ``gs
     from autovfx_b200.sugar_field import sample_points_in_gaussians
     SuGaR.sample_points_in_gaussians = sample_points_in_gaussians
 
+coarse_sdf's depth-map estimate ("CS/" = sugar/sugar_trainers/coarse_sdf.py: the close-to-surface mask :655-665 and the 'sdf'
+estimation loss :689-712) runs through ``gsr_sugar_surface_mask`` and ``gsr_sugar_depth_sdf_loss`` / ``..._backward``::
+
+    from autovfx_b200.sugar_field import close_to_surface_mask, depth_sdf_estimation_loss
+    gaussians_close_to_surface = close_to_surface_mask(sugar, fov_camera, depth, close_gaussian_threshold)
+    loss = loss + sdf_estimation_factor * depth_sdf_estimation_loss(sugar, fov_camera, depth, sdf_samples, fields['sdf'],
+                                                                    sdf_sample_std, 10. * sugar.get_cameras_spatial_extent())
+
 The model is read through its getters (``points``, ``scaling``, ``quaternions``, ``strengths``, ``knn_idx``, ``beta_mode``), so
 autograd carries the gradients of x and of the getters' outputs back to the raw parameters.  No [N,K,3,3] tensor is built: the
 kernels gather one 64-byte record per (sample, neighbour) pair and recompute everything in the backward.
@@ -32,7 +40,7 @@ import torch
 from . import _lib
 
 __all__ = ["get_field_values", "compute_density", "projection_estimate", "better_normal_loss", "sample_points_in_gaussians",
-           "FIELD_MAX_K"]
+           "close_to_surface_mask", "depth_sdf_estimation_loss", "FIELD_MAX_K"]
 
 FIELD_MAX_K = 32
 
@@ -452,3 +460,171 @@ def sample_points_in_gaussians(self, num_samples, sampling_scale_factor=1., mask
             return _SugarSample.apply(*ins, N, f, bool(probabilities_proportional_to_volume), mask, strengths, u, z)
         out, idx, _ = _sample_forward(N, f, probabilities_proportional_to_volume, mask, strengths, u, z, *ins)
         return out, idx
+
+
+# ------------------------------------------------------------------------------------------------ coarse_sdf's depth-map estimate
+def _number(who, name, v):
+    if isinstance(v, bool) or not isinstance(v, (int, float, np.floating, np.integer)):
+        raise ValueError("%s: %s must be a Python number, got %r" % (who, name, v))
+    return float(v)
+
+
+def _depth_map(who, self, depth):
+    """(H, W, stride_h, stride_w, sx, sy) of the depth view; sx, sy are SuGaR's factor / image_width and factor / image_height
+    (SS/:1193-1196), Python doubles rounded to float32 as torch rounds a Python scalar that multiplies a float32 tensor."""
+    if not isinstance(depth, torch.Tensor) or depth.dim() != 2 or depth.dtype != torch.float32:
+        raise ValueError("%s: depth must be a float32 [H, W] tensor, got %s" % (who, getattr(depth, "shape", type(depth).__name__)))
+    H, W = depth.shape
+    if H < 1 or W < 1:
+        raise ValueError("%s: depth must not be empty, got %s" % (who, tuple(depth.shape)))
+    h_img, w_img = getattr(self, "image_height", None), getattr(self, "image_width", None)
+    for name, v in (("self.image_height", h_img), ("self.image_width", w_img)):
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < 1:
+            raise ValueError("%s: %s must be a positive int, got %r" % (who, name, v))
+    factor = -1 * min(h_img, w_img)
+    return H, W, depth.stride(0), depth.stride(1), float(np.float32(factor / w_img)), float(np.float32(factor / h_img))
+
+
+def _camera(who, fov_camera, dev, with_center):
+    """[36] float32 on dev: get_world_to_view_transform().get_matrix(), get_projection_transform().get_matrix(), znear and
+    get_camera_center(), read through pytorch3d's own methods and concatenated on the device (nothing is read back).  Only the
+    mask reads the centre: without with_center its three floats are zeros and get_camera_center() is not called."""
+    w2v = fov_camera.get_world_to_view_transform().get_matrix()
+    proj = fov_camera.get_projection_transform().get_matrix()
+    center = fov_camera.get_camera_center() if with_center else torch.zeros(3, dtype=torch.float32, device=dev)
+    znear = fov_camera.znear
+    for name, t, n in (("get_world_to_view_transform().get_matrix()", w2v, 16), ("get_projection_transform().get_matrix()", proj, 16),
+                       ("get_camera_center()", center, 3)):
+        if not isinstance(t, torch.Tensor) or t.numel() != n or t.dtype != torch.float32:
+            raise ValueError("%s: fov_camera.%s must be one camera's float32 tensor of %d values, got %s"
+                             % (who, name, n, getattr(t, "shape", type(t).__name__)))
+    if isinstance(znear, torch.Tensor):
+        if znear.numel() != 1 or znear.dtype != torch.float32:
+            raise ValueError("%s: fov_camera.znear must be one float32 value, got %s" % (who, tuple(znear.shape)))
+        _require_cuda(who, w2v, proj, center, znear)
+        znear = znear.detach().reshape(1)
+    else:
+        _require_cuda(who, w2v, proj, center)
+        znear = torch.full((1,), _number(who, "fov_camera.znear", znear), dtype=torch.float32, device=w2v.device)
+    if w2v.device != dev:
+        raise ValueError("%s: the camera is on %s and the model on %s" % (who, w2v.device, dev))
+    return torch.cat([t.detach().reshape(-1) for t in (w2v, proj, znear, center)])
+
+
+def _surface_mask(self, fov_camera, depth, close_gaussian_threshold, want_map_z):
+    who = "close_to_surface_mask"
+    thr = _number(who, "close_gaussian_threshold", close_gaussian_threshold)
+    points, scaling, quaternions = self.points, self.scaling, self.quaternions
+    _check_tensor(who, "self.points", points, (None, 3), torch.float32)
+    P = points.shape[0]
+    _check_tensor(who, "self.scaling", scaling, (P, 3), torch.float32)
+    _check_tensor(who, "self.quaternions", quaternions, (P, 4), torch.float32)
+    H, W, sh, sw, sx, sy = _depth_map(who, self, depth)
+    _require_cuda(who, points, scaling, quaternions, depth)
+    dev = points.device
+    with torch.cuda.device(dev):
+        cam = _camera(who, fov_camera, dev, True)
+        points, scaling, quaternions = (t.detach().contiguous() for t in (points, scaling, quaternions))
+        mask = torch.empty(P, dtype=torch.bool, device=dev)
+        map_z = torch.empty(P, dtype=torch.float32, device=dev) if want_map_z else None
+        rc = _lib_handle().gsr_sugar_surface_mask(P, H, W, sh, sw, depth.data_ptr(), sx, sy, cam.data_ptr(), points.data_ptr(),
+                                                  scaling.data_ptr(), quaternions.data_ptr(), float(np.float32(thr)), mask.data_ptr(),
+                                                  _ptr(map_z), _lib.stream_ptr(dev))
+        _lib.check(rc, "gsr_sugar_surface_mask")
+    return mask, map_z
+
+
+def close_to_surface_mask(self, fov_camera, depth, close_gaussian_threshold=2.):
+    """coarse_sdf's gaussians_close_to_surface (CS/:655-666) in CUDA: bool [P], True where |map_z(p) - z| < threshold *
+    |scaling * quaternion_apply(quaternion_invert(q), normalize(c - p))|, with z the depth of the centre p in the camera and map_z
+    the rendered depth there (SuGaR.get_points_depth_in_depth_map, SS/:1189-1204).  ``depth`` is the [H, W] depth render (a strided
+    channel view is read in place); the camera is read through pytorch3d's get_world_to_view_transform(),
+    get_projection_transform(), znear and get_camera_center().  No gradient, as under the trainer's torch.no_grad().
+
+    Raises ValueError, naming the argument, for a wrong shape or dtype, a threshold that is not a number or a model without
+    image_height / image_width; RuntimeError for CPU tensors (there is no CPU path)."""
+    return _surface_mask(self, fov_camera, depth, close_gaussian_threshold, False)[0]
+
+
+def _depth_loss_forward(cfg, x, depth, sdf, cam):
+    N, H, W, sh, sw, sx, sy, inv_std, cmax = cfg
+    dev = x.device
+    out = torch.empty((), dtype=torch.float32, device=dev)
+    count = torch.empty(1, dtype=torch.int64, device=dev)
+    L = _lib_handle()
+    nbytes = L.gsr_sugar_depth_sdf_loss_bytes(N)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    rc = L.gsr_sugar_depth_sdf_loss(N, H, W, sh, sw, depth.data_ptr(), sx, sy, cam.data_ptr(), _ptr(x) if N else None,
+                                    _ptr(sdf) if N else None, inv_std, cmax, out.data_ptr(), count.data_ptr(), ws.data_ptr(), nbytes,
+                                    _lib.stream_ptr(dev))
+    _lib.check(rc, "gsr_sugar_depth_sdf_loss")
+    return out, count
+
+
+class _DepthSdfLoss(torch.autograd.Function):
+    """One output: the 0-dim mean; differentiable with respect to the samples, the depth map and the sdf values."""
+
+    @staticmethod
+    def forward(ctx, x, depth, sdf, cam, cfg):
+        ctx.set_materialize_grads(False)
+        out, count = _depth_loss_forward(cfg, x, depth, sdf, cam)
+        ctx.cfg = cfg
+        ctx.save_for_backward(x, depth, sdf, cam, count)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        x, depth, sdf, cam, count = ctx.saved_tensors
+        N, H, W, sh, sw, sx, sy, inv_std, cmax = ctx.cfg
+        need = ctx.needs_input_grad
+        if g is None:
+            return None, None, None, None, None
+        dev = x.device
+        g = g.reshape(1).contiguous()
+        d_x = torch.empty((N, 3), dtype=torch.float32, device=dev)
+        d_sdf = torch.empty(N, dtype=torch.float32, device=dev)
+        d_depth = torch.empty((H, W), dtype=torch.float32, device=dev)
+        L = _lib_handle()
+        args = (N, H, W, sh, sw, depth.data_ptr(), sx, sy, cam.data_ptr(), _ptr(x) if N else None, _ptr(sdf) if N else None, inv_std,
+                cmax, count.data_ptr(), g.data_ptr(), _ptr(d_x) if N else None, _ptr(d_sdf) if N else None, d_depth.data_ptr())
+        if torch.are_deterministic_algorithms_enabled():  # fixed-order sums (DESIGN §4), no atomics
+            nbytes = L.gsr_sugar_depth_sdf_loss_backward_det_bytes(N, H, W)
+            scratch = _lib.scratch_bytes(max(nbytes, 16), dev)
+            rc = L.gsr_sugar_depth_sdf_loss_backward_det(*args, scratch.data_ptr(), nbytes, _lib.stream_ptr(dev))
+            _lib.check(rc, "gsr_sugar_depth_sdf_loss_backward_det")
+        else:
+            rc = L.gsr_sugar_depth_sdf_loss_backward(*args, _lib.stream_ptr(dev))
+            _lib.check(rc, "gsr_sugar_depth_sdf_loss_backward")
+        return d_x if need[0] else None, d_depth if need[1] else None, d_sdf if need[2] else None, None, None
+
+
+def depth_sdf_estimation_loss(self, fov_camera, depth, sdf_samples, sdf_values, sdf_sample_std, clamp_max):
+    """coarse_sdf's 'sdf' estimation loss (CS/:689-712 with the trainers' defaults: not squared, normalize_by_sdf_std=False) in
+    CUDA, the 0-dim mean before the trainer's sdf_estimation_factor: over the samples in front of the camera (z > znear),
+    clamp(|sdf_values - |map_z - z|| / sdf_sample_std, max=clamp_max).mean(), map_z being the depth map's value at the sample's
+    projection (SuGaR.get_points_depth_in_depth_map, SS/:1189-1204).  NaN when no sample is in front, as torch's mean of an empty
+    tensor.  Differentiable with respect to sdf_samples [N,3], depth [H,W] (a strided channel view is read in place) and
+    sdf_values [N]; under torch.use_deterministic_algorithms the depth gradient is summed in a fixed order.  Nothing is read back
+    to the host, in the forward or the backward.  sdf_sample_std (the trainer's get_cameras_spatial_extent() / 10) and clamp_max
+    (10 * get_cameras_spatial_extent()) are Python numbers; the camera is read as by close_to_surface_mask.
+
+    Raises ValueError, naming the argument, for a wrong shape or dtype or a std or clamp that is not a number; RuntimeError for
+    CPU tensors (there is no CPU path)."""
+    who = "depth_sdf_estimation_loss"
+    std = _number(who, "sdf_sample_std", sdf_sample_std)
+    cmax = _number(who, "clamp_max", clamp_max)
+    _check_tensor(who, "sdf_samples", sdf_samples, (None, 3), torch.float32)
+    N = sdf_samples.shape[0]
+    _check_tensor(who, "sdf_values", sdf_values, (N,), torch.float32)
+    H, W, sh, sw, sx, sy = _depth_map(who, self, depth)
+    _require_cuda(who, sdf_samples, sdf_values, depth)
+    dev = sdf_samples.device
+    with np.errstate(divide="ignore", over="ignore"):
+        inv_std = float(np.float32(1.0) / np.float32(std))  # torch divides a CUDA tensor by a Python number as x * (1 / b)
+    cfg = (N, H, W, sh, sw, sx, sy, inv_std, float(np.float32(cmax)))
+    with torch.cuda.device(dev):
+        cam = _camera(who, fov_camera, dev, False)
+        x, sdf = sdf_samples.contiguous(), sdf_values.contiguous()
+        if torch.is_grad_enabled() and any(t.requires_grad for t in (x, depth, sdf)):
+            return _DepthSdfLoss.apply(x, depth, sdf, cam, cfg)
+        return _depth_loss_forward(cfg, x, depth, sdf, cam)[0]

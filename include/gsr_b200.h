@@ -19,6 +19,9 @@
  *                               (scene/gaussian_model.py:268-417) and SuGaRDensifier (sugar_scene/sugar_densifier.py:48-246)
  *   gsr_sugar_sample  replaces  SuGaR.sample_points_in_gaussians               sugar_scene/sugar_model.py:757-799;
  *                               gsr_sugar_sample_backward its autograd backward
+ *   gsr_sugar_surface_mask replaces coarse_sdf's close-to-surface mask           sugar_trainers/coarse_sdf.py:655-665
+ *   gsr_sugar_depth_sdf_loss replaces coarse_sdf's depth-map 'sdf' estimation loss  coarse_sdf.py:689-712 (get_points_depth_in_depth_map
+ *                               sugar_model.py:1189-1204); gsr_sugar_depth_sdf_loss_backward its autograd backward
  *   gsr_adam_step     replaces  torch.optim.Adam.step() (foreach) of every trainer  GS/train.py:183-184, scene_representation.py:538-540,
  *                               sugar_trainers/coarse_density.py:822
  *   gsr_photometric_loss replaces l1_loss and ssim of every trainer's objective  GS/utils/loss_utils.py:17-18, :33-62 (train.py:98-99,
@@ -471,6 +474,61 @@ int gsr_sugar_sample_backward_det(int32_t N, int32_t P, float sampling_scale_fac
                                   const float* scaling, const float* quaternions, const double* total, const float* dL_dsamples,
                                   float* dL_dpoints, float* dL_dscaling, float* dL_dquaternions, void* scratch, size_t scratch_bytes,
                                   void* stream);
+
+/* coarse_sdf's depth-map SDF estimate (sugar_trainers/coarse_sdf.py:650-712, SuGaR.get_points_depth_in_depth_map
+ * sugar_model.py:1189-1204).  The depth map is the float32 view depth [H,W] read with element strides (stride_h, stride_w), so a
+ * channel of an [H,W,3] render is read in place.  camera [36] (device, float32) = the world-to-view matrix M (16, row-major, row
+ * vectors: [p, 1] @ M, as pytorch3d's get_world_to_view_transform().get_matrix()), the projection matrix (16, likewise, as
+ * get_projection_transform().get_matrix(): K^T for SuGaR's SfM cameras), znear, the camera centre (3).  sx, sy are SuGaR's
+ * -min(H_img, W_img) / W_img and -min(H_img, W_img) / H_img rounded to float32.  The map depth of a world point p is
+ *   v = ([p, 1] @ M).xyz / w;  h = [v, 1] @ K^T;  grid = (sx h.x / h.w, sy h.y / h.w)
+ *   map_z = torch's CUDA grid_sample(depth, grid, bilinear, border, align_corners=False): same unnormalize, clip, weights, taps.
+ * The 4x4 products are fp32 multiply-add chains in row order; the rest is one rounding per torch op, with the multiply-adds
+ * torch's grid sampler is compiled to.
+ *
+ * gsr_sugar_surface_mask: for P Gaussians (points, scaling [P,3], quaternions [P,4] as SuGaR's getters return them), out_mask [P]
+ * (bytes 0/1) = |map_z(p) - v.z| < threshold * |scaling * quaternion_apply(quaternion_invert(q), normalize(c - p))| (coarse_sdf.py
+ * :655-666; pytorch3d's Hamilton products, one rounding per op); out_map_z [P] (may be NULL) = map_z(p).  No gradient.
+ * P = 0 is a no-op; P < 0, H or W < 1, H * W >= 2^31 or a missing pointer other than out_map_z is GSR_ERR_INVALID. */
+int gsr_sugar_surface_mask(int32_t P, int32_t H, int32_t W, int64_t depth_stride_h, int64_t depth_stride_w, const float* depth,
+                           float sx, float sy, const float* camera, const float* points, const float* scaling, const float* quaternions,
+                           float threshold, uint8_t* out_mask, float* out_map_z, void* stream);
+
+/* gsr_sugar_depth_sdf_loss: coarse_sdf's 'sdf' estimation loss (coarse_sdf.py:689-712, not squared, not normalised by the sample
+ * std) over N samples [N,3] with their field sdf_values [N]: with v the camera-space sample and masked = v.z > znear,
+ *   term = clamp(|sdf - |map_z - v.z|| * inv_std, max=clamp_max)   (inv_std = float32 1 / float32(std), as torch divides a
+ *                                                                    CUDA tensor by a Python number)
+ *   out_loss [1] = sum of term over the masked samples / their count (NaN when none is masked), out_count [1] (int64) = the count.
+ * Both sums run on the device in a fixed order (float64, then one division), so the result does not depend on the launch.
+ * N < 0, H or W < 1, H * W >= 2^31, 4 N >= 2^32 or a missing pointer is GSR_ERR_INVALID; `workspace` (16-byte aligned) needs
+ * gsr_sugar_depth_sdf_loss_bytes(N) bytes, else GSR_ERR_WORKSPACE.  No host synchronisation. */
+size_t gsr_sugar_depth_sdf_loss_bytes(int32_t N);
+int gsr_sugar_depth_sdf_loss(int32_t N, int32_t H, int32_t W, int64_t depth_stride_h, int64_t depth_stride_w, const float* depth,
+                             float sx, float sy, const float* camera, const float* samples, const float* sdf_values, float inv_std,
+                             float clamp_max, float* out_loss, int64_t* out_count, void* workspace, size_t workspace_bytes,
+                             void* stream);
+
+/* Backward of gsr_sugar_depth_sdf_loss (same arguments; count as the forward wrote it; dL_dloss [1]): dL_dsamples [N,3] (through
+ * v.z, the projection and the bilinear weights), dL_dsdf [N] and dL_ddepth [H,W] (contiguous, the four taps of every masked
+ * sample), all written in full.  A gradient is 0 where torch's autograd of the same expression gives 0: an unmasked sample, a
+ * clamped term (term > clamp_max), sign(0) of either |.|, and a grid coordinate the border clip moved or left exactly on a limit.
+ * dL_ddepth is summed with atomics here; gsr_sugar_depth_sdf_loss_backward_det sums it in a fixed order. */
+int gsr_sugar_depth_sdf_loss_backward(int32_t N, int32_t H, int32_t W, int64_t depth_stride_h, int64_t depth_stride_w, const float* depth,
+                                      float sx, float sy, const float* camera, const float* samples, const float* sdf_values, float inv_std,
+                                      float clamp_max, const int64_t* count, const float* dL_dloss, float* dL_dsamples, float* dL_dsdf,
+                                      float* dL_ddepth, void* stream);
+
+/* Deterministic backward of gsr_sugar_depth_sdf_loss: gsr_sugar_depth_sdf_loss_backward's arguments plus a device scratch (16-byte
+ * aligned) of at least gsr_sugar_depth_sdf_loss_backward_det_bytes(N, H, W) = G(4 N, H W) bytes (G as for
+ * gsr_sugar_field_backward_det).  Tap k of sample n (id 4n + k) goes to its texel; every texel of dL_ddepth is a sequential fp32
+ * sum from +0.0 of its partials in ascending id.  dL_dsamples and dL_dsdf are per sample and equal the atomic backward's.  A NULL
+ * or misaligned scratch (when N > 0) is GSR_ERR_INVALID, a smaller one GSR_ERR_WORKSPACE, both before anything is enqueued. */
+size_t gsr_sugar_depth_sdf_loss_backward_det_bytes(int32_t N, int32_t H, int32_t W);
+int gsr_sugar_depth_sdf_loss_backward_det(int32_t N, int32_t H, int32_t W, int64_t depth_stride_h, int64_t depth_stride_w,
+                                          const float* depth, float sx, float sy, const float* camera, const float* samples,
+                                          const float* sdf_values, float inv_std, float clamp_max, const int64_t* count,
+                                          const float* dL_dloss, float* dL_dsamples, float* dL_dsdf, float* dL_ddepth, void* scratch,
+                                          size_t scratch_bytes, void* stream);
 
 /* Densification statistics (GaussianModel.add_densification_stats plus the trainers' max-radii line, gaussian_model.py:415-417,
  * train.py:163-164; SuGaRDensifier.update_densification_stats, sugar_densifier.py:156-164).  For every row i < P with mask[i] != 0:
