@@ -35,7 +35,7 @@ class gsr_workspace(C.Structure):
 class gsr_counters(C.Structure):
     _fields_ = [("num_rendered", C.c_uint32), ("overflow", C.c_uint32), ("max_tile", C.c_uint32), ("trapped", C.c_uint32),
                 ("num_visible", C.c_uint32), ("foot_total", C.c_uint32), ("exact_redos", C.c_uint32),
-                ("blend_next", C.c_uint32)]
+                ("reserved", C.c_uint32)]
 
 
 class gsr_grads(C.Structure):
@@ -157,7 +157,6 @@ SIGNATURES = {
     "gsr_profile_begin": (_int, [_int]),
     "gsr_profile_begin_strided": (_int, [_int, _int]),
     "gsr_profile_end": (_int, [C.POINTER(C.c_float), C.POINTER(C.c_int)]),
-    "gsr_set_option": (_int, [C.c_char_p, _int]),
     "gsr_last_error": (C.c_char_p, []),
     "gsr_abi_version": (_int, []),
 }
@@ -186,12 +185,6 @@ def _load() -> C.CDLL:
 
 
 lib = _load()
-
-# GSR_OPTIONS="name=value,name=value": gsr_set_option calls at import (experiment harnesses; every setting renders the same bits)
-for _kv in filter(None, os.environ.get("GSR_OPTIONS", "").split(",")):
-    _k, _v = _kv.split("=")
-    if lib.gsr_set_option(_k.strip().encode(), int(_v)) != 0:
-        raise ImportError("autovfx_b200: bad GSR_OPTIONS entry %r" % _kv)
 
 
 def check(rc: int, what: str) -> None:

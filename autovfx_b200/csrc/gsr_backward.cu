@@ -17,7 +17,6 @@
 //     (the reference zero-fills all 304 B/Gaussian, rasterize_points.cu:158-168).
 // Gradient sums are accumulated in a different order than the reference's atomics (which are themselves
 // unordered), so parity is to a tolerance, not bitwise.
-#include <cstdlib>
 #include <type_traits>
 #include "gsr_common.cuh"
 #include "gsr_packed.cuh"
@@ -856,16 +855,12 @@ __global__ void __launch_bounds__(GB_THREADS) k_gaussian_backward(const GBParams
     }
 }
 
-// Resident CTAs per SM the blend backward is compiled for: GSR_BWD_OCC=8|6|5 (64 / 80 / 96 registers), an experiment knob.
-// Default 6 for the plain kernel; 5 for the one with a second colour set, whose three more live values per survivor and per
-// pixel do not fit in 80 registers without spilling.
+// Resident CTAs per SM the blend backward is compiled for: 6 (80 registers) for the plain kernel, 5 (96 registers) for the
+// one with a second colour set, whose three more live values per survivor and per pixel do not fit in 80 registers without
+// spilling.
 template <int NX, bool DET>
 static void launch_blend_backward(const BwdArgs& ba, dim3 grid, cudaStream_t st) {
-    static int occ = -1;
-    if (occ < 0) { const char* e = getenv("GSR_BWD_OCC"); occ = e ? atoi(e) : 0; }
-    if (occ == 8) k_blend_backward<NX, 8, DET><<<grid, BWL_WARPS * 32, 0, st>>>(ba);
-    else if (occ == 5 || (NX && occ != 6)) k_blend_backward<NX, 5, DET><<<grid, BWL_WARPS * 32, 0, st>>>(ba);
-    else k_blend_backward<NX, 6, DET><<<grid, BWL_WARPS * 32, 0, st>>>(ba);
+    k_blend_backward<NX, NX ? 5 : 6, DET><<<grid, BWL_WARPS * 32, 0, st>>>(ba);
 }
 
 }  // namespace gsr

@@ -340,91 +340,18 @@ __device__ __forceinline__ void blend_item(const BlendArgs& a, const int bx, con
     }
 }
 
-// OCC: resident warps per SM the kernel is compiled for (32 -> 64 registers, 40 -> 48, 48 -> 40)
+// OCC: resident warps per SM the kernel is compiled for (32 -> 64 registers; 24 -> 80, which the second colour set needs)
 template <int NX, bool NC, bool EXACT, int WARPS, int OCC>
 __global__ void __launch_bounds__(WARPS * 32, OCC / WARPS) k_blend_lists(const BlendArgs a) {
     __shared__ __align__(16) unsigned char sq[WARPS * ListCfg<NX>::WB];
     blend_item<NX, NC, EXACT, WARPS>(a, (int)blockIdx.x, (int)blockIdx.y, sq);
 }
 
-// Persistent variant (gsr_set_option("blend_persist", K), off by default): K CTAs per SM draw work items from
-// counters->blend_next, so the kernel never holds more than K * WARPS warps of an SM and kernels of the NEXT frame, issued on
-// another stream, can co-reside with it.  An experiment knob (tools/sweep_options.py compares it per kernel); it renders the
-// same bits (tests/test_gpu_options.py).
-template <int NX, bool NC, bool EXACT, int WARPS, int OCC>
-__global__ void __launch_bounds__(WARPS * 32, OCC / WARPS) k_blend_lists_persistent(const BlendArgs a) {
-    __shared__ __align__(16) unsigned char sq[WARPS * ListCfg<NX>::WB];
-    __shared__ uint32_t s_work[2];
-    constexpr int PARTS = GSR_FOOTS / WARPS;
-    const uint32_t per_row = (uint32_t)(a.gx * PARTS), nwork = per_row * (uint32_t)a.gy;
-    uint32_t next = 0;
-    int par = 0;
-    if (threadIdx.x == 0) next = atomicAdd(&a.counters->blend_next, 1u);
-    for (;;) {
-        if (threadIdx.x == 0) s_work[par] = next;
-        __syncthreads();
-        const uint32_t w = s_work[par];
-        par ^= 1;
-        if (w >= nwork) break;
-        if (threadIdx.x == 0) next = atomicAdd(&a.counters->blend_next, 1u);  // the next item's ticket is in flight during this one
-        const uint32_t by = w / per_row;
-        blend_item<NX, NC, EXACT, WARPS>(a, (int)(w - by * per_row), (int)by, sq);
-    }
-}
-
-static int blend_occ() {  // GSR_BLEND_OCC=32|40|48: resident warps per SM (register budget) of the 5-channel kernel, an experiment knob
-    static int w = -1;
-    if (w < 0) {
-        const char* e = getenv("GSR_BLEND_OCC");
-        w = e ? atoi(e) : 32;
-        if (w != 32 && w != 40 && w != 48) w = 32;
-    }
-    return w;
-}
-
-// gsr_set_option("blend_persist", K): 0 = one CTA per work item (default), K > 0 = persistent kernel with K CTAs per SM
-static int g_blend_persist = -1;
-static int g_sm_count = 0;
-int set_blend_persist(int k) {
-    if (k < 0 || k > 16) return GSR_ERR_INVALID;
-    g_blend_persist = k;
-    return GSR_OK;
-}
-static int blend_persist() {
-    if (g_blend_persist < 0) {
-        const char* e = getenv("GSR_BLEND_PERSIST");
-        g_blend_persist = e ? atoi(e) : 0;
-        if (g_blend_persist < 0 || g_blend_persist > 16) g_blend_persist = 0;
-    }
-    if (g_blend_persist > 0 && g_sm_count == 0) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || g_sm_count <= 0) g_sm_count = 132;
-    }
-    return g_blend_persist;
-}
-
 template <int NX, bool NC, bool EXACT>
 static void launch_w(const BlendArgs& a, cudaStream_t st) {
     constexpr int WARPS = 4;  // footprints per CTA
     const dim3 grid(a.gx * (GSR_FOOTS / WARPS), a.gy);
-    const int persist = blend_persist();
-    if (persist > 0) {
-        // the work cursor lives in the frame's counters (zeroed with them at the start of the frame; a second blend on the same
-        // workspaces — GSR_FLAG_REUSE_GEOMETRY — needs it cleared again)
-        cudaMemsetAsync(&a.counters->blend_next, 0, sizeof(uint32_t), st);
-        const int ctas = (int)min((long long)persist * g_sm_count, (long long)grid.x * grid.y);
-        k_blend_lists_persistent<NX, NC, EXACT, WARPS, (NX ? 24 : 32)><<<ctas, WARPS * 32, 0, st>>>(a);
-        return;
-    }
-    if constexpr (NX != 0) k_blend_lists<NX, NC, EXACT, WARPS, 24><<<grid, WARPS * 32, 0, st>>>(a);
-    else {
-        switch (blend_occ()) {
-            case 48: k_blend_lists<NX, NC, EXACT, WARPS, 48><<<grid, WARPS * 32, 0, st>>>(a); break;
-            case 40: k_blend_lists<NX, NC, EXACT, WARPS, 40><<<grid, WARPS * 32, 0, st>>>(a); break;
-            default: k_blend_lists<NX, NC, EXACT, WARPS, 32><<<grid, WARPS * 32, 0, st>>>(a); break;
-        }
-    }
+    k_blend_lists<NX, NC, EXACT, WARPS, (NX ? 24 : 32)><<<grid, WARPS * 32, 0, st>>>(a);
 }
 template <int NX, bool NC>
 static void launch_e(const BlendArgs& a, cudaStream_t st) {

@@ -21,7 +21,6 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
-#include <cstring>
 #include "gsr_common.cuh"
 #include "gsr_packed.cuh"
 
@@ -76,11 +75,6 @@ __host__ __device__ constexpr int sh_stride(int deg, bool vec, bool win = false)
     return vec ? (sh_nv(deg, win) % 2 == 0 ? (sh_nv(deg, win) + 1) * 4 : sh_nv(deg, win) * 4) : (sh_nf(deg) | 1);
 }
 
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
-    unsigned s = (unsigned)__cvta_generic_to_shared(smem);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(gmem));
-}
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
 // orders this thread's earlier generic-proxy accesses to shared memory before later async-proxy (TMA) writes to it
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 
@@ -202,17 +196,17 @@ __device__ __forceinline__ void cov3d_ref_rounding(float sx, float sy, float sz,
 // row is requested first, so that its latency overlaps the 3D covariance, EWA projection, conic, radius, tile rectangle
 // (forward.cu:155-256) and the per-tile histogram with ranked tickets; then SH -> RGB (forward.cu:20-71), the whole 48-byte
 // record in one go, and the compact list of visible Gaussians the emission kernel walks.
-// DEG = -1: colours are precomputed.  VEC: SH rows are 16-byte aligned (M % 4 == 0) -> 16-byte staging, either one TMA bulk
-// copy per Gaussian issued by its own lane (BULK) or coalesced cp.async by the whole warp; otherwise scalar loads.  WIN (with
-// VEC and BULK): rows are only 4-byte aligned (M = 25, the SuGaR storage: 300-byte rows) — each lane bulk-copies the 16-byte
-// aligned window that contains its coefficients (one extra float4) and evaluates from its row's offset inside the window.
+// DEG = -1: colours are precomputed.  VEC: SH rows are 16-byte aligned (M % 4 == 0) -> one TMA bulk copy per Gaussian, issued
+// by its own lane; otherwise scalar loads.  WIN (with VEC): rows are only 4-byte aligned (M = 25, the SuGaR storage: 300-byte
+// rows) — each lane bulk-copies the 16-byte aligned window that contains its coefficients (one extra float4) and evaluates
+// from its row's offset inside the window.
 struct ProjCand {  // one phase-1 survivor
     float mx, my, mz, opacity;
     float a0, a1, a2, a3, a4, a5, a6;  // scale.xyz + rotation.rxyz, or cov3D[0..5]
     int idx;
 };
 
-template <int DEG, bool VEC, bool BULK, bool WIN, bool TIGHT>
+template <int DEG, bool VEC, bool WIN, bool TIGHT>
 __global__ void __launch_bounds__(PRE_THREADS, 8) k_project(const PreParams p) {
     constexpr int DG = DEG < 0 ? 0 : DEG;
     constexpr int NF = sh_nf(DG);
@@ -230,7 +224,7 @@ __global__ void __launch_bounds__(PRE_THREADS, 8) k_project(const PreParams p) {
     if (tid < 16) cam.view[tid] = p.view[tid];
     else if (tid < 32) cam.proj[tid - 16] = p.proj[tid - 16];
     else if (tid < 35) cam.campos[tid - 32] = p.campos[tid - 32];
-    if (DEG >= 0 && VEC && BULK && lane == 0) {
+    if (DEG >= 0 && VEC && lane == 0) {
         mbar_init((uint32_t)__cvta_generic_to_shared(&stage_bar[warp]), 1u);
         mbar_fence_init();
     }
@@ -326,7 +320,7 @@ __global__ void __launch_bounds__(PRE_THREADS, 8) k_project(const PreParams p) {
     int win_off = 0;  // floats between the start of the staged window and the row's first coefficient (WIN only)
     if constexpr (DEG >= 0) {
         const size_t row_floats = (size_t)p.M * 3;
-        if (VEC && BULK) {
+        if (VEC) {
             constexpr int NV = sh_nv(DG, WIN);
             if (lane == 0) mbar_arrive_expect_tx(bar, (uint32_t)__popc(cmask) * NV * 16u);
             if (valid) {
@@ -336,15 +330,6 @@ __global__ void __launch_bounds__(PRE_THREADS, 8) k_project(const PreParams p) {
                     src -= win_off;
                 }
                 bulk_g2s((uint32_t)__cvta_generic_to_shared(wstage + lane * STRIDE), src, NV * 16u, bar);
-            }
-        } else if (VEC) {
-            constexpr int NV = (NF + 3) / 4;
-#pragma unroll
-            for (int it = 0; it < NV; it++) {
-                const int item = it * 32 + lane;
-                const int gl = item / NV, part = item - gl * NV;
-                const uint32_t gid = __shfl_sync(GSR_FULL, (uint32_t)idx, gl);
-                if ((cmask >> gl) & 1u) cp_async16(wstage + gl * STRIDE + part * 4, p.shs + (size_t)gid * row_floats + part * 4);
             }
         } else {
 #pragma unroll 4
@@ -457,8 +442,7 @@ __global__ void __launch_bounds__(PRE_THREADS, 8) k_project(const PreParams p) {
             rgb[2] = p.colors_precomp[3 * (size_t)idx + 2];
         }
     } else {
-        if (VEC && BULK) mbar_wait(bar, 0u);
-        else if (VEC) cp_async_wait_all();
+        if (VEC) mbar_wait(bar, 0u);
         __syncwarp();
         if (vis) sh_eval<DG>(wstage + lane * STRIDE + win_off, make_float3(c.mx, c.my, c.mz), cam.campos, rgb, clamp_bits);
     }
@@ -1167,15 +1151,14 @@ __device__ void sort_tile(const uint2 rg, unsigned long long* __restrict__ g, un
 template <bool PACKED>
 __global__ void __launch_bounds__(SORT_THREADS, 5) k_sort_tiles(const uint2* __restrict__ ranges, unsigned long long* pairs,
                                                              unsigned long long* slab, uint32_t slab_stride, uint32_t* __restrict__ point_list,
-                                                             const gsr_counters* __restrict__ counters, int keep_pairs, const FootArgs fa,
-                                                             const int sort_small_enabled) {
+                                                             const gsr_counters* __restrict__ counters, int keep_pairs, const FootArgs fa) {
     if (counters->overflow) return;  // set by k_tile_scan, before this kernel started
     __shared__ unsigned long long s[SORT_CAP];
     __shared__ uint32_t hist[SORT_BUCKETS + 1];
     __shared__ uint16_t tk16[SORT_SMALL];
     const uint2 rg = ranges[blockIdx.x];
     unsigned long long* g = slab ? slab + (size_t)blockIdx.x * slab_stride : pairs + rg.x;
-    sort_tile<PACKED>(rg, g, pairs, point_list, keep_pairs, s, hist, sort_small_enabled ? tk16 : nullptr, fa, (int)blockIdx.x);
+    sort_tile<PACKED>(rg, g, pairs, point_list, keep_pairs, s, hist, tk16, fa, (int)blockIdx.x);
 }
 
 // =====================================================================================================
@@ -1222,22 +1205,13 @@ static inline void prof_mark(int k, cudaStream_t st) {
 // =====================================================================================================
 // host side
 // =====================================================================================================
-static int sh_bulk_mode() {  // GSR_SH_STAGING=cpasync selects the LDGSTS path, default is the TMA bulk copy
-    static int mode = -1;
-    if (mode < 0) {
-        const char* e = getenv("GSR_SH_STAGING");
-        mode = (e && strcmp(e, "cpasync") == 0) ? 0 : 1;
-    }
-    return mode;
-}
 template <int DEG, bool TIGHT>
 static void launch_project_v(bool vec, bool win, const PreParams& pp, cudaStream_t st) {
     const int grid = (pp.P + PRE_THREADS - 1) / PRE_THREADS;
-    if constexpr (DEG < 0) k_project<-1, false, false, false, TIGHT><<<grid, PRE_THREADS, 0, st>>>(pp);
-    else if (win && sh_bulk_mode()) k_project<DEG, true, true, true, TIGHT><<<grid, PRE_THREADS, 0, st>>>(pp);
-    else if (vec && sh_bulk_mode()) k_project<DEG, true, true, false, TIGHT><<<grid, PRE_THREADS, 0, st>>>(pp);
-    else if (vec) k_project<DEG, true, false, false, TIGHT><<<grid, PRE_THREADS, 0, st>>>(pp);
-    else k_project<DEG, false, false, false, TIGHT><<<grid, PRE_THREADS, 0, st>>>(pp);
+    if constexpr (DEG < 0) k_project<-1, false, false, TIGHT><<<grid, PRE_THREADS, 0, st>>>(pp);
+    else if (win) k_project<DEG, true, true, TIGHT><<<grid, PRE_THREADS, 0, st>>>(pp);
+    else if (vec) k_project<DEG, true, false, TIGHT><<<grid, PRE_THREADS, 0, st>>>(pp);
+    else k_project<DEG, false, false, TIGHT><<<grid, PRE_THREADS, 0, st>>>(pp);
 }
 template <int DEG>
 static void launch_project(bool vec, bool win, bool tight, const PreParams& pp, cudaStream_t st) {
@@ -1246,13 +1220,6 @@ static void launch_project(bool vec, bool win, bool tight, const PreParams& pp, 
 }
 
 static void launch_blend(const BlendArgs& a, cudaStream_t st) { launch_blend_lists(a, st); }
-
-// process-wide experiment / tuning options of the forward (gsr_set_option)
-struct ForwardOptions {
-    int sort_single_pass = 1;  // tiles of <= SORT_SMALL instances are read from global memory once (sort_bucket_small)
-};
-static ForwardOptions g_opt;
-int set_blend_persist(int k);
 
 }  // namespace gsr
 
@@ -1329,15 +1296,6 @@ int gsr_profile_end(float* ms, int* frames) {
     for (int k = 0; k < 5; k++) ms[k] = g_prof.frames ? (float)(acc[k] / g_prof.frames) : 0.f;
     if (frames) *frames = g_prof.frames;
     return GSR_OK;
-}
-
-int gsr_set_option(const char* name, int value) {
-    if (!name) { set_error("gsr_set_option: null name"); return GSR_ERR_INVALID; }
-    int rc = GSR_ERR_INVALID;
-    if (strcmp(name, "blend_persist") == 0) rc = set_blend_persist(value);
-    else if (strcmp(name, "sort_single_pass") == 0) { g_opt.sort_single_pass = value ? 1 : 0; rc = GSR_OK; }
-    if (rc != GSR_OK) set_error("gsr_set_option: unknown option or bad value (%s = %d)", name, value);
-    return rc;
 }
 
 static int forward_impl(const gsr_frame* f, const gsr_workspace* ws, float* out_color, float* out_depth, float* out_alpha,
@@ -1482,8 +1440,8 @@ static int forward_impl(const gsr_frame* f, const gsr_workspace* ws, float* out_
     uint32_t* n_contrib = (flags & GSR_FLAG_FOR_BACKWARD) ? (uint32_t*)(img + il.n_contrib) : nullptr;
     FootArgs fa{pp.records, (uint32_t*)(bin + bl.bal), il.gx};
     unsigned long long* pairs = (unsigned long long*)(bin + bl.pairs);
-    if (packed) k_sort_tiles<true><<<il.tiles, SORT_THREADS, 0, st>>>(ranges, pairs, slab, slab_stride, (uint32_t*)(bin + bl.point_list), counters, keep_pairs, fa, g_opt.sort_single_pass);
-    else k_sort_tiles<false><<<il.tiles, SORT_THREADS, 0, st>>>(ranges, pairs, nullptr, 0u, (uint32_t*)(bin + bl.point_list), counters, keep_pairs, fa, g_opt.sort_single_pass);
+    if (packed) k_sort_tiles<true><<<il.tiles, SORT_THREADS, 0, st>>>(ranges, pairs, slab, slab_stride, (uint32_t*)(bin + bl.point_list), counters, keep_pairs, fa);
+    else k_sort_tiles<false><<<il.tiles, SORT_THREADS, 0, st>>>(ranges, pairs, nullptr, 0u, (uint32_t*)(bin + bl.point_list), counters, keep_pairs, fa);
     prof_mark(4, st);
     if ((rc = check_launch("gsr_forward/sort", debug, st))) return rc;
     BlendArgs ba{ranges, (const uint32_t*)(bin + bl.point_list), pp.records, extra_colors, f->W, f->H, il.gx, il.gy, f->bg,

@@ -153,7 +153,7 @@ typedef struct gsr_counters {
     uint32_t num_visible;  /* Gaussians with radii > 0                                             */
     uint32_t foot_total;   /* reserved (0)                                                          */
     uint32_t exact_redos;  /* warps whose pixels were re-blended exactly (default image mode)       */
-    uint32_t blend_next;   /* work cursor of the persistent blend (gsr_set_option("blend_persist", K)); 0 otherwise          */
+    uint32_t reserved;     /* reserved (0)                                                          */
 } gsr_counters;
 
 size_t gsr_geom_bytes(int32_t P);
@@ -707,13 +707,6 @@ int gsr_profile_begin(int max_frames);
 /* Same, timing only every stride-th gsr_forward call. */
 int gsr_profile_begin_strided(int max_frames, int stride);
 int gsr_profile_end(float* ms_per_kernel, int* frames);
-
-/* Process-wide tuning options (not part of the reference's surface; defaults are what bench.py measures unless it says so):
- *   "blend_persist" = K   0: one CTA per half tile (default).  K in 1..16: the blend runs as a persistent kernel with K CTAs per SM
- *                         drawing work from gsr_counters.blend_next, so that it never holds more than 4 K warps of an SM and the
- *                         geometry kernels of the next frame, issued on another stream, run beside it.
- *   "sort_single_pass" = 0|1   1 (default): the per-tile sort reads a tile of <= 2048 instances from global memory once. */
-int gsr_set_option(const char* name, int value);
 
 const char* gsr_last_error(void);
 int gsr_abi_version(void);

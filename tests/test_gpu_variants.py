@@ -3,16 +3,15 @@
 Which colour + emission kernel runs depends on the SH storage: M coefficients per row, the active degree D (clamped to 3)
 and the alignment of the shs rows (16-byte aligned rows with M % 4 == 0 are staged with vector copies, 16-byte aligned
 rows of other widths through an aligned window when it fits, everything else one float at a time), and the backward's
-Gaussian kernel has a special case for M = 16.  More paths are selected per process: GSR_PACKED_KEYS=0 (the general
-sort and emission that scenes of more than 2^24 Gaussians use), GSR_SH_STAGING=cpasync (LDGSTS staging instead of the
-TMA bulk copy) and GSR_BWD_OCC=8|5 (the blend backward compiled for other register budgets).  This file runs each of them:
+Gaussian kernel has a special case for M = 16.  One more path is selected per process: GSR_PACKED_KEYS=0 (the general
+sort and emission that scenes of more than 2^24 Gaussians use).  This file runs each of them:
 
   A. the layout matrix: every (M, D) a GaussianModel can store, with shs rows 16-byte aligned and 4 bytes off, against each
      other (bit identity), the CPU oracle, the compiled reference (bit identity in exact mode) and the exact-mode images;
   B. per-Gaussian gradients against fp64 autograd (tests/torch_ref.py) with each image gradient isolated, judged against the
      CPU oracle's own error on the same case, and the gradients that must be exactly zero;
-  C. the per-process variants, in fresh processes, against the in-process defaults on part of the layout matrix, the gradient
-     cases and the named cases (tiles in every sort regime), and the real P > 2^24 switch;
+  C. the general path, in a fresh process, against the in-process default on part of the layout matrix, the gradient cases
+     and the named cases (tiles in every sort regime), and the real P > 2^24 switch;
   D. distCUDA2 against an exact float64 k-d tree, at the sizes and shapes its search treats specially.
 """
 import os
@@ -244,13 +243,13 @@ def test_clamped_alpha_gradients_against_oracle_and_reference(dev):
 
 
 # ---- C. per-process variants -------------------------------------------------------------------------------------------------
-# the 16-byte aligned M = 16 rows take the vector staging (cp.async under GSR_SH_STAGING=cpasync) at every degree
+# the 16-byte aligned M = 16 rows take the vector staging at every degree
 VARIANT_LAYOUTS = [(1, 0, False), (4, 1, False), (9, 2, False), (16, 0, False), (16, 2, False), (16, 3, True), (25, 3, False),
                    (25, 1, False), (None, 0, False)]
 # named cases of test_gpu_parity.py (dense_tile: tiles of > 4096 instances; coplanar: equal depths, ties broken by id), a scene
 # with tiles in each of the three sort regimes, so that the general (unpacked) path runs every per-tile sort, and the dense
 # gradient cases that reach the blend backward's redo band, ballot block edge, partial footprints and deep termination
-# (tests/helpers.DENSE_CASES), so that every register budget of the backward runs them
+# (tests/helpers.DENSE_CASES)
 VARIANT_CASES = ["dense_tile", "coplanar", "config1", "deg3_m25", "sort_regimes", "skip_band", "faint_slab"]
 
 
@@ -311,8 +310,7 @@ def test_variant_cases_cover_every_tile_sort_regime(default_outputs):
     assert ((n > 0) & (n <= 2048)).any() and ((n > 2048) & (n <= 4096)).any() and (n > 4096).any()
 
 
-@pytest.mark.parametrize("env", [{"GSR_PACKED_KEYS": "0"}, {"GSR_SH_STAGING": "cpasync"}, {"GSR_BWD_OCC": "8"}, {"GSR_BWD_OCC": "5"}],
-                         ids=["packed_keys_off", "sh_staging_cpasync", "bwd_occ_8", "bwd_occ_5"])
+@pytest.mark.parametrize("env", [{"GSR_PACKED_KEYS": "0"}], ids=["packed_keys_off"])
 def test_process_variant_matches_the_default_path(dev, default_outputs, env, tmp_path):
     got = _run_variant(env, tmp_path)
     assert sorted(got) == sorted(default_outputs)

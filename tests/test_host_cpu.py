@@ -32,18 +32,6 @@ def test_library_loads_and_exports_every_declared_symbol():
     assert _lib.lib.gsr_abi_version() == _lib.ABI_VERSION == 4
 
 
-def test_set_option_validates_names_and_values():
-    """gsr_set_option touches no device state: unknown names and out-of-range values are rejected with a message."""
-    from autovfx_b200 import _lib
-    L = _lib.lib
-    assert L.gsr_set_option(b"blend_persist", 0) == 0
-    assert L.gsr_set_option(b"sort_single_pass", 1) == 0
-    assert L.gsr_set_option(b"no_such_option", 1) == -1
-    assert b"no_such_option" in L.gsr_last_error()
-    assert L.gsr_set_option(b"blend_persist", 99) == -1
-    assert L.gsr_set_option(None, 1) == -1
-
-
 def test_workspace_size_queries():
     from autovfx_b200._lib import lib
     assert lib.gsr_geom_bytes(0) > 0

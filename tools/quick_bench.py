@@ -1,6 +1,6 @@
 """Developer A/B harness: per-kernel times of the forward on the bench workload (3M Gaussians, 1080p, trajectory cameras).
 
-    GSR_BLEND=legacy GSR_BLEND_WARPS=4 python tools/quick_bench.py --frames 60 [--exact] [--tight] [--tag name]
+    python tools/quick_bench.py --frames 60 [--exact] [--tight] [--tag name]
 
 Prints one JSON line (and appends it to gpurun_out/quick_bench.jsonl).  Kernel-selection knobs are environment variables read
 once per process, so every variant is its own process.  Not the bench of record (that is bench.py)."""
@@ -101,8 +101,7 @@ def main():
         _lib.check(_lib.lib.gsr_profile_end(ms_k, C.byref(n)), "profile_end")
     st = [t.stats() for t in tk]
     ms = e0.elapsed_time(e1) / K
-    res = {"tag": args.tag, "env": {k: os.environ.get(k) for k in ("GSR_BLEND", "GSR_BLEND_WARPS") if os.environ.get(k)},
-           "exact": args.exact, "tight": args.tight, "streams": NS, "ms_per_frame": round(ms, 4), "fps": round(1000.0 / ms, 1),
+    res = {"tag": args.tag, "exact": args.exact, "tight": args.tight, "streams": NS, "ms_per_frame": round(ms, 4), "fps": round(1000.0 / ms, 1),
            "kernel_ms": {k: round(float(ms_k[i]), 4) for i, k in enumerate(["project", "tile_scan", "emit", "sort_tiles", "blend"])},
            "avg_R": sum(s["num_rendered"] for s in st) / K, "avg_foot": sum(s["foot_total"] for s in st) / K,
            "avg_redos": sum(s["exact_redos"] for s in st) / K, "overflow": sum(s["overflow"] for s in st)}
