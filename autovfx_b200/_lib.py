@@ -64,6 +64,13 @@ class gsr_adam_tensor(C.Structure):
                 ("eps", C.c_float), ("step_size", C.c_float)]
 
 
+class gsr_png_image(C.Structure):
+    _fields_ = [("data", C.c_void_p), ("stride_h", C.c_int64), ("stride_w", C.c_int64), ("stride_c", C.c_int64), ("H", C.c_int32),
+                ("W", C.c_int32), ("C", C.c_int32), ("flags", C.c_int32), ("lut", C.c_void_p)]
+
+
+GSR_PNG_SWAP_RB = 1
+GSR_PNG_MAX_BATCH = 16
 GSR_ADAM_MAX_TENSORS = 32
 GSR_LOSS_REDUCE_BYTES = 256 + 16 * 1024
 GSR_DENSIFY_MAX_GROUPS = 8
@@ -153,6 +160,9 @@ SIGNATURES = {
     "gsr_select_rows": (_int, [_i64] + [_ptr] * 11 + [_size, _ptr]),
     "gsr_pack_masks": (_int, [_i32] * 3 + [_ptr] * 3),
     "gsr_mask_disagreement": (_int, [_i32] * 2 + [_ptr] * 2 + [_f32, _ptr, _ptr]),
+    "gsr_png_bound": (_size, [_i32] * 3),
+    "gsr_png_workspace_bytes": (_size, [_i32, C.POINTER(gsr_png_image)]),
+    "gsr_png_encode": (_int, [C.POINTER(gsr_png_image), _i32, C.POINTER(C.c_void_p), _ptr, _ptr, _size, _ptr]),
     "gsr_get_views": (_int, [_ws, _i32, _i32, _i32, C.POINTER(gsr_views)]),
     "gsr_profile_begin": (_int, [_int]),
     "gsr_profile_begin_strided": (_int, [_int, _int]),

@@ -127,11 +127,12 @@ def _layer_paths(cache, i):
             "smoke_depth": d("depth_smoke_fire"), "fire": c("rgb_smoke_fire_pre")}
 
 
-def blend_frames(blend_results_dir, input_config_path=None):
+def blend_frames(blend_results_dir, input_config_path=None, png_writer=None):
     """Drop-in for BA/:92-348 ``blend_frames``: the same globbing and frame count (BA/:117-132), the module's own loaders
     (``load_rgb``, ``load_depth_exr``), ``composite_frame`` per frame on the current CUDA device, the same ``frames/NNNN.png`` files,
     and the module's ``generate_video_from_frames`` for ``blended.mp4``.  Frame i+1 is decoded on host threads while frame i
-    composites, and the PNGs are written on host threads."""
+    composites, and the PNGs are written on host threads: by PIL by default, or, with ``png_writer`` (a ``png.PngWriter``), encoded
+    on the device (same pixels, different bytes); the writer is flushed before the video is made."""
     ba = _host_module()
     root_dir = os.path.dirname(os.path.normpath(os.path.dirname(os.path.normpath(blend_results_dir))))
     input_config = None
@@ -170,11 +171,18 @@ def blend_frames(blend_results_dir, input_config_path=None):
                 layers["obj3dgs_depth"] = None
             if layers["smoke"] is None:
                 layers["smoke_depth"] = None
-            frame = composite_frame(layers.pop("rgba8"), None, **layers).cpu().numpy()
+            frame_dev = composite_frame(layers.pop("rgba8"), None, **layers)
+            path = os.path.join(out_img_dir, '{:0>4d}.png'.format(i))
+            if png_writer is not None:
+                png_writer.submit(path, frame_dev)
+            frame = frame_dev.cpu().numpy()
             frames.append(frame)
-            saves.append(writers.submit(_save_png, frame, os.path.join(out_img_dir, '{:0>4d}.png'.format(i))))
+            if png_writer is None:
+                saves.append(writers.submit(_save_png, frame, path))
         for s in saves:
             s.result()
+        if png_writer is not None:
+            png_writer.flush()
     ba.generate_video_from_frames(np.array(frames), os.path.join(blend_results_dir, 'blended.mp4'), fps=15)
 
 

@@ -32,6 +32,7 @@
  *   gsr_composite     replaces  the per-frame compositing of blend_frames          blender/blend_all.py:236-342
  *   gsr_select_rows   replaces  the deepcopy + boolean indexing of each candidate subset  extract/extract_object.py:196-202, :315-321
  *   gsr_pack_masks, gsr_mask_disagreement replace the host readback and numpy XOR count of each tracked view  :215-221, :334-340
+ *   gsr_png_encode    replaces  save_image / cv2.imwrite of the frame loop's PNGs     scene_representation.py:424-438; blend_all's frames
  *
  * and, for the render() wrapper around the two rasterizer passes ("GR/" = sugar/gaussian_splatting/gaussian_renderer/__init__.py):
  *
@@ -684,6 +685,32 @@ int gsr_pack_masks(int32_t V, int32_t W, int32_t H, const uint8_t* masks, uint32
  * gsr_pack_masks).  The comparison is float32, and false for a NaN alpha, as numpy's `alpha >= np.float32(thr)` is.  count is an
  * 8-byte aligned device int64; the sum is exact and the same on every run. */
 int gsr_mask_disagreement(int32_t W, int32_t H, const float* alpha, const uint32_t* bits, float thr, int64_t* count, void* stream);
+
+/* PNG encoding (gsr_png.cu): standard 8-bit, non-interlaced PNG files (one IHDR, one IDAT holding one zlib stream, IEND) whose
+ * pixels decode to the input exactly.  The bytes are this encoder's own, not libpng's or zlib's: they depend only on the pixels
+ * and the shape (not on the stream, the batch or the order of atomics).  Nothing synchronises with the host. */
+#define GSR_PNG_SWAP_RB 1    /* read channels 0 and 2 swapped: BGR / BGRA input, RGB / RGBA file */
+#define GSR_PNG_MAX_BATCH 16 /* images per launch; gsr_png_encode launches 4 kernels per group of this many images */
+typedef struct gsr_png_image {
+    const uint8_t* data;                 /* byte (y, x, c) at data + y * stride_h + x * stride_w + c * stride_c (device or UVA) */
+    int64_t stride_h, stride_w, stride_c; /* byte strides, may be negative */
+    int32_t H, W, C;                     /* C in {1, 3, 4}: grey (colour type 0), RGB (2) or RGBA (6) */
+    int32_t flags;                       /* GSR_PNG_SWAP_RB */
+    const uint8_t* lut;                  /* NULL, or a device [256,3] RGB table for C = 1: the file is RGB lut[data] */
+} gsr_png_image;
+/* The largest file an H x W image with C channels in the file (3 for a lookup-table image) can take: the filtered stream
+ * H (1 + W C), 5 bytes per 32 KiB deflate block, and 63 bytes of signature, chunks and zlib framing.  0 for a bad shape or a
+ * stream too long for one IDAT chunk. */
+size_t gsr_png_bound(int32_t H, int32_t W, int32_t C);
+/* Bytes of gsr_png_encode's workspace for these images (about 5.1 times their filtered streams); 0 for bad arguments. */
+size_t gsr_png_workspace_bytes(int32_t n, const gsr_png_image* images);
+/* Encode n images: outputs[i] (device or pinned host memory, at least gsr_png_bound bytes) receives the file and sizes[i] (an
+ * 8-byte aligned device or pinned int64) its length.  `workspace` is 256-byte aligned device memory of gsr_png_workspace_bytes.
+ * An image with no data, H or W < 1, C not in {1, 3, 4}, a lookup table with C != 1, unknown flags or a too-long stream, a NULL
+ * output or misaligned sizes is GSR_ERR_INVALID, a smaller workspace GSR_ERR_WORKSPACE, all before anything is enqueued.
+ * n = 0 is a no-op. */
+int gsr_png_encode(const gsr_png_image* images, int32_t n, uint8_t* const* outputs, int64_t* sizes, void* workspace, size_t workspace_bytes,
+                   void* stream);
 
 /* Device pointers into the workspaces of the last layout (P, capacity, W, H) — for parity tests that
  * compare per-stage buffers with the reference (SURVEY §4).  Pure pointer arithmetic, no CUDA calls. */
