@@ -154,6 +154,16 @@ SIGNATURES = {
     "gsr_normal_loss_backward": (_int, [_i64] + [_ptr] * 5 + [_i64, _f32] + [_ptr] * 3 + [_size, _ptr]),
     "gsr_anisotropic_loss": (_int, [_i64, _ptr, _f32, _ptr, _ptr, _size, _ptr]),
     "gsr_anisotropic_loss_backward": (_int, [_i64, _ptr, _f32] + [_ptr] * 3),
+    "gsr_depth_loss": (_int, [_i64, _ptr, _i64, _ptr, _i64, _f32, _ptr, _ptr, _size, _ptr]),
+    "gsr_depth_loss_backward": (_int, [_i64, _ptr, _i64, _ptr, _i64, _f32] + [_ptr] * 3 + [_size, _ptr]),
+    "gsr_opacity_loss": (_int, [_i64, _ptr, _i64, _ptr, _ptr, _size, _ptr]),
+    "gsr_opacity_loss_backward": (_int, [_i64] + [_ptr] * 3),
+    "gsr_sparsity_loss": (_int, [_i64, _ptr, _i64, _ptr, _ptr, _size, _ptr]),
+    "gsr_sparsity_loss_backward": (_int, [_i64, _ptr, _i64] + [_ptr] * 3),
+    "gsr_entropy_loss": (_int, [_i64, _ptr, _i64, _ptr, _i64, _ptr, _ptr, _size, _ptr]),
+    "gsr_entropy_loss_backward": (_int, [_i64, _ptr, _i64, _ptr, _i64] + [_ptr] * 3 + [_size, _ptr]),
+    "gsr_density_estimation_loss": (_int, [_i64, _ptr, _i64, _ptr, _i64, _ptr, _i64, _i32, _ptr, _ptr, _size, _ptr]),
+    "gsr_density_estimation_loss_backward": (_int, [_i64, _ptr, _i64, _ptr, _i64, _ptr, _i64, _i32] + [_ptr] * 5),
     "gsr_percentile_low": (_int, [_i64] + [_ptr] * 3 + [_size, _ptr]),
     "gsr_composite": (_int, [_i32] * 2 + [_ptr] * 14),
     "gsr_select_rows_bytes": (_size, [_i64]),

@@ -13,7 +13,12 @@
 //                      selected on the device, mean |n - g| + 0.1 * (-mean n.g); the backward through normalize's Jacobian.
 //   k_aniso_fwd/bwd    anisotropic_loss (LU/:159-168): mean(clamp_min(max / (min + 1e-6), r) - r); the backward sends the max's
 //                      and the min's gradient to the first extreme index, as torch's max(dim) / min(dim) return it on ties.
-//   k_loss_finalize    every mean: per-CTA float partials, then one CTA sums them in double in a fixed order, so a value is
+//   k_depth_sums/fwd/bwd  depth_loss (LU/:65-111): the masked sums of compute_scale_and_shift in double, the 2x2 solve in one
+//                      thread of the finalize (x0, x1 stay on the device), then mean w exp(-p/s) (x0 p + x1 - d)^2 and its gradient.
+//   k_opacity_fwd/bwd  opacity_loss (LU/:143-147) and sparsity_loss (LU/:149-157).
+//   k_entropy_fwd/bwd  the coarse trainers' entropy term over the Gaussians with radii > 0, the visible count on the device.
+//   k_density_fwd/bwd  coarse_density's 'density' SDF estimation loss, |d - exp(-s^2 / (2 beta^2))| or its square.
+//   k_loss_finalize    every mean: per-CTA partials, then one CTA sums them in double in a fixed order, so a value is
 //                      bit-identical from call to call.
 //
 // Elementwise arithmetic uses _rn intrinsics in torch's operation order so nvcc contracts nothing across torch's roundings; the
@@ -39,8 +44,8 @@ struct Strides { int64_t b, c, y, x; };
 size_t align256(size_t n) { return (n + 255) & ~(size_t)255; }
 
 // fixed-order block sum of K values per thread (warp butterflies, then warps in order); the result is valid in thread 0
-template <int K>
-__device__ __forceinline__ void block_sum(float (&v)[K], float (*red)[PB / 32]) {
+template <int K, typename T>
+__device__ __forceinline__ void block_sum(T (&v)[K], T (*red)[PB / 32]) {
 #pragma unroll
     for (int k = 0; k < K; ++k)
 #pragma unroll
@@ -53,7 +58,7 @@ __device__ __forceinline__ void block_sum(float (&v)[K], float (*red)[PB / 32]) 
     if (threadIdx.x == 0)
 #pragma unroll
         for (int k = 0; k < K; ++k) {
-            float s = red[k][0];
+            T s = red[k][0];
             for (int w = 1; w < (int)(blockDim.x >> 5); ++w) s += red[k][w];
             v[k] = s;
         }
@@ -322,10 +327,200 @@ __global__ void __launch_bounds__(RB) k_aniso_bwd(int64_t P, const float* __rest
     }
 }
 
-enum { FIN_PHOTO = 0, FIN_NORMAL = 1, FIN_ANISO = 2 };
+// torch's abs backward: sign(e), 0 at e == 0, NaN stays NaN
+__device__ __forceinline__ float sgn(float e) { return e > 0.f ? 1.0f : e < 0.f ? -1.0f : e == 0.f ? 0.0f : e; }
+
+// ---- depth_loss: d = gt / 25 and -p / scene_scale as torch divides a float32 CUDA tensor by a Python number, x * float32(1 / b)
+constexpr float DEPTH_INV_25 = 1.0f / 25.0f;
+constexpr int RMAX_BLOCKS64 = 256;  // CTAs of the double-partial reduction: 256 x 8 doubles fill GSR_LOSS_REDUCE_BYTES - 256
+
+struct DepthArgs {
+    int64_t n;
+    const float* p;
+    int64_t p_s;
+    const float* gt;
+    int64_t g_s;
+    float inv_scale;
+};
+
+__global__ void __launch_bounds__(RB) k_depth_sums(const DepthArgs a, double* partials) {
+    __shared__ double red[5][PB / 32];
+    double acc[5] = {0.0, 0.0, 0.0, 0.0, 0.0};  // sum p^2, sum p, count, sum p d, sum d over d > 0
+    for (int64_t i = (int64_t)blockIdx.x * RB + threadIdx.x; i < a.n; i += (int64_t)gridDim.x * RB) {
+        const float d = __fmul_rn(a.gt[i * a.g_s], DEPTH_INV_25);
+        if (!(d > 0.0f)) continue;
+        const float p = a.p[i * a.p_s];
+        acc[0] += (double)__fmul_rn(p, p);
+        acc[1] += (double)p;
+        acc[2] += 1.0;
+        acc[3] += (double)__fmul_rn(p, d);
+        acc[4] += (double)d;
+    }
+    block_sum<5>(acc, red);
+    if (threadIdx.x == 0)
+        for (int k = 0; k < 5; ++k) partials[8 * blockIdx.x + k] = acc[k];
+}
+
+// r = x0 p + x1 - d and we = weight * exp(-p / scene_scale), in the reference's operation order
+__device__ __forceinline__ float depth_residual(const DepthArgs& a, int64_t i, float x0, float x1, float& we) {
+    const float p = a.p[i * a.p_s], d = __fmul_rn(a.gt[i * a.g_s], DEPTH_INV_25);
+    we = __fmul_rn(d > 0.0f ? 1.0f : 0.0f, expf(__fmul_rn(-p, a.inv_scale)));
+    return __fsub_rn(__fadd_rn(__fmul_rn(x0, p), x1), d);
+}
+
+__global__ void __launch_bounds__(RB) k_depth_fwd(const DepthArgs a, const float* x, float* partials) {
+    __shared__ float red[1][PB / 32];
+    const float x0 = x[0], x1 = x[1];
+    float acc[1] = {0.f};
+    for (int64_t i = (int64_t)blockIdx.x * RB + threadIdx.x; i < a.n; i += (int64_t)gridDim.x * RB) {
+        float we;
+        const float r = depth_residual(a, i, x0, x1, we);
+        acc[0] += __fmul_rn(we, __fmul_rn(r, r));
+    }
+    block_sum<1>(acc, red);
+    if (threadIdx.x == 0) partials[4 * blockIdx.x] = acc[0];
+}
+
+// d p = (g / n) * we * (2 r) * x0: the scale, the shift and the exp factor are detached in the reference
+__global__ void __launch_bounds__(RB) k_depth_bwd(const DepthArgs a, const float* x, const float* g_out, float* __restrict__ d_p) {
+    const float x0 = x[0], x1 = x[1];
+    const float g = (float)((double)*g_out / (double)a.n);
+    for (int64_t i = (int64_t)blockIdx.x * RB + threadIdx.x; i < a.n; i += (int64_t)gridDim.x * RB) {
+        float we;
+        const float r = depth_residual(a, i, x0, x1, we);
+        d_p[i] = __fmul_rn(__fmul_rn(__fmul_rn(g, we), __fmul_rn(2.0f, r)), x0);
+    }
+}
+
+// ---- opacity_loss: mean(x); sparsity_loss: mean(log c + log(1 - c)), c = clamp(x, 1e-3, 1 - 1e-3) with float32 bounds
+constexpr float SPARSE_LO = 1e-3f;
+constexpr float SPARSE_HI = (float)(1.0 - 1e-3);
+
+__device__ __forceinline__ float sparsity_term(float x) {
+    const float c = x != x ? x : fminf(fmaxf(x, SPARSE_LO), SPARSE_HI);  // clamp keeps NaN
+    return __fadd_rn(logf(c), logf(__fsub_rn(1.0f, c)));
+}
+
+template <bool SPARSE>
+__global__ void __launch_bounds__(RB) k_opacity_fwd(int64_t n, const float* __restrict__ x, int64_t xs, float* partials) {
+    __shared__ float red[1][PB / 32];
+    float acc[1] = {0.f};
+    for (int64_t i = (int64_t)blockIdx.x * RB + threadIdx.x; i < n; i += (int64_t)gridDim.x * RB) {
+        const float v = x[i * xs];
+        acc[0] += SPARSE ? sparsity_term(v) : v;
+    }
+    block_sum<1>(acc, red);
+    if (threadIdx.x == 0) partials[4 * blockIdx.x] = acc[0];
+}
+
+// opacity: dx = g / n; sparsity: g / c - g / (1 - c) where 1e-3 <= x <= 1 - 1e-3 (clamp's backward passes both bounds), else 0
+template <bool SPARSE>
+__global__ void __launch_bounds__(RB) k_opacity_bwd(int64_t n, const float* __restrict__ x, int64_t xs, const float* g_out,
+                                                    float* __restrict__ dx) {
+    const float g = (float)((double)*g_out / (double)n);
+    for (int64_t i = (int64_t)blockIdx.x * RB + threadIdx.x; i < n; i += (int64_t)gridDim.x * RB) {
+        if (!SPARSE) {
+            dx[i] = g;
+            continue;
+        }
+        const float c = x[i * xs];
+        dx[i] = c >= SPARSE_LO && c <= SPARSE_HI ? __fsub_rn(__fdiv_rn(g, c), __fdiv_rn(g, __fsub_rn(1.0f, c))) : 0.0f;
+    }
+}
+
+// ---- entropy: -o log(o + 1e-10) - (1 - o) log(1 - o + 1e-10) over the Gaussians with radii > 0
+constexpr float ENTROPY_EPS = 1e-10f;
+
+__global__ void __launch_bounds__(RB) k_entropy_fwd(int64_t P, const float* __restrict__ o, int64_t os, const int32_t* __restrict__ radii,
+                                                    int64_t rs, float* partials) {
+    __shared__ float red[2][PB / 32];
+    float acc[2] = {0.f, 0.f};  // sum of the terms, visible count
+    for (int64_t i = (int64_t)blockIdx.x * RB + threadIdx.x; i < P; i += (int64_t)gridDim.x * RB) {
+        if (radii[i * rs] <= 0) continue;
+        const float v = o[i * os], u = __fsub_rn(1.0f, v);
+        acc[0] += __fsub_rn(__fmul_rn(-v, logf(__fadd_rn(v, ENTROPY_EPS))), __fmul_rn(u, logf(__fadd_rn(u, ENTROPY_EPS))));
+        acc[1] += 1.0f;
+    }
+    block_sum<2>(acc, red);
+    if (threadIdx.x == 0) {
+        partials[4 * blockIdx.x] = acc[0];
+        partials[4 * blockIdx.x + 1] = acc[1];
+    }
+}
+
+// torch's chain: -(g L1) + g (-o) / (o + eps) - ((-g) L2 + (-g) u / (u + eps)) with u = 1 - o; 0 where radii <= 0
+__global__ void __launch_bounds__(RB) k_entropy_bwd(int64_t P, const float* __restrict__ o, int64_t os, const int32_t* __restrict__ radii,
+                                                    int64_t rs, const double* totals, const float* g_out, float* __restrict__ d_o) {
+    const float g = (float)((double)*g_out / totals[1]);
+    for (int64_t i = (int64_t)blockIdx.x * RB + threadIdx.x; i < P; i += (int64_t)gridDim.x * RB) {
+        float d = 0.0f;
+        if (radii[i * rs] > 0) {
+            const float v = o[i * os], u = __fsub_rn(1.0f, v);
+            const float e1 = __fadd_rn(v, ENTROPY_EPS), e2 = __fadd_rn(u, ENTROPY_EPS);
+            const float t1 = __fadd_rn(-__fmul_rn(g, logf(e1)), __fdiv_rn(__fmul_rn(g, -v), e1));
+            const float t2 = __fadd_rn(__fmul_rn(-g, logf(e2)), __fdiv_rn(__fmul_rn(-g, u), e2));
+            d = __fsub_rn(t1, t2);
+        }
+        d_o[i] = d;
+    }
+}
+
+// ---- density-mode SDF estimation: e = d - exp(-0.5 s^2 / beta^2), mean |e| or mean e^2
+struct DensityArgs {
+    int64_t n;
+    const float* d;
+    int64_t d_s;
+    const float* b;
+    int64_t b_s;
+    const float* s;
+    int64_t s_s;
+    int squared;
+};
+
+// the reference's expression with one rounding per torch op; t = exp(q), q = (-0.5 s^2) / beta^2, b2 = beta^2
+__device__ __forceinline__ float density_error(const DensityArgs& a, int64_t i, float& t, float& q, float& b2) {
+    const float s = a.s[i * a.s_s], beta = a.b[i * a.b_s];
+    b2 = __fmul_rn(beta, beta);
+    q = __fdiv_rn(__fmul_rn(-0.5f, __fmul_rn(s, s)), b2);
+    t = expf(q);
+    return __fsub_rn(a.d[i * a.d_s], t);
+}
+
+__global__ void __launch_bounds__(RB) k_density_fwd(const DensityArgs a, float* partials) {
+    __shared__ float red[1][PB / 32];
+    float acc[1] = {0.f};
+    for (int64_t i = (int64_t)blockIdx.x * RB + threadIdx.x; i < a.n; i += (int64_t)gridDim.x * RB) {
+        float t, q, b2;
+        const float e = density_error(a, i, t, q, b2);
+        acc[0] += a.squared ? __fmul_rn(e, e) : fabsf(e);
+    }
+    block_sum<1>(acc, red);
+    if (threadIdx.x == 0) partials[4 * blockIdx.x] = acc[0];
+}
+
+// torch's backward chain through pow(2) or abs, the subtraction, exp, the division ((-g q') / b2 and -g q' * (q / b2)), the -0.5
+// factor and the two pow(2)s; sgn(0) = 0 makes every gradient of that sample zero, as in torch
+__global__ void __launch_bounds__(RB) k_density_bwd(const DensityArgs a, const float* g_out, float* __restrict__ d_d,
+                                                    float* __restrict__ d_b, float* __restrict__ d_s) {
+    const float g = (float)((double)*g_out / (double)a.n);
+    for (int64_t i = (int64_t)blockIdx.x * RB + threadIdx.x; i < a.n; i += (int64_t)gridDim.x * RB) {
+        float t, q, b2;
+        const float e = density_error(a, i, t, q, b2);
+        const float ge = a.squared ? __fmul_rn(g, __fmul_rn(2.0f, e)) : __fmul_rn(g, sgn(e));
+        const float gq = __fmul_rn(-ge, t);
+        const float gb2 = __fmul_rn(-gq, __fdiv_rn(q, b2));
+        const float gs2 = __fmul_rn(__fdiv_rn(gq, b2), -0.5f);
+        d_d[i] = ge;
+        d_s[i] = __fmul_rn(gs2, __fmul_rn(2.0f, a.s[i * a.s_s]));
+        d_b[i] = __fmul_rn(gb2, __fmul_rn(2.0f, a.b[i * a.b_s]));
+    }
+}
+
+enum { FIN_PHOTO = 0, FIN_NORMAL = 1, FIN_MEAN = 2, FIN_RATIO = 3, FIN_DEPTH_SOLVE = 4 };
 
 // one CTA: totals[k] = sum of partials[blk * stride + k] in double, thread-strided then tree order; then the mode's means
-__global__ void __launch_bounds__(RB) k_loss_finalize(int mode, const float* partials, int64_t blocks, int stride, int K, double n,
+template <typename T>
+__global__ void __launch_bounds__(RB) k_loss_finalize(int mode, const T* partials, int64_t blocks, int stride, int K, double n,
                                                       double* totals, float* out, float* out2) {
     __shared__ double sh[RB];
     for (int k = 0; k < K; ++k) {
@@ -347,6 +542,19 @@ __global__ void __launch_bounds__(RB) k_loss_finalize(int mode, const float* par
     } else if (mode == FIN_NORMAL) {  // l1 + 0.1 * cos, an empty selection is 0 / 0 = NaN as torch's mean of nothing
         const float l1 = (float)(totals[0] / (3.0 * totals[2])), cos = -(float)(totals[1] / totals[2]);
         out[0] = __fadd_rn(l1, __fmul_rn(0.1f, cos));
+    } else if (mode == FIN_RATIO) {  // sum / count; no counted element is 0 / 0 = NaN
+        out[0] = (float)(totals[0] / totals[1]);
+    } else if (mode == FIN_DEPTH_SOLVE) {  // compute_scale_and_shift (LU/:65-92) on the sums rounded to float32, torch's order
+        const float a00 = (float)totals[0], a01 = (float)totals[1], a11 = (float)totals[2];
+        const float b0 = (float)totals[3], b1 = (float)totals[4];
+        const float det = __fsub_rn(__fmul_rn(a00, a11), __fmul_rn(a01, a01));
+        float x0 = __int_as_float(0x7fffffff), x1 = x0;  // det == 0: the reference fails; NaN here (INTEGRATION.md)
+        if (det != 0.0f) {
+            x0 = __fdiv_rn(__fsub_rn(__fmul_rn(a11, b0), __fmul_rn(a01, b1)), det);
+            x1 = __fdiv_rn(__fadd_rn(__fmul_rn(-a01, b0), __fmul_rn(a00, b1)), det);
+        }
+        out[0] = x0;
+        out[1] = x1;
     } else {
         out[0] = (float)(totals[0] / n);
     }
@@ -502,7 +710,7 @@ int gsr_anisotropic_loss(int64_t P, const float* scales, float r, float* out, vo
     const int blocks = reduce_blocks(P);
     float* partials = (float*)((char*)ws + 256);
     k_aniso_fwd<<<blocks, RB, 0, st>>>(P, scales, r, partials);
-    k_loss_finalize<<<1, RB, 0, st>>>(FIN_ANISO, partials, blocks, 4, 1, (double)P, (double*)ws, out, nullptr);
+    k_loss_finalize<<<1, RB, 0, st>>>(FIN_MEAN, partials, blocks, 4, 1, (double)P, (double*)ws, out, nullptr);
     return check_launch("gsr_anisotropic_loss", false, st);
 }
 
@@ -515,4 +723,155 @@ int gsr_anisotropic_loss_backward(int64_t P, const float* scales, float r, const
     }
     k_aniso_bwd<<<reduce_blocks(P), RB, 0, st>>>(P, scales, r, g_out, d_scales);
     return check_launch("gsr_anisotropic_loss_backward", false, st);
+}
+
+int gsr_depth_loss(int64_t n, const float* pred, int64_t pred_stride, const float* gt, int64_t gt_stride, float scene_scale_inv,
+                   float* out, void* ws, size_t ws_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_depth_loss");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (n <= 0 || !pred || !gt || !out) {
+        set_error("gsr_depth_loss: bad arguments (n %lld)", (long long)n);
+        return GSR_ERR_INVALID;
+    }
+    const int rc = check_reduce_ws("gsr_depth_loss", ws, ws_bytes);
+    if (rc != GSR_OK) return rc;
+    const DepthArgs a{n, pred, pred_stride, gt, gt_stride, scene_scale_inv};
+    double* totals = (double*)ws;
+    float* x = (float*)((char*)ws + 128);
+    void* partials = (char*)ws + 256;
+    const int blocks = reduce_blocks(n), b64 = blocks < RMAX_BLOCKS64 ? blocks : RMAX_BLOCKS64;
+    k_depth_sums<<<b64, RB, 0, st>>>(a, (double*)partials);
+    k_loss_finalize<<<1, RB, 0, st>>>(FIN_DEPTH_SOLVE, (const double*)partials, b64, 8, 5, (double)n, totals, x, nullptr);
+    k_depth_fwd<<<blocks, RB, 0, st>>>(a, x, (float*)partials);
+    k_loss_finalize<<<1, RB, 0, st>>>(FIN_MEAN, (const float*)partials, blocks, 4, 1, (double)n, totals, out, nullptr);
+    return check_launch("gsr_depth_loss", false, st);
+}
+
+int gsr_depth_loss_backward(int64_t n, const float* pred, int64_t pred_stride, const float* gt, int64_t gt_stride,
+                            float scene_scale_inv, const float* g_out, float* d_pred, const void* ws, size_t ws_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_depth_loss_backward");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (n <= 0 || !pred || !gt || !g_out || !d_pred) {
+        set_error("gsr_depth_loss_backward: bad arguments (n %lld)", (long long)n);
+        return GSR_ERR_INVALID;
+    }
+    const int rc = check_reduce_ws("gsr_depth_loss_backward", ws, ws_bytes);
+    if (rc != GSR_OK) return rc;
+    const DepthArgs a{n, pred, pred_stride, gt, gt_stride, scene_scale_inv};
+    k_depth_bwd<<<reduce_blocks(n), RB, 0, st>>>(a, (const float*)((const char*)ws + 128), g_out, d_pred);
+    return check_launch("gsr_depth_loss_backward", false, st);
+}
+
+static int opacity_fwd(const char* who, bool sparse, int64_t n, const float* x, int64_t xs, float* out, void* ws, size_t ws_bytes,
+                       cudaStream_t st) {
+    if (n <= 0 || !x || !out) {
+        set_error("%s: bad arguments (n %lld)", who, (long long)n);
+        return GSR_ERR_INVALID;
+    }
+    const int rc = check_reduce_ws(who, ws, ws_bytes);
+    if (rc != GSR_OK) return rc;
+    const int blocks = reduce_blocks(n);
+    float* partials = (float*)((char*)ws + 256);
+    if (sparse)
+        k_opacity_fwd<true><<<blocks, RB, 0, st>>>(n, x, xs, partials);
+    else
+        k_opacity_fwd<false><<<blocks, RB, 0, st>>>(n, x, xs, partials);
+    k_loss_finalize<<<1, RB, 0, st>>>(FIN_MEAN, (const float*)partials, blocks, 4, 1, (double)n, (double*)ws, out, nullptr);
+    return check_launch(who, false, st);
+}
+
+int gsr_opacity_loss(int64_t n, const float* x, int64_t x_stride, float* out, void* ws, size_t ws_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_opacity_loss");
+    return opacity_fwd("gsr_opacity_loss", false, n, x, x_stride, out, ws, ws_bytes, (cudaStream_t)stream);
+}
+
+int gsr_opacity_loss_backward(int64_t n, const float* g_out, float* dx, void* stream) {
+    NvtxRange nvtx_("gsr_opacity_loss_backward");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (n <= 0 || !g_out || !dx) {
+        set_error("gsr_opacity_loss_backward: bad arguments (n %lld)", (long long)n);
+        return GSR_ERR_INVALID;
+    }
+    k_opacity_bwd<false><<<reduce_blocks(n), RB, 0, st>>>(n, nullptr, 0, g_out, dx);
+    return check_launch("gsr_opacity_loss_backward", false, st);
+}
+
+int gsr_sparsity_loss(int64_t n, const float* x, int64_t x_stride, float* out, void* ws, size_t ws_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_sparsity_loss");
+    return opacity_fwd("gsr_sparsity_loss", true, n, x, x_stride, out, ws, ws_bytes, (cudaStream_t)stream);
+}
+
+int gsr_sparsity_loss_backward(int64_t n, const float* x, int64_t x_stride, const float* g_out, float* dx, void* stream) {
+    NvtxRange nvtx_("gsr_sparsity_loss_backward");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (n <= 0 || !x || !g_out || !dx) {
+        set_error("gsr_sparsity_loss_backward: bad arguments (n %lld)", (long long)n);
+        return GSR_ERR_INVALID;
+    }
+    k_opacity_bwd<true><<<reduce_blocks(n), RB, 0, st>>>(n, x, x_stride, g_out, dx);
+    return check_launch("gsr_sparsity_loss_backward", false, st);
+}
+
+int gsr_entropy_loss(int64_t P, const float* opacities, int64_t o_stride, const int32_t* radii, int64_t r_stride, float* out, void* ws,
+                     size_t ws_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_entropy_loss");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (P <= 0 || !opacities || !radii || !out) {
+        set_error("gsr_entropy_loss: bad arguments (P %lld)", (long long)P);
+        return GSR_ERR_INVALID;
+    }
+    const int rc = check_reduce_ws("gsr_entropy_loss", ws, ws_bytes);
+    if (rc != GSR_OK) return rc;
+    const int blocks = reduce_blocks(P);
+    float* partials = (float*)((char*)ws + 256);
+    k_entropy_fwd<<<blocks, RB, 0, st>>>(P, opacities, o_stride, radii, r_stride, partials);
+    k_loss_finalize<<<1, RB, 0, st>>>(FIN_RATIO, (const float*)partials, blocks, 4, 2, (double)P, (double*)ws, out, nullptr);
+    return check_launch("gsr_entropy_loss", false, st);
+}
+
+int gsr_entropy_loss_backward(int64_t P, const float* opacities, int64_t o_stride, const int32_t* radii, int64_t r_stride,
+                              const float* g_out, float* d_opacities, const void* ws, size_t ws_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_entropy_loss_backward");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (P <= 0 || !opacities || !radii || !g_out || !d_opacities) {
+        set_error("gsr_entropy_loss_backward: bad arguments (P %lld)", (long long)P);
+        return GSR_ERR_INVALID;
+    }
+    const int rc = check_reduce_ws("gsr_entropy_loss_backward", ws, ws_bytes);
+    if (rc != GSR_OK) return rc;
+    k_entropy_bwd<<<reduce_blocks(P), RB, 0, st>>>(P, opacities, o_stride, radii, r_stride, (const double*)ws, g_out, d_opacities);
+    return check_launch("gsr_entropy_loss_backward", false, st);
+}
+
+int gsr_density_estimation_loss(int64_t n, const float* density, int64_t d_stride, const float* beta, int64_t b_stride,
+                                const float* sdf_estimation, int64_t s_stride, int32_t squared, float* out, void* ws, size_t ws_bytes,
+                                void* stream) {
+    NvtxRange nvtx_("gsr_density_estimation_loss");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (n <= 0 || !density || !beta || !sdf_estimation || !out) {
+        set_error("gsr_density_estimation_loss: bad arguments (n %lld)", (long long)n);
+        return GSR_ERR_INVALID;
+    }
+    const int rc = check_reduce_ws("gsr_density_estimation_loss", ws, ws_bytes);
+    if (rc != GSR_OK) return rc;
+    const DensityArgs a{n, density, d_stride, beta, b_stride, sdf_estimation, s_stride, squared != 0};
+    const int blocks = reduce_blocks(n);
+    float* partials = (float*)((char*)ws + 256);
+    k_density_fwd<<<blocks, RB, 0, st>>>(a, partials);
+    k_loss_finalize<<<1, RB, 0, st>>>(FIN_MEAN, (const float*)partials, blocks, 4, 1, (double)n, (double*)ws, out, nullptr);
+    return check_launch("gsr_density_estimation_loss", false, st);
+}
+
+int gsr_density_estimation_loss_backward(int64_t n, const float* density, int64_t d_stride, const float* beta, int64_t b_stride,
+                                         const float* sdf_estimation, int64_t s_stride, int32_t squared, const float* g_out,
+                                         float* d_density, float* d_beta, float* d_sdf_estimation, void* stream) {
+    NvtxRange nvtx_("gsr_density_estimation_loss_backward");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (n <= 0 || !density || !beta || !sdf_estimation || !g_out || !d_density || !d_beta || !d_sdf_estimation) {
+        set_error("gsr_density_estimation_loss_backward: bad arguments (n %lld)", (long long)n);
+        return GSR_ERR_INVALID;
+    }
+    const DensityArgs a{n, density, d_stride, beta, b_stride, sdf_estimation, s_stride, squared != 0};
+    k_density_bwd<<<reduce_blocks(n), RB, 0, st>>>(a, g_out, d_density, d_beta, d_sdf_estimation);
+    return check_launch("gsr_density_estimation_loss_backward", false, st);
 }

@@ -28,6 +28,13 @@ estimation loss :689-712) runs through ``gsr_sugar_surface_mask`` and ``gsr_suga
     loss = loss + sdf_estimation_factor * depth_sdf_estimation_loss(sugar, fov_camera, depth, sdf_samples, fields['sdf'],
                                                                     sdf_sample_std, 10. * sugar.get_cameras_spatial_extent())
 
+coarse_density's 'density' SDF estimation loss ("CD/" :735-741, the same at coarse_sdf.py:714-720) runs through
+``gsr_density_estimation_loss`` / ``..._backward`` when ``proj_mask`` is all true (use_projection_as_estimation, the default)::
+
+    from autovfx_b200.sugar_field import density_estimation_loss
+    loss = loss + sdf_estimation_factor * density_estimation_loss(fields['density'], fields['beta'], sdf_estimation,
+                                                                  squared_sdf_estimation_loss)
+
 The model is read through its getters (``points``, ``scaling``, ``quaternions``, ``strengths``, ``knn_idx``, ``beta_mode``), so
 autograd carries the gradients of x and of the getters' outputs back to the raw parameters.  No [N,K,3,3] tensor is built: the
 kernels gather one 64-byte record per (sample, neighbour) pair and recompute everything in the backward.
@@ -40,7 +47,7 @@ import torch
 from . import _lib
 
 __all__ = ["get_field_values", "compute_density", "projection_estimate", "better_normal_loss", "sample_points_in_gaussians",
-           "close_to_surface_mask", "depth_sdf_estimation_loss", "FIELD_MAX_K"]
+           "close_to_surface_mask", "depth_sdf_estimation_loss", "density_estimation_loss", "FIELD_MAX_K"]
 
 FIELD_MAX_K = 32
 
@@ -628,3 +635,77 @@ def depth_sdf_estimation_loss(self, fov_camera, depth, sdf_samples, sdf_values, 
         if torch.is_grad_enabled() and any(t.requires_grad for t in (x, depth, sdf)):
             return _DepthSdfLoss.apply(x, depth, sdf, cam, cfg)
         return _depth_loss_forward(cfg, x, depth, sdf, cam)[0]
+
+
+# ------------------------------------------------------------------------------------- coarse_density's density-mode estimation loss
+def _density_loss_forward(n, views, squared):
+    (d, ds), (b, bs), (e, es) = views
+    dev = d.device
+    out = torch.empty((), dtype=torch.float32, device=dev)
+    ws = torch.empty(_lib.GSR_LOSS_REDUCE_BYTES, dtype=torch.uint8, device=dev)
+    rc = _lib_handle().gsr_density_estimation_loss(n, d.data_ptr(), ds, b.data_ptr(), bs, e.data_ptr(), es, int(squared), out.data_ptr(),
+                                                   ws.data_ptr(), ws.numel(), _lib.stream_ptr(dev))
+    _lib.check(rc, "gsr_density_estimation_loss")
+    return out
+
+
+def _flat(t):
+    v = t.reshape(-1)
+    return v, v.stride(0)
+
+
+class _DensityLoss(torch.autograd.Function):
+    """One output: the 0-dim mean; differentiable with respect to the densities, beta and the SDF estimate."""
+
+    @staticmethod
+    def forward(ctx, densities, beta, sdf_estimation, squared):
+        ctx.set_materialize_grads(False)
+        ctx.squared = squared
+        ctx.save_for_backward(densities, beta, sdf_estimation)
+        return _density_loss_forward(densities.numel(), [_flat(t) for t in (densities, beta, sdf_estimation)], squared)
+
+    @staticmethod
+    def backward(ctx, g):
+        if g is None:
+            return None, None, None, None
+        ins = ctx.saved_tensors
+        (d, ds), (b, bs), (e, es) = [_flat(t) for t in ins]
+        dev, n = d.device, d.numel()
+        grads = [torch.empty(t.shape, dtype=torch.float32, device=dev) for t in ins]
+        g = g.detach().reshape(1).to(dtype=torch.float32).contiguous()
+        rc = _lib_handle().gsr_density_estimation_loss_backward(n, d.data_ptr(), ds, b.data_ptr(), bs, e.data_ptr(), es, int(ctx.squared),
+                                                                g.data_ptr(), *[t.data_ptr() for t in grads], _lib.stream_ptr(dev))
+        _lib.check(rc, "gsr_density_estimation_loss_backward")
+        return tuple(t if need else None for t, need in zip(grads, ctx.needs_input_grad[:3])) + (None,)
+
+
+def density_estimation_loss(densities, beta, sdf_estimation, squared=False):
+    """coarse_density's 'density' SDF estimation loss (CD/:735-741, coarse_sdf.py:714-720) when proj_mask is all true, before the
+    trainer's sdf_estimation_factor: ``mean(|densities - exp(-0.5 * sdf_estimation ** 2 / beta ** 2)|)``, or the mean of its
+    square with ``squared`` (squared_sdf_estimation_loss).  ``densities`` and ``beta`` are get_field_values' 'density' and 'beta',
+    ``sdf_estimation`` projection_estimate's output: three float32 tensors of one shape, any strides.  The gradient goes to all
+    three through torch's own chain, so a sample whose density equals its target gets a zero gradient in all three (torch's
+    sign(0)).  Nothing is read back to the host, where the reference's ``[proj_mask]`` indexing synchronises twice per step.  With
+    use_projection_as_estimation = False the caller still indexes the three tensors with proj_mask first.
+
+    Raises ValueError, naming the argument, for a wrong dtype, a shape mismatch, an empty input or mixed devices; RuntimeError for
+    CPU tensors (there is no CPU path)."""
+    who = "density_estimation_loss"
+    names = ("densities", "beta", "sdf_estimation")
+    ts = (densities, beta, sdf_estimation)
+    for name, t in zip(names, ts):
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.float32:
+            raise ValueError("%s: %s must be a float32 tensor, got %s" % (who, name, getattr(t, "dtype", type(t).__name__)))
+    for name, t in zip(names[1:], ts[1:]):
+        if t.shape != densities.shape:
+            raise ValueError("%s: %s has shape %s, densities %s" % (who, name, tuple(t.shape), tuple(densities.shape)))
+    if densities.numel() == 0:
+        raise ValueError("%s: densities is empty (shape %s)" % (who, tuple(densities.shape)))
+    for name, t in zip(names[1:], ts[1:]):
+        if t.device != densities.device:
+            raise ValueError("%s: %s is on %s, densities on %s" % (who, name, t.device, densities.device))
+    _require_cuda(who, *ts)
+    with torch.cuda.device(densities.device):
+        if torch.is_grad_enabled() and any(t.requires_grad for t in ts):
+            return _DensityLoss.apply(densities, beta, sdf_estimation, bool(squared))
+        return _density_loss_forward(densities.numel(), [_flat(t) for t in ts], bool(squared))

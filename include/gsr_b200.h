@@ -28,6 +28,10 @@
  *                               coarse_density.py:550-590, scene_representation.py:513-515); gsr_photometric_loss_backward their autograd
  *   gsr_normal_loss   replaces  normal_loss                                       GS/utils/loss_utils.py:118-132; gsr_normal_loss_backward
  *   gsr_anisotropic_loss replaces anisotropic_loss                                GS/utils/loss_utils.py:159-168; gsr_anisotropic_loss_backward
+ *   gsr_depth_loss    replaces  depth_loss (compute_scale_and_shift)              GS/utils/loss_utils.py:65-111; gsr_depth_loss_backward
+ *   gsr_opacity_loss, gsr_sparsity_loss replace opacity_loss, sparsity_loss      GS/utils/loss_utils.py:143-157; their _backward
+ *   gsr_entropy_loss  replaces  the coarse trainers' opacity entropy term          sugar_trainers/coarse_density.py:598-606; its _backward
+ *   gsr_density_estimation_loss replaces coarse_density's 'density' SDF estimation loss  coarse_density.py:735-741; its _backward
  *   gsr_percentile_low replaces np.percentile(smoke_depth, 0.001)                blender/blend_all.py:206-208
  *   gsr_composite     replaces  the per-frame compositing of blend_frames          blender/blend_all.py:236-342
  *   gsr_select_rows   replaces  the deepcopy + boolean indexing of each candidate subset  extract/extract_object.py:196-202, :315-321
@@ -614,7 +618,7 @@ int gsr_adam_step(int32_t n, const gsr_adam_tensor* tensors, void* stream);
 /* The training objective's terms (gsr_loss.cu).  Every value is a float32 device scalar written by the call; every mean is a
  * fixed-order reduction (per-CTA float partials, one ordered double sum), bit-identical from call to call.  Upstream gradients are
  * device pointers, so nothing synchronises with the host. */
-#define GSR_LOSS_REDUCE_BYTES (256 + 16 * 1024) /* the workspace of gsr_normal_loss[_backward] and gsr_anisotropic_loss              */
+#define GSR_LOSS_REDUCE_BYTES (256 + 16 * 1024) /* the workspace of every reduction term below but gsr_photometric_loss               */
 
 /* Workspace of gsr_photometric_loss for [B,C,H,W] images: the partial sums, and with for_backward != 0 three float maps of
  * B*C*H*W.  0 for an empty or oversized shape (B*C >= 65536). */
@@ -651,6 +655,47 @@ int gsr_anisotropic_loss(int64_t P, const float* scales, float r, float* out, vo
 /* d_scales [P,3] = g_out[0] * d out / d scales: the max's and the min's gradient go to the first extreme index (NaN first), as
  * torch's max(dim) / min(dim) return it; nothing where the ratio is below r (clamp_min passes ratio == r).  One thread per Gaussian. */
 int gsr_anisotropic_loss_backward(int64_t P, const float* scales, float r, const float* g_out, float* d_scales, void* stream);
+/* depth_loss over n pixels of pred (the rendered depth) and gt (the monocular depth), each by one element stride.  With
+ * d = gt * float32(1 / 25) and the mask d > 0, the five masked sums (p^2, p, count, p d, d) are accumulated in double in a fixed
+ * order and rounded to float32; x0 (scale) and x1 (shift) solve the 2x2 system with torch's operation order in one thread and stay
+ * in `workspace`.  out[0] = mean over all n of w * exp(-p * scene_scale_inv) * (x0 p + x1 - d)^2, w = 1 on the mask, else 0;
+ * scene_scale_inv is float32(1 / float32(scene_scale)), as torch divides by a Python number.  det == 0 (an empty mask included)
+ * gives x0 = x1 = NaN, so the value and every gradient are NaN.  `workspace` (16-byte aligned) needs GSR_LOSS_REDUCE_BYTES. */
+int gsr_depth_loss(int64_t n, const float* pred, int64_t pred_stride, const float* gt, int64_t gt_stride, float scene_scale_inv,
+                   float* out, void* workspace, size_t workspace_bytes, void* stream);
+/* d_pred (contiguous [n]) = g_out[0] / n * w exp(-p s^-1) * 2 (x0 p + x1 - d) * x0; the scale, the shift and the exp factor are
+ * constants, as the reference detaches them.  `workspace` is the forward's (it holds x0 and x1). */
+int gsr_depth_loss_backward(int64_t n, const float* pred, int64_t pred_stride, const float* gt, int64_t gt_stride,
+                            float scene_scale_inv, const float* g_out, float* d_pred, const void* workspace, size_t workspace_bytes,
+                            void* stream);
+/* out[0] = mean of n values x[i * x_stride].  `workspace` (16-byte aligned) needs GSR_LOSS_REDUCE_BYTES. */
+int gsr_opacity_loss(int64_t n, const float* x, int64_t x_stride, float* out, void* workspace, size_t workspace_bytes, void* stream);
+/* dx (contiguous [n]) = g_out[0] / n. */
+int gsr_opacity_loss_backward(int64_t n, const float* g_out, float* dx, void* stream);
+/* out[0] = mean of log c + log(1 - c), c = clamp(x, 1e-3, 1 - 1e-3) with the bounds rounded to float32.  `workspace` as above. */
+int gsr_sparsity_loss(int64_t n, const float* x, int64_t x_stride, float* out, void* workspace, size_t workspace_bytes, void* stream);
+/* dx (contiguous [n]) = g_out[0] / n * (1 / c - 1 / (1 - c)) where 1e-3 <= x <= 1 - 1e-3 (both bounds pass, as torch's clamp
+ * backward), else 0. */
+int gsr_sparsity_loss_backward(int64_t n, const float* x, int64_t x_stride, const float* g_out, float* dx, void* stream);
+/* out[0] = mean over the P Gaussians with radii[i * r_stride] > 0 of -o log(o + 1e-10) - (1 - o) log(1 - o + 1e-10),
+ * o = opacities[i * o_stride]; the visible count stays in `workspace` (16-byte aligned, GSR_LOSS_REDUCE_BYTES).  No visible
+ * Gaussian gives NaN, as torch's mean of an empty tensor. */
+int gsr_entropy_loss(int64_t P, const float* opacities, int64_t o_stride, const int32_t* radii, int64_t r_stride, float* out,
+                     void* workspace, size_t workspace_bytes, void* stream);
+/* d_opacities (contiguous [P]) = g_out[0] / count * d term / d o on the visible Gaussians, 0 elsewhere.  `workspace` is the
+ * forward's. */
+int gsr_entropy_loss_backward(int64_t P, const float* opacities, int64_t o_stride, const int32_t* radii, int64_t r_stride,
+                              const float* g_out, float* d_opacities, const void* workspace, size_t workspace_bytes, void* stream);
+/* out[0] = mean over n samples of |d - exp(-0.5 s^2 / beta^2)| (squared != 0: its square), d = density, s = sdf_estimation, each
+ * by one element stride, with one float32 rounding per torch op.  `workspace` (16-byte aligned) needs GSR_LOSS_REDUCE_BYTES. */
+int gsr_density_estimation_loss(int64_t n, const float* density, int64_t d_stride, const float* beta, int64_t b_stride,
+                                const float* sdf_estimation, int64_t s_stride, int32_t squared, float* out, void* workspace,
+                                size_t workspace_bytes, void* stream);
+/* The three gradients (contiguous [n] each) = g_out[0] * d out / d (density, beta, sdf_estimation), by torch's backward chain:
+ * the abs's gradient is 0 where d equals its target, and then so are the other two. */
+int gsr_density_estimation_loss_backward(int64_t n, const float* density, int64_t d_stride, const float* beta, int64_t b_stride,
+                                         const float* sdf_estimation, int64_t s_stride, int32_t squared, const float* g_out,
+                                         float* d_density, float* d_beta, float* d_sdf_estimation, void* stream);
 
 /* Frame compositing (gsr_composite.cu), bit-identical to blender/blend_all.py:blend_frames on the same decoded arrays. */
 #define GSR_PERCENTILE_BYTES 2048 /* the workspace of gsr_percentile_low */
