@@ -173,6 +173,11 @@ SIGNATURES = {
     "gsr_png_bound": (_size, [_i32] * 3),
     "gsr_png_workspace_bytes": (_size, [_i32, C.POINTER(gsr_png_image)]),
     "gsr_png_encode": (_int, [C.POINTER(gsr_png_image), _i32, C.POINTER(C.c_void_p), _ptr, _ptr, _size, _ptr]),
+    "gsr_mesh_bvh_bytes": (_size, [_i32]),
+    "gsr_mesh_build_bytes": (_size, [_i32]),
+    "gsr_mesh_build": (_int, [_i64, _i32] + [_ptr] * 3 + [_size, _ptr, _size, _ptr]),
+    "gsr_mesh_first_hit": (_int, [_i32, _ptr, _i64, _ptr, _ptr, _i32] + [_ptr] * 4),
+    "gsr_mesh_inpaint_mask": (_int, [_i64, _ptr, _ptr, _i32] + [_ptr] * 8),
     "gsr_get_views": (_int, [_ws, _i32, _i32, _i32, C.POINTER(gsr_views)]),
     "gsr_profile_begin": (_int, [_int]),
     "gsr_profile_begin_strided": (_int, [_int, _int]),

@@ -757,6 +757,29 @@ size_t gsr_png_workspace_bytes(int32_t n, const gsr_png_image* images);
 int gsr_png_encode(const gsr_png_image* images, int32_t n, uint8_t* const* outputs, int64_t* sizes, void* workspace, size_t workspace_bytes,
                    void* stream);
 
+/* ---- first-hit ray casts against a triangle mesh (gsr_mesh.cu): an LBVH over F triangles, DESIGN.md §4 ---- */
+/* Bytes of the BVH buffer of F triangles (float32 boxes, float64 triangles in leaf order), and of gsr_mesh_build's scratch. */
+size_t gsr_mesh_bvh_bytes(int32_t F);
+size_t gsr_mesh_build_bytes(int32_t F);
+/* Build the BVH of F triangles: vertices float64 [V,3], faces int64 [F,3] (device).  A triangle with a vertex index outside
+ * [0, V), a non-finite vertex, or (v1 - v0) x (v2 - v0) == 0 in float64 is never hit.  bvh and workspace are 256-byte aligned
+ * device memory; the workspace may be reused once the build has run on the stream. */
+int gsr_mesh_build(int64_t V, int32_t F, const double* vertices, const int64_t* faces, void* bvh, size_t bvh_bytes, void* workspace,
+                   size_t workspace_bytes, void* stream);
+/* First hit of N rays (origins, directions [N,3], float32 if f64 == 0, float64 if f64 == 1, widened exactly) on a BVH built for
+ * F triangles: tri[i] the original index of the triangle with the smallest t > 0 (ties: the lower index), -1 on a miss;
+ * t[i] (may be NULL) its distance in units of the direction as given, +inf on a miss.  The watertight test in float64, every
+ * operation rounded on its own, both faces; a zero, NaN or infinite ray misses.  active (may be NULL): rays with
+ * active[i] < 0 are not cast and miss.  Identical results on any stream and from run to run. */
+int gsr_mesh_first_hit(int32_t F, const void* bvh, int64_t N, const void* origins, const void* directions, int32_t f64, const int64_t* active,
+                       int64_t* tri, double* t, void* stream);
+/* The inpainting mask of one view (extract_object.py:563-606) from a planar-mesh cast and a combined-mesh cast of the same N rays:
+ * mask[i] = 255 where ray i hits the planar mesh and |depth_all - depth_planar| < 0.01, else 0, with location = o + t d per
+ * component, depth = ((x w2c[8] + y w2c[9]) + z w2c[10]) + w2c[11] (w2c row-major float64 [4,4]), and depth_all = 0 where the
+ * combined mesh is missed.  counts (8-byte aligned int64 [2]) = (planar hits, planar hits that also hit the combined mesh). */
+int gsr_mesh_inpaint_mask(int64_t N, const void* origins, const void* directions, int32_t f64, const int64_t* tri_planar, const double* t_planar,
+                          const int64_t* tri_all, const double* t_all, const double* w2c, uint8_t* mask, int64_t* counts, void* stream);
+
 /* Device pointers into the workspaces of the last layout (P, capacity, W, H) — for parity tests that
  * compare per-stage buffers with the reference (SURVEY §4).  Pure pointer arithmetic, no CUDA calls. */
 typedef struct gsr_views {
