@@ -21,13 +21,19 @@
 //           < 1.3e-6 relative, which cannot move an image by 1e-4 — unless it flips a DECISION.  The two decisions are guarded:
 //             * alpha < 1/255 (skip): each lane tracks min |log2(255*alpha)| over its evaluations; below BL_QBAND the
 //               decision is inside the approximation's error band;
-//             * T(1-alpha) < 1e-4 (terminate): the fast drain terminates at 1e-4*(1-1e-5), so a pixel whose decision could
-//               differ from the reference's ends with |T| inside [1e-4*(1-1e-5), 1e-4*(1+1e-5)) and stays there;
+//             * T(1-alpha) < 1e-4 (terminate): the fast drain terminates at 1e-4*(1-BL_T_BAND), so a pixel whose decision could
+//               differ from the reference's ends with |T| inside [1e-4*(1-BL_T_BAND), 1e-4*(1+BL_T_BAND)) and stays there.  The
+//               band must cover how far the fast T drifts from the exact one: each unclamped splat in front moves it by
+//               alpha/(1-alpha) times the relative difference of the two alphas, so two fronts near alpha 0.98 amplify it ~100x.
+//               Measured on an H100 over 1080p stacks of one to three fronts with alpha up to 0.989 in front of a deciding
+//               splat (tests/test_gpu_blend_decisions.py): the largest drift is 1.82e-5, which a band of 1e-5 let through;
+//               BL_T_BAND = 4e-5 keeps 2.2x that.  (Alpha's worst-case relative difference, ~1e-6, times the largest possible
+//               amplification, 2*99 for the fronts and 99 for the deciding splat, would ask for 3e-4: 17x the redos.)
 //             * power > 0 (skip): cannot happen for a well-conditioned positive-definite conic (det > 1e-5*a*c, rounding of
 //               the power expression is 4e-7 of its terms); batches holding any other splat are drained exactly.
-//           A warp with any lane inside a band re-blends its whole list with the exact drain (counters->exact_redos, a few
-//           hundred of 65,280 warps per 1080p frame), so the default images carry the reference's decisions everywhere and
-//           n_contrib is identical to the exact mode's.
+//           A warp with any lane inside a band re-blends its whole list with the exact drain (counters->exact_redos: about
+//           1,300 of 65,280 warps per 3M/1080p frame on an H100 80GB HBM3 at 700 W, 460 with a 1e-5 band), so the default
+//           images carry the reference's decisions everywhere and n_contrib is identical to the exact mode's.
 #include "gsr_common.cuh"
 #include "gsr_packed.cuh"
 
@@ -36,8 +42,9 @@ namespace gsr {
 constexpr float BL_LOG2E = 1.4426950408889634f;
 constexpr float BL_LOG2_255 = 7.994353436858858f;
 constexpr float BL_QBAND = 3.0e-6f;                     // |log2(255 alpha)| below this: the skip decision is re-done exactly
-constexpr float BL_T_LO = 0.0001f * (1.0f - 1.0e-5f);   // fast drain's termination threshold
-constexpr float BL_T_HI = 0.0001f * (1.0f + 1.0e-5f);   // |T| below this at the end: termination decisions re-done exactly
+constexpr float BL_T_BAND = 4.0e-5f;                   // covers the fast T's relative drift from the exact T (see above)
+constexpr float BL_T_LO = 0.0001f * (1.0f - BL_T_BAND);  // fast drain's termination threshold
+constexpr float BL_T_HI = 0.0001f * (1.0f + BL_T_BAND);  // |T| below this at the end: termination decisions re-done exactly
 
 template <int NX>
 struct ListCfg {

@@ -169,6 +169,195 @@ def skip_band_case(device=None) -> Dict:
     return resolve(dict(case, g=g), device)
 
 
+def _records(a: Dict, device=None):
+    """[P, 6] fp32 {x, y, a, b, c, opacity} records and the visibility of a case's splats: the GPU forward's own (debug_views) when
+    device is a CUDA device, else the oracle's preprocess."""
+    if device is not None and torch.device(device).type == "cuda":
+        o = run_ours(a, for_backward=True)
+        return o["views"]["records"].cpu().numpy()[:, :6].copy(), o["radii"].cpu().numpy() > 0
+    pre = run_oracle({k: (v.cpu() if isinstance(v, torch.Tensor) else v) for k, v in a.items()}, stop_after="preprocess")
+    return np.concatenate([pre["means2D"], pre["conic_opacity"]], axis=1), pre["radii"] > 0
+
+
+def _points_at_pixels(cam, pix: np.ndarray, z: np.ndarray) -> torch.Tensor:
+    """World points that project to pixel coordinates pix [N, 2] at view-space depth z [N] (float64 inverse of the projection)."""
+    ndc = (2.0 * pix + 1.0) / np.array([cam.image_width, cam.image_height]) - 1.0
+    pv = np.stack([ndc[:, 0] * cam.tanfovx * z, ndc[:, 1] * cam.tanfovy * z, z, np.ones_like(z)], axis=1)
+    pw = pv @ np.linalg.inv(cam.world_view_transform.double().numpy())
+    return torch.from_numpy(pw[:, :3]).float().contiguous()
+
+
+def _point_splats(cam, pix: np.ndarray, z: np.ndarray, colors: np.ndarray, device=None) -> Dict:
+    """Resolved arguments of tiny isotropic splats (scale 1e-5: the 0.3-pixel low-pass sets the footprint) centred on pix at
+    depth z, with colours precomputed; the opacities are placeholders until the records are known."""
+    n = len(pix)
+    g = dict(means3D=_points_at_pixels(cam, pix, z), scales=torch.full((n, 3), 1e-5), opacities=torch.full((n, 1), 0.5),
+             rotations=torch.tensor([[1.0, 0.0, 0.0, 0.0]]).repeat(n, 1), shs=None)
+    a = resolve(dict(g=g, cam=cam, sh_degree=0, bg=(0.0, 0.0, 0.0), scale_modifier=1.0), device)
+    a["colors_precomp"] = torch.from_numpy(np.ascontiguousarray(colors, dtype=np.float32)).to(a["means3D"].device)
+    return a
+
+
+def _alpha_window(rec: np.ndarray, o: np.ndarray, centre: np.ndarray, R: int = 4):
+    """alpha = o * exp(power) in float64 (power with the GPU forward's rounding) at every pixel centre + (u, v), |u|, |v| <= R:
+    ([N, (2R+1)^2] alphas, [(2R+1)^2, 2] offsets).  Evaluated in chunks."""
+    off = np.stack(np.meshgrid(np.arange(-R, R + 1), np.arange(-R, R + 1), indexing="xy"), -1).reshape(-1, 2)
+    out = np.empty((len(rec), len(off)))
+    for s in range(0, len(rec), 65536):
+        r, c = rec[s:s + 65536, None, :], centre[s:s + 65536, None, :] + off[None]
+        out[s:s + 65536] = o[s:s + 65536, None].astype(np.float64) * np.exp(forward_power(r, c.astype(np.float32)).astype(np.float64))
+    return out, off
+
+
+def exact_alpha(o: np.ndarray, power: np.ndarray) -> np.ndarray:
+    """The exact drain's alpha in fp32: min(0.99, opacity * exp(power)), exp correctly rounded."""
+    e = np.exp(power.astype(np.float64)).astype(np.float32)
+    return np.minimum(np.float32(0.99), (o.astype(np.float32) * e).astype(np.float32))
+
+
+def exact_step(T: np.ndarray, alpha: np.ndarray) -> np.ndarray:
+    """The exact drain's termination test value T * (1 - alpha) in fp32."""
+    return (T * (np.float32(1) - alpha).astype(np.float32)).astype(np.float32)
+
+
+# Termination stacks: roles in depth order.  One-hot colours on a zero background: green carries the fronts and the clamped
+# control, red the deciding splat C alone (so red = T in front of C times alpha_C), blue the splat after C.
+ST_FRONT, ST_CTRL, ST_C, ST_AFTER = 0, 1, 2, 3
+STACK_WINDOW = 1e-4  # C's exact T (1 - alpha) is swept over 1e-4 * (1 +- STACK_WINDOW) ...
+STACK_FAR = (6e-4, 2e-3)  # ... or, for a fifth of the stacks, 1e-4 * (1 +- r) with r in this range
+
+
+def termination_stacks_case(W: int = 1920, H: int = 1080, seed: int = 131, device=None):
+    """Independent stacks of tiny splats on a 4-pixel grid, each centred within 0.04 pixel of its pixel centre, that put the
+    termination decision T (1 - alpha) < 1e-4 of a deciding splat C at its threshold.  In front of C: one front splat with
+    unclamped alpha in [0.90, 0.983] and a clamped control (alpha 0.99 in both drains), in either order; or two fronts with
+    alpha in [0.90, 0.989]; or three in [0.90, 0.944].  C's opacity is chosen so that the exact drain's fp32 T (1 - alpha_C) at
+    the stack's pixel is 1e-4 * (1 + r), r uniform in +-STACK_WINDOW (or +-STACK_FAR for one in five, outside the default blend's
+    termination band); every other stack is followed by one more splat (alpha
+    0.5..0.8).  The fronts' fast alphas drift from the exact ones by ~a / (1 - a) of ex2.approx's relative error each, so the
+    two drains' T in front of C can differ by more than the default blend's 1e-5 termination band.  No (pixel, splat) pair
+    comes within 2 % of alpha = 1/255, and at every stack's pixel the other stacks' splats stay below 1/510.
+    Returns (resolved arguments, facts): facts holds each stack's pixel, kind (1..3 fronts), whether a splat follows C, the
+    index of C, the exact fp32 T in front of C, the relative position r of its test value to the fp32 threshold and which
+    stacks are the far ones."""
+    rng = np.random.default_rng(seed)
+    cam = scene.lookat_camera((0.0, -3.0, 0.0), (0, 0, 0), W, H, 60.0)
+    gx, gy = np.meshgrid(2 + 4 * np.arange((W - 1) // 4), 2 + 4 * np.arange((H - 1) // 4), indexing="xy")
+    spix = np.stack([gx.reshape(-1), gy.reshape(-1)], 1).astype(np.float64)
+    S = len(spix)
+    kind = rng.integers(1, 4, S)
+    after = rng.random(S) < 0.5
+    ctrl_first = rng.random(S) < 0.5
+    # 1 - alpha of the fronts, log-uniform so that alphas near the top of their range are well represented
+    lu = lambda lo, hi, n: np.exp(rng.uniform(np.log(lo), np.log(hi), n))  # noqa: E731
+    om = np.zeros((S, 3))
+    om[:, 0] = np.where(kind == 3, lu(0.056, 0.1, S), np.where(kind == 1, lu(0.017, 0.1, S), lu(0.011, 0.1, S)))
+    lo2, hi2 = np.maximum(0.011, 1.7e-4 / om[:, 0]), np.minimum(0.1, 2e-3 / om[:, 0])
+    om[:, 1] = np.where(kind == 3, lu(0.056, 0.1, S), np.exp(rng.uniform(np.log(lo2), np.log(hi2))))
+    om[:, 2] = lu(0.056, 0.1, S)
+    # one stack in five lies outside the default blend's termination band (STACK_FAR): there the fast T in front of C is not
+    # replaced by a redo and can be compared with the exact one
+    far = rng.random(S) < 0.2
+    r = np.where(far, rng.uniform(*STACK_FAR, S) * rng.choice([-1.0, 1.0], S), rng.uniform(-STACK_WINDOW, STACK_WINDOW, S))
+    roles, stack, target, depth_rank = [], [], [], []
+    for s in range(S):
+        k = int(kind[s])
+        seq = [(ST_FRONT, 1 - om[s, 0])] + ([(ST_CTRL, 0.99)] if k == 1 else [(ST_FRONT, 1 - om[s, i]) for i in range(1, k)])
+        if k == 1 and ctrl_first[s]:
+            seq = seq[::-1]
+        seq += [(ST_C, 0.0)] + ([(ST_AFTER, rng.uniform(0.5, 0.8))] if after[s] else [])
+        roles += [q[0] for q in seq]
+        target += [q[1] for q in seq]
+        stack += [s] * len(seq)
+        depth_rank += list(range(len(seq)))
+    roles, stack, target, depth_rank = (np.asarray(v) for v in (roles, stack, target, depth_rank))
+    pix = spix[stack]
+    colors = np.zeros((len(roles), 3))
+    colors[roles == ST_C, 0] = 1.0
+    colors[(roles == ST_FRONT) | (roles == ST_CTRL), 1] = 1.0
+    colors[roles == ST_AFTER, 2] = 1.0
+    a = _point_splats(cam, pix + rng.uniform(-0.04, 0.04, pix.shape), 3.0 + 0.05 * depth_rank, colors, device)
+    rec, vis = _records(a, device)
+    assert vis.all() and (np.abs(rec[:, :2] - pix) <= 0.05).all()
+    E = np.exp(forward_power(rec, pix.astype(np.float32)).astype(np.float64))
+    o = (target / E).astype(np.float32)
+    o[roles == ST_CTRL] = np.float32(0.99 * 1.001) / E[roles == ST_CTRL].astype(np.float32)
+    # the exact drain's T in front of C, replayed in fp32, then C's opacity for T (1 - alpha_C) = 1e-4 (1 + r)
+    power = forward_power(rec, pix.astype(np.float32))
+    T = np.ones(S, np.float32)
+    for d in range(int(depth_rank.max()) + 1):
+        sel = (depth_rank == d) & ((roles == ST_FRONT) | (roles == ST_CTRL))
+        s = stack[sel]
+        al = exact_alpha(o[sel], power[sel])
+        T[s] = exact_step(T[s], al)
+    c_idx = np.flatnonzero(roles == ST_C)
+    assert (stack[c_idx] == np.arange(S)).all()
+    a_c = 1.0 - 1e-4 * (1.0 + r) / T.astype(np.float64)
+    o[c_idx] = (a_c / E[c_idx]).astype(np.float32)
+    test = exact_step(T, exact_alpha(o[c_idx], power[c_idx]))
+    assert (o > 0.3).all() and (o < 1.0).all(), (o.min(), o.max())
+    # no pair near the skip threshold; the other stacks' splats far below it at a stack's pixel
+    aw, off = _alpha_window(rec, o, pix)
+    assert (np.abs(255.0 * aw - 1.0) > 0.02).all()
+    other = ((off % 4) == 0).all(axis=1) & (off != 0).any(axis=1)
+    assert (aw[:, other] < 0.5 / 255.0).all()
+    a["opacities"] = torch.from_numpy(o.reshape(-1, 1)).to(a["means3D"].device)
+    facts = dict(pix=spix.astype(np.int64), kind=kind, after=after, c_idx=c_idx, T_front=T, far=far,
+                 r=test.astype(np.float64) / np.float64(np.float32(1e-4)) - 1.0)
+    return a, facts
+
+
+def far_edge_skip_case(W: int = 1920, H: int = 1080, seed: int = 137, device=None):
+    """Tiny splats on an 8-pixel grid with opacities in [0.5, 1), each placed so that at one pixel 1.6..1.9 pixel from its centre
+    (power <= -4, power * log2e about -7.5) opacity * exp(power) is 1/255 in fp32, or 1 ulp above or below it, for three in four
+    of them, and 2..34 ulp above or below for the rest (skip_band_case's pattern and nudge loop).  There log2(opacity) is small
+    and power carries q's rounding error, the other end of the skip decision's error budget from skip_band_case.  Every other
+    (pixel, splat) pair is at least 0.2 % from 1/255 (splats for which one is not are left out).  Returns (resolved arguments,
+    the [N, 2] target pixel of each splat)."""
+    rng = np.random.default_rng(seed)
+    cam = scene.lookat_camera((0.0, -3.0, 0.0), (0, 0, 0), W, H, 60.0)
+    gx, gy = np.meshgrid(4 + 8 * np.arange((W - 8) // 8), 4 + 8 * np.arange((H - 8) // 8), indexing="xy")
+    tpix = np.stack([gx.reshape(-1), gy.reshape(-1)], 1).astype(np.float64)
+    N = len(tpix)
+    o0 = rng.uniform(0.55, 0.95, N)
+    d = np.sqrt(np.log(255.0 * o0) / (0.5 / 0.3))  # distance at which o0 exp(-d^2 / 0.6) = 1/255 under the low-pass alone
+    th = rng.uniform(0, 2 * np.pi, N)
+    centre = tpix + np.stack([d * np.cos(th), d * np.sin(th)], 1)
+    a = _point_splats(cam, centre, np.full(N, 3.0), rng.uniform(0.0, 1.0, (N, 3)), device)
+    rec, vis = _records(a, device)
+    assert vis.all()
+    power = forward_power(rec, tpix.astype(np.float32))
+    assert (power <= -4.0).all(), power.max()
+    E = np.exp(power.astype(np.float64)).astype(np.float32)
+    n = np.arange(N)
+    k = np.where(n % 4 < 3, (n % 4) - 1, (2 + (n * 7) % 33) * np.where((n // 4) % 2 == 0, 1, -1)).astype(np.float64)
+    target = np.float32(1.0 / 255.0).astype(np.float64) + k * BAND_ULPS
+    o = (target / E.astype(np.float64)).astype(np.float32)
+    for _ in range(4):  # nudge each opacity until the fp32 product is the target exactly
+        got = (o.astype(np.float64) * E).astype(np.float32).astype(np.float64)
+        o = np.where(got < target, np.nextafter(o, np.float32(1)), np.where(got > target, np.nextafter(o, np.float32(0)), o))
+    assert ((o.astype(np.float64) * E).astype(np.float32).astype(np.float64) == target).all()
+    assert (o >= 0.5).all() and (o < 1.0).all()
+    aw, off = _alpha_window(rec, o, tpix)
+    aw[:, (off == 0).all(axis=1)] = 0.0
+    keep = (np.abs(255.0 * aw - 1.0) > 2e-3).all(axis=1)
+    assert keep.mean() > 0.95, keep.mean()
+    a["opacities"] = torch.from_numpy(o.reshape(-1, 1)).to(a["means3D"].device)
+    kt = torch.from_numpy(keep).to(a["means3D"].device)
+    for key in ("means3D", "scales", "rotations", "opacities", "colors_precomp"):
+        a[key] = a[key][kt].contiguous()
+    return a, tpix[keep].astype(np.int64)
+
+
+def trained_like_case(cam_index: int, device=None) -> Dict:
+    """config3's 3M Gaussians with every second opacity redrawn in [0.90, 0.99) (a trained scene's opaque surfaces: fronts whose
+    fast alpha drifts from the exact one by up to ~a / (1 - a) of ex2.approx's error), at 1920x1080 from a trajectory camera."""
+    g = scene.config3_scene()
+    g["opacities"][::2] = 0.90 + 0.09 * torch.rand(g["opacities"][::2].shape, generator=torch.Generator().manual_seed(139))
+    cam = scene.cameras_from_trajectory(scene.trajectory_dict(num_views=300))[cam_index]
+    return resolve(dict(g=g, cam=cam, sh_degree=3, bg=(0.0, 0.0, 0.0), scale_modifier=1.0), device)
+
+
 def band_pixels(a: Dict) -> np.ndarray:
     """[BAND_SPLATS, 2] (x, y) pixel of each band splat of skip_band_case: the nearest to its projected centre."""
     from oracle import gsr_oracle  # noqa: F401

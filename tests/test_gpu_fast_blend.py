@@ -12,7 +12,8 @@ from autovfx_b200 import scene
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-CASES = ["config1", "small_sh", "small_deg1_m25", "deg3_m25", "deg2_m25", "small_precomp", "big_splats", "dense_tile", "coplanar"]
+CASES = ["config1", "small_sh", "small_deg1_m25", "deg3_m25", "deg2_m25", "small_precomp", "big_splats", "dense_tile", "coplanar",
+         "skip_band", "faint_slab"]
 
 
 def _have_ref():
@@ -22,7 +23,7 @@ def _have_ref():
 @pytest.mark.parametrize("name", CASES)
 @pytest.mark.parametrize("for_backward", [False, True])
 def test_fast_equals_exact_decisions_and_is_close(name, for_backward):
-    a = Hh.resolve(Hh.case_inputs(name), DEV)
+    a = Hh.dense_case(name, DEV)
     fast = Hh.run_ours(a, for_backward=for_backward)
     f_img = {k: fast[k].clone() for k in ("color", "depth", "alpha")}
     nc_fast = fast["views"]["n_contrib"].clone()
@@ -90,6 +91,6 @@ def test_fast_blend_full_size_three_cameras():
         for k in worst:
             worst[k] = max(worst[k], Hh.maxabs(f_img[k], exact[k]))
         assert torch.equal(nc, exact["views"]["n_contrib"]), ci
-        assert 0 < redos < 6000, redos
+        assert 0 < redos < 3000, redos  # measured: 1,283..1,374 (H100 80GB HBM3, 700 W)
     print("fast vs exact, 3M/1080p, max abs:", worst)
     assert worst["color"] <= 1e-5 and worst["alpha"] <= 1e-5 and worst["depth"] <= 5e-5
