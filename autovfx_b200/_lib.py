@@ -178,6 +178,11 @@ SIGNATURES = {
     "gsr_mesh_build": (_int, [_i64, _i32] + [_ptr] * 3 + [_size, _ptr, _size, _ptr]),
     "gsr_mesh_first_hit": (_int, [_i32, _ptr, _i64, _ptr, _ptr, _i32] + [_ptr] * 4),
     "gsr_mesh_inpaint_mask": (_int, [_i64, _ptr, _ptr, _i32] + [_ptr] * 8),
+    "gsr_mesh_closest_bytes": (_size, [_i64]),
+    "gsr_mesh_closest": (_int, [_i32, _ptr, _i64, _ptr, _i32, _ptr, _ptr, _ptr, _size, _ptr]),
+    "gsr_mesh_isin_rows_bytes": (_size, [_i64, _i32]),
+    "gsr_mesh_isin_rows": (_int, [_i64, _ptr, _i64, _ptr, _i32, _i32, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(_i32), _ptr,
+                                  _ptr, _size, _ptr]),
     "gsr_get_views": (_int, [_ws, _i32, _i32, _i32, C.POINTER(gsr_views)]),
     "gsr_profile_begin": (_int, [_int]),
     "gsr_profile_begin_strided": (_int, [_int, _int]),

@@ -11,7 +11,12 @@
 //   query:  k_first_hit    one ray per thread, caller order, a 64-entry stack: the watertight test (Woop, Benthin and Wald 2013)
 //                          in float64 with every operation rounded on its own (no FMA contraction), smallest t, then lowest index
 //           k_inpaint_mask the inpainting mask of extract_object.py:563-606 from two casts' hits
-// DESIGN.md §4 argues why the box test never culls a triangle the exact test hits.
+//           k_closest_morton / k_rs_hist / scan / k_rs_scatter   the queries' order along a Morton curve in the root box
+//           k_closest      open3d's compute_closest_points on the same BVH: one point per thread in that order, nearer child first;
+//                          Ericson's closest-point test in float64, every operation rounded on its own, smallest d2, then lowest index
+//           k_isin_flags / k_isin_count / k_rs_scan / k_isin_scatter
+//                          np.isin(tri, query_tri) and the boolean indexing of the melting-mesh frame, rows in their original order
+// DESIGN.md §4 argues why the box tests never cull a triangle the exact tests would pick.
 #include "gsr_radix.cuh"
 #include <cfloat>
 #include <cstddef>
@@ -441,6 +446,265 @@ __global__ void __launch_bounds__(MESH_THREADS) k_inpaint_mask(int64_t N, const 
     }
 }
 
+__device__ __forceinline__ double ddot(const double u[3], const double w[3]) { return dadd(dadd(dmul(u[0], w[0]), dmul(u[1], w[1])), dmul(u[2], w[2])); }
+
+// The squared distance from p to its closest point q on triangle (a, b, c): Ericson's ClosestPtPointTriangle (Real-Time Collision
+// Detection §5.1.5) in float64, every operation rounded on its own, in this order (tests/closest_ref.py restates it):
+//   ab = b - a, ac = c - a, ap = p - a, bp = p - b, cp = p - c per component; dot(u, w) = (ux wx + uy wy) + uz wz
+//   d1 = dot(ab, ap), d2 = dot(ac, ap)                        d1 <= 0 and d2 <= 0:                    q = a
+//   d3 = dot(ab, bp), d4 = dot(ac, bp)                        d3 >= 0 and d4 <= d3:                   q = b
+//   vc = d1 d4 - d3 d2                                        vc <= 0 and d1 >= 0 and d3 <= 0:        q = a + (d1 / (d1 - d3)) ab
+//   d5 = dot(ab, cp), d6 = dot(ac, cp)                        d6 >= 0 and d5 <= d6:                   q = c
+//   vb = d5 d2 - d1 d6                                        vb <= 0 and d2 >= 0 and d6 <= 0:        q = a + (d2 / (d2 - d6)) ac
+//   va = d3 d6 - d5 d4, e = d4 - d3, f = d5 - d6              va <= 0 and e >= 0 and f >= 0:          q = b + (e / (e + f)) (c - b)
+//   otherwise den = (va + vb) + vc, v = vb / den, w = vc / den:                                      q = (a + v ab) + w ac
+//   and the result ((p - q)x^2 + (p - q)y^2) + (p - q)z^2, with s x = rn(s * x) and a + s x = rn(a + rn(s * x)) per component.
+__device__ __forceinline__ double closest_d2(const double p[3], const double* __restrict__ t) {
+    const double* a = t;
+    const double* b = t + 3;
+    const double* c = t + 6;
+    double ab[3], ac[3], ap[3], bp[3], cp[3], q[3];
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        ab[k] = dsub(b[k], a[k]);
+        ac[k] = dsub(c[k], a[k]);
+        ap[k] = dsub(p[k], a[k]);
+        bp[k] = dsub(p[k], b[k]);
+        cp[k] = dsub(p[k], c[k]);
+    }
+    const double d1 = ddot(ab, ap), d2 = ddot(ac, ap);
+    const double d3 = ddot(ab, bp), d4 = ddot(ac, bp);
+    const double d5 = ddot(ab, cp), d6 = ddot(ac, cp);
+    const double vc = dsub(dmul(d1, d4), dmul(d3, d2));
+    const double vb = dsub(dmul(d5, d2), dmul(d1, d6));
+    const double va = dsub(dmul(d3, d6), dmul(d5, d4));
+    const double e = dsub(d4, d3), f = dsub(d5, d6);
+    if (d1 <= 0.0 && d2 <= 0.0) {
+#pragma unroll
+        for (int k = 0; k < 3; k++) q[k] = a[k];
+    } else if (d3 >= 0.0 && d4 <= d3) {
+#pragma unroll
+        for (int k = 0; k < 3; k++) q[k] = b[k];
+    } else if (vc <= 0.0 && d1 >= 0.0 && d3 <= 0.0) {
+        const double v = __ddiv_rn(d1, dsub(d1, d3));
+#pragma unroll
+        for (int k = 0; k < 3; k++) q[k] = dadd(a[k], dmul(v, ab[k]));
+    } else if (d6 >= 0.0 && d5 <= d6) {
+#pragma unroll
+        for (int k = 0; k < 3; k++) q[k] = c[k];
+    } else if (vb <= 0.0 && d2 >= 0.0 && d6 <= 0.0) {
+        const double w = __ddiv_rn(d2, dsub(d2, d6));
+#pragma unroll
+        for (int k = 0; k < 3; k++) q[k] = dadd(a[k], dmul(w, ac[k]));
+    } else if (va <= 0.0 && e >= 0.0 && f >= 0.0) {
+        const double w = __ddiv_rn(e, dadd(e, f));
+#pragma unroll
+        for (int k = 0; k < 3; k++) q[k] = dadd(b[k], dmul(w, dsub(c[k], b[k])));
+    } else {
+        const double den = dadd(dadd(va, vb), vc);
+        const double v = __ddiv_rn(vb, den), w = __ddiv_rn(vc, den);
+#pragma unroll
+        for (int k = 0; k < 3; k++) q[k] = dadd(dadd(a[k], dmul(v, ab[k])), dmul(w, ac[k]));
+    }
+    const double ex = dsub(p[0], q[0]), ey = dsub(p[1], q[1]), ez = dsub(p[2], q[2]);
+    return dadd(dadd(dmul(ex, ex), dmul(ey, ey)), dmul(ez, ez));
+}
+
+// The lower bound of the box test: the squared distance from p to the box grown by pad, per-axis gaps clamped at 0.  It never
+// exceeds the computed squared distance of a valid triangle inside the box (DESIGN.md §4); an empty box gives +inf.
+__device__ __forceinline__ double box_lower(const double p[3], const float* b, double pad) {
+    double g[3];
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        const double lo = dsub((double)b[k], pad), hi = dadd((double)b[3 + k], pad);
+        g[k] = fmax(fmax(dsub(lo, p[k]), dsub(p[k], hi)), 0.0);
+    }
+    return dadd(dadd(dmul(g[0], g[0]), dmul(g[1], g[1])), dmul(g[2], g[2]));
+}
+
+template <typename T>
+__global__ void __launch_bounds__(MESH_THREADS) k_closest(int64_t N, int32_t F, const MeshHeader* __restrict__ hdr, const MeshNode* __restrict__ nodes,
+                                                          const double* __restrict__ tris, const int32_t* __restrict__ ids,
+                                                          const T* __restrict__ pts, const uint32_t* __restrict__ order,
+                                                          int64_t* __restrict__ tri_out, double* __restrict__ d2_out) {
+    const int64_t k = (int64_t)blockIdx.x * MESH_THREADS + threadIdx.x;
+    if (k >= N) return;
+    const int64_t i = order ? (int64_t)order[k] : k;  // neighbouring threads take spatially close points; results go to row i
+    double best_d2 = INFINITY;
+    int32_t best = -1;
+    double p[3];
+    bool ok = true;
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+        p[c] = (double)pts[3 * i + c];
+        ok = ok && isfinite(p[c]);
+    }
+    if (ok && F > 0) {
+        const double pad = dmul(0x1p-24, dadd(fmax(fmax(fabs(p[0]), fabs(p[1])), fabs(p[2])), (double)hdr->coord_max));
+        // a candidate wins with a smaller d2, or the same d2 and a lower index; NaN and +inf (overflow) never win
+        auto leaf = [&](int k) {
+            const int32_t id = ids[k];
+            if (id < 0) return;
+            const double dd = closest_d2(p, tris + 9 * (size_t)k);
+            if (dd < best_d2 || (dd == best_d2 && id < best)) {
+                best_d2 = dd;
+                best = id;
+            }
+        };
+        // culled: a lower bound strictly above the best d2 (a tie at a lower index stays reachable), or +inf
+        auto keep = [&](double lb) { return lb < INFINITY && !(lb > best_d2); };
+        if (F == 1) {
+            leaf(0);
+        } else {
+            int stack[MESH_STACK];
+            int sp = 0, node = 0;
+            while (true) {
+                const MeshNode n = nodes[node];
+                const float bl[6] = {n.a.x, n.a.y, n.a.z, n.a.w, n.b.x, n.b.y};
+                const float br[6] = {n.b.z, n.b.w, n.c.x, n.c.y, n.c.z, n.c.w};
+                const double kl = box_lower(p, bl, pad), kr = box_lower(p, br, pad);
+                bool hl = keep(kl), hr = keep(kr);
+                if (hl && n.left < 0) { leaf(~n.left); hl = false; }
+                if (hr && n.right < 0) { leaf(~n.right); hr = false; }
+                // the pushed child is tested again when popped: the best d2 may have shrunk meanwhile
+                if (hl && hr) {
+                    const bool lfirst = kl <= kr;
+                    stack[sp++] = lfirst ? n.right : n.left;
+                    node = lfirst ? n.left : n.right;
+                } else if (hl) {
+                    node = n.left;
+                } else if (hr) {
+                    node = n.right;
+                } else {
+                    if (sp == 0) break;
+                    node = stack[--sp];
+                }
+            }
+        }
+    }
+    tri_out[i] = best;
+    if (d2_out) d2_out[i] = best_d2;
+}
+
+// Query order for k_closest: 30-bit Morton codes of the points in the root box (float32 arithmetic, clamped; a non-finite point gets
+// 0xffffffff), sorted with their row indices.  Only the order of the work changes, never a result.
+template <typename T>
+__global__ void __launch_bounds__(MESH_THREADS) k_closest_morton(int64_t N, const MeshNode* __restrict__ nodes, const T* __restrict__ pts,
+                                                                 uint32_t* __restrict__ codes, uint32_t* __restrict__ vals) {
+    const int64_t i = (int64_t)blockIdx.x * MESH_THREADS + threadIdx.x;
+    if (i >= N) return;
+    const MeshNode n = nodes[0];
+    const float lo[3] = {fminf(n.a.x, n.b.z), fminf(n.a.y, n.b.w), fminf(n.a.z, n.c.x)};
+    const float hi[3] = {fmaxf(n.a.w, n.c.y), fmaxf(n.b.x, n.c.z), fmaxf(n.b.y, n.c.w)};
+    uint32_t code = 0;
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        const float x = (float)pts[3 * i + k];
+        if (!isfinite(x)) code = MESH_INVALID_CODE;
+        const float ext = hi[k] - lo[k];
+        float q = ext > 0.f ? (x - lo[k]) / ext * 1023.f : 0.f;
+        q = fminf(fmaxf(q, 0.f), 1023.f);  // also maps NaN to 0
+        if (code != MESH_INVALID_CODE) code |= mesh_spread10((uint32_t)q) << k;
+    }
+    codes[i] = code;
+    vals[i] = (uint32_t)i;
+}
+
+struct ClosestWs {
+    size_t codes0, codes1, vals0, vals1, hist, part, total;
+    int nchunks;
+    explicit ClosestWs(size_t N) {
+        nchunks = rs_chunks(N);
+        const size_t nhist = 256 * (size_t)nchunks;
+        size_t o = 0;
+        codes0 = o; o = align_up(o + 4 * N, 256);
+        codes1 = o; o = align_up(o + 4 * N, 256);
+        vals0 = o;  o = align_up(o + 4 * N, 256);
+        vals1 = o;  o = align_up(o + 4 * N, 256);
+        hist = o;   o = align_up(o + 4 * nhist, 256);
+        part = o;   o = align_up(o + 4 * scan_parts(nhist), 256);
+        total = o;
+    }
+};
+
+constexpr int ISIN_THREADS = 256;
+constexpr int ISIN_ROUNDS = 4;  // a block selects from ISIN_ROUNDS * ISIN_THREADS consecutive rows
+constexpr int ISIN_TILE = ISIN_THREADS * ISIN_ROUNDS;
+constexpr int ISIN_MAX_ARRAYS = 8;
+
+struct IsinArrays {
+    const uint32_t* src[ISIN_MAX_ARRAYS];
+    uint32_t* dst[ISIN_MAX_ARRAYS];
+    int32_t words[ISIN_MAX_ARRAYS];
+    int32_t K;
+};
+
+__global__ void __launch_bounds__(ISIN_THREADS) k_isin_flags(int64_t Q, const int64_t* __restrict__ query, int32_t F, uint8_t* __restrict__ flags) {
+    const int64_t j = (int64_t)blockIdx.x * ISIN_THREADS + threadIdx.x;
+    if (j >= Q) return;
+    const int64_t t = query[j];
+    if (t >= 0 && t < F) flags[t] = 1;
+}
+
+__device__ __forceinline__ bool isin_keep(int64_t N, const int64_t* __restrict__ tri, int32_t F, const uint8_t* __restrict__ flags, int64_t i) {
+    if (i >= N) return false;
+    const int64_t t = tri[i];
+    return t >= 0 && t < F && flags[t] != 0;
+}
+
+// Kept rows per tile; block_counts[tiles] is the scan's extra entry, which becomes the total.
+__global__ void __launch_bounds__(ISIN_THREADS) k_isin_count(int64_t N, const int64_t* __restrict__ tri, int32_t F, const uint8_t* __restrict__ flags,
+                                                             uint32_t* __restrict__ block_counts, int tiles) {
+    __shared__ uint32_t warp_n[ISIN_THREADS / 32];
+    const int64_t base = (int64_t)blockIdx.x * ISIN_TILE;
+    uint32_t n = 0;
+#pragma unroll
+    for (int r = 0; r < ISIN_ROUNDS; r++) n += isin_keep(N, tri, F, flags, base + r * ISIN_THREADS + threadIdx.x) ? 1u : 0u;
+    n = __reduce_add_sync(GSR_FULL, n);
+    if ((threadIdx.x & 31) == 0) warp_n[threadIdx.x >> 5] = n;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint32_t s = 0;
+        for (int w = 0; w < ISIN_THREADS / 32; w++) s += warp_n[w];
+        block_counts[blockIdx.x] = s;
+        if (blockIdx.x == 0) block_counts[tiles] = 0u;
+    }
+}
+
+// Every kept row i goes to its rank among the kept rows (block offset + rank inside the tile), in row order; words are copied as
+// integers, so every bit pattern arrives unchanged, as with t[mask].
+__global__ void __launch_bounds__(ISIN_THREADS) k_isin_scatter(int64_t N, const int64_t* __restrict__ tri, int32_t F, const uint8_t* __restrict__ flags,
+                                                               const uint32_t* __restrict__ offsets, int tiles, IsinArrays A,
+                                                               int64_t* __restrict__ count) {
+    __shared__ uint32_t warp_n[ISIN_THREADS / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t base = (int64_t)blockIdx.x * ISIN_TILE;
+    uint32_t run = offsets[blockIdx.x];
+    for (int r = 0; r < ISIN_ROUNDS; r++) {
+        const int64_t i = base + r * ISIN_THREADS + threadIdx.x;
+        const bool k = isin_keep(N, tri, F, flags, i);
+        const unsigned bal = __ballot_sync(GSR_FULL, k);
+        if (lane == 0) warp_n[warp] = __popc(bal);
+        __syncthreads();
+        uint32_t before = 0, total = 0;
+        for (int w = 0; w < ISIN_THREADS / 32; w++) {
+            const uint32_t c = warp_n[w];
+            before += w < warp ? c : 0u;
+            total += c;
+        }
+        if (k) {
+            const int64_t o = (int64_t)run + before + __popc(bal & ((1u << lane) - 1u));
+            for (int a = 0; a < A.K; a++) {
+                const int w = A.words[a];
+                for (int c = 0; c < w; c++) A.dst[a][o * w + c] = A.src[a][i * w + c];
+            }
+        }
+        run += total;
+        __syncthreads();  // warp_n is rewritten by the next round
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) *count = (int64_t)offsets[tiles];
+}
+
 }  // namespace
 }  // namespace gsr
 
@@ -545,4 +809,101 @@ int gsr_mesh_inpaint_mask(int64_t N, const void* origins, const void* directions
                                                                  t_all, w2c, mask, c);
     }
     return check_launch("gsr_mesh_inpaint_mask", false, st);
+}
+
+size_t gsr_mesh_closest_bytes(int64_t N) { return N < 0 || N > 0x7fffffffLL ? 0 : ClosestWs((size_t)N).total; }
+
+int gsr_mesh_closest(int32_t F, const void* bvh, int64_t N, const void* points, int32_t f64, int64_t* tri, double* d2, void* ws, size_t ws_bytes,
+                     void* stream) {
+    NvtxRange nvtx_("gsr_mesh_closest");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (F < 0 || !bvh || ((uintptr_t)bvh & 255) || N < 0 || N > 0x7fffffffLL || (f64 != 0 && f64 != 1) || (N > 0 && (!points || !tri))) {
+        set_error("gsr_mesh_closest: bad arguments (F %d, N %lld, f64 %d)", F, (long long)N, f64);
+        return GSR_ERR_INVALID;
+    }
+    const ClosestWs L((size_t)N);
+    if (!ws || ((uintptr_t)ws & 255) || ws_bytes < L.total) {
+        set_error("gsr_mesh_closest: workspace of %zu bytes, gsr_mesh_closest_bytes(%lld) = %zu needed (256-byte aligned)", ws_bytes, (long long)N,
+                  L.total);
+        return GSR_ERR_WORKSPACE;
+    }
+    if (N == 0) return GSR_OK;
+    const MeshBvh B((size_t)F);
+    const char* b = (const char*)bvh;
+    const MeshHeader* h = (const MeshHeader*)b;
+    const MeshNode* nodes = (const MeshNode*)(b + B.nodes);
+    const double* tris = (const double*)(b + B.tris);
+    const int32_t* ids = (const int32_t*)(b + B.ids);
+    const unsigned grid = (unsigned)((N + MESH_THREADS - 1) / MESH_THREADS);
+    const uint32_t* order = nullptr;
+    if (F > 1) {  // sort the queries along a Morton curve (DESIGN.md §4: trained models keep their rows in no spatial order)
+        char* w = (char*)ws;
+        uint32_t *k0 = (uint32_t*)(w + L.codes0), *k1 = (uint32_t*)(w + L.codes1), *v0 = (uint32_t*)(w + L.vals0), *v1 = (uint32_t*)(w + L.vals1);
+        uint32_t *hist = (uint32_t*)(w + L.hist), *part = (uint32_t*)(w + L.part);
+        if (f64)
+            k_closest_morton<double><<<grid, MESH_THREADS, 0, st>>>(N, nodes, (const double*)points, k0, v0);
+        else
+            k_closest_morton<float><<<grid, MESH_THREADS, 0, st>>>(N, nodes, (const float*)points, k0, v0);
+        const int rs_blocks = (L.nchunks + RS_WARPS - 1) / RS_WARPS;
+        for (int shift = 0; shift < 32; shift += 8) {
+            k_rs_hist<<<rs_blocks, RS_WARPS * 32, 0, st>>>((uint32_t)N, k0, shift, L.nchunks, hist);
+            scan_wide(hist, 256 * (size_t)L.nchunks, part, st);
+            k_rs_scatter<<<rs_blocks, RS_WARPS * 32, 0, st>>>((uint32_t)N, k0, v0, shift, L.nchunks, hist, k1, v1);
+            uint32_t* t = k0; k0 = k1; k1 = t;
+            t = v0; v0 = v1; v1 = t;
+        }
+        order = v0;
+    }
+    if (f64)
+        k_closest<double><<<grid, MESH_THREADS, 0, st>>>(N, F, h, nodes, tris, ids, (const double*)points, order, tri, d2);
+    else
+        k_closest<float><<<grid, MESH_THREADS, 0, st>>>(N, F, h, nodes, tris, ids, (const float*)points, order, tri, d2);
+    return check_launch("gsr_mesh_closest", false, st);
+}
+
+static int isin_tiles(int64_t N) { return (int)((N + ISIN_TILE - 1) / ISIN_TILE); }
+
+size_t gsr_mesh_isin_rows_bytes(int64_t N, int32_t F) {
+    if (N < 0 || N > 0x7fffffffLL || F < 0) return 0;
+    return align_up((size_t)F, 256) + ((size_t)isin_tiles(N) + 1) * sizeof(uint32_t);
+}
+
+int gsr_mesh_isin_rows(int64_t N, const int64_t* tri, int64_t Q, const int64_t* query_tri, int32_t F, int32_t K, const void* const* src,
+                       void* const* dst, const int32_t* words, int64_t* count, void* ws, size_t ws_bytes, void* stream) {
+    NvtxRange nvtx_("gsr_mesh_isin_rows");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (N < 0 || N > 0x7fffffffLL || Q < 0 || F < 0 || K < 0 || K > ISIN_MAX_ARRAYS || !count || ((uintptr_t)count & 7) ||
+        (N > 0 && !tri) || (Q > 0 && !query_tri) || (K > 0 && (!src || !dst || !words))) {
+        set_error("gsr_mesh_isin_rows: bad arguments (N %lld, Q %lld, F %d, K %d)", (long long)N, (long long)Q, F, K);
+        return GSR_ERR_INVALID;
+    }
+    IsinArrays A{};
+    A.K = K;
+    for (int a = 0; a < K; a++) {
+        if (words[a] < 0 || (words[a] > 0 && N > 0 && (!src[a] || !dst[a]))) {
+            set_error("gsr_mesh_isin_rows: array %d has %d words per row or a NULL pointer", a, words[a]);
+            return GSR_ERR_INVALID;
+        }
+        A.src[a] = (const uint32_t*)src[a];
+        A.dst[a] = (uint32_t*)dst[a];
+        A.words[a] = words[a];
+    }
+    if (!ws || ((uintptr_t)ws & 3) || ws_bytes < gsr_mesh_isin_rows_bytes(N, F)) {
+        set_error("gsr_mesh_isin_rows: workspace of %zu bytes, gsr_mesh_isin_rows_bytes(%lld, %d) = %zu needed (4-byte aligned)", ws_bytes,
+                  (long long)N, F, gsr_mesh_isin_rows_bytes(N, F));
+        return GSR_ERR_WORKSPACE;
+    }
+    if (N == 0) {
+        cudaMemsetAsync(count, 0, sizeof(int64_t), st);
+        return check_launch("gsr_mesh_isin_rows", false, st);
+    }
+    uint8_t* flags = (uint8_t*)ws;
+    uint32_t* counts = (uint32_t*)((char*)ws + align_up((size_t)F, 256));
+    if (F > 0) cudaMemsetAsync(flags, 0, (size_t)F, st);
+    if (F > 0 && Q > 0) k_isin_flags<<<(unsigned)((Q + ISIN_THREADS - 1) / ISIN_THREADS), ISIN_THREADS, 0, st>>>(Q, query_tri, F, flags);
+    const int tiles = isin_tiles(N);
+    k_isin_count<<<tiles, ISIN_THREADS, 0, st>>>(N, tri, F, flags, counts, tiles);
+    k_rs_scan<uint32_t><<<1, 1024, 0, st>>>(counts, tiles + 1);
+    k_isin_scatter<<<tiles, ISIN_THREADS, 0, st>>>(N, tri, F, flags, counts, tiles, A, count);
+    return check_launch("gsr_mesh_isin_rows", false, st);
 }

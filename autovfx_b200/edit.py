@@ -8,7 +8,11 @@ Replaces, for the render loop of ``scene_representation.py:355-438``:
 * per frame and per inserted object: ``load_gaussians`` (a .ply read!), ``transform_gaussians`` and ``merge_two_gaussians``
   (``gaussians_utils.py:62-125``) plus a ``copy.deepcopy`` of the whole scene (``scene_representation.py:358``) — by one
   ``gsr_activate_gaussians`` launch per (frame, object) that writes the transformed, activated object into the tail of the
-  resident scene arrays.
+  resident scene arrays;
+* per frame and per melting object (``scene_representation.py:372-421``): the mesh and ``.ply`` reloads, open3d's closest
+  triangles of the object's Gaussians and of the melting meshes' triangle centres, ``np.isin``, the boolean indexing and the
+  merge — by the Gaussians' closest triangles found once, one ``gsr_mesh_closest`` and one ``gsr_mesh_isin_rows`` per melting
+  mesh, one readback of the subsets' sizes and one activation per subset.
 
 Raw parameter dict (the reference's ``GaussianModel`` fields, as ``scene.load_ply`` returns them):
 ``xyz [N,3]``, ``f_dc [N,1,3]``, ``f_rest [N,M-1,3]``, ``opacity [N,1]``, ``scaling [N,3]`` (log), ``rotation [N,4]``.
@@ -134,6 +138,24 @@ def activate(raw: Mapping[str, torch.Tensor], device=None, xform: Optional[_lib.
     return dst
 
 
+# the melting meshes of one object per frame: ``{idx:03d}_obj.stl`` and ``{idx:03d}_obj_dup.stl``
+MELT_SUBSETS = 2
+
+
+class _Melting:
+    """One melting object: its raw Gaussians, its original mesh, their closest triangles, and two compaction buffers."""
+
+    def __init__(self, raw: Dict[str, torch.Tensor], mesh, ids: torch.Tensor):
+        self.raw, self.mesh, self.ids = raw, mesh, ids
+        self.bufs = [{k: torch.empty_like(v) for k, v in raw.items()} for _ in range(MELT_SUBSETS)]
+
+
+def _sh_count(raw: Mapping[str, torch.Tensor]) -> Optional[int]:
+    """M, the SH coefficients per channel, from the shapes of ``raw`` alone (no copy, no device work); None without rows."""
+    n = int(torch.as_tensor(raw["xyz"]).shape[0])
+    return int(torch.as_tensor(raw["f_rest"]).numel()) // (n * 3) + 1 if n else None
+
+
 class ResidentScene:
     """A background scene plus insertable objects, resident on one GPU.
 
@@ -142,11 +164,30 @@ class ResidentScene:
     ``deepcopy`` + ``load_gaussians`` + ``transform_gaussians`` + ``merge_two_gaussians``
     (scene_representation.py:357-371).  The returned views alias the resident arrays: they are valid until the next
     ``compose`` call on the same stream (frames are rendered in stream order, so a render loop needs no extra synchronisation).
+
+    ``melting={obj_id: (orig_raw, RayMesh(orig_mesh.vertices, orig_mesh.faces))}`` keeps each melting object's original
+    Gaussians resident and finds their closest original triangles once.  ``compose(melting={obj_id: [centres, ...]})`` is then
+    the melting-mesh branch of the render loop (scene_representation.py:372-421): for each of the frame's melting meshes
+    (``triangles_center`` arrays, at most ``_obj`` and ``_obj_dup`` per object, objects in sorted order) the original Gaussians
+    whose closest triangle is also the closest triangle of one of the centres (``np.isin``) are activated, in row order, behind
+    the scene.  The subsets' sizes are read back once per frame, together.
     """
 
     def __init__(self, scene_raw: Mapping[str, torch.Tensor], objects: Optional[Mapping[str, Mapping[str, torch.Tensor]]] = None,
-                 device=None):
+                 device=None, melting: Optional[Mapping[str, Tuple[Mapping[str, torch.Tensor], object]]] = None):
+        from .raycast import RayMesh
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        melting = dict(melting or {})
+        M = _sh_count(scene_raw) or 1
+        for k, entry in melting.items():  # checked before anything is uploaded
+            if not isinstance(entry, (tuple, list)) or len(entry) != 2:
+                raise ValueError("melting[%r] must be a pair (orig_raw, RayMesh)" % (k,))
+            if _sh_count(entry[0]) not in (None, M):
+                raise ValueError("melting object %r stores %d SH coefficients, the scene %d" % (k, _sh_count(entry[0]), M))
+            if not isinstance(entry[1], RayMesh):
+                raise ValueError("melting[%r][1] must be a RayMesh of the object's original mesh, not %s" % (k, type(entry[1]).__name__))
+            if entry[1].device != self.device:
+                raise ValueError("melting[%r][1] is on %s, the scene on %s" % (k, entry[1].device, self.device))
         scene = _raw_on(scene_raw, self.device)
         self.P_scene = scene["xyz"].shape[0]
         self.M = scene["f_rest"].numel() // max(self.P_scene * 3, 1) + 1
@@ -155,13 +196,39 @@ class ResidentScene:
             n = o["xyz"].shape[0]
             if n and o["f_rest"].numel() // (n * 3) + 1 != self.M:
                 raise ValueError("object %r stores %d SH coefficients, the scene %d" % (k, o["f_rest"].numel() // (n * 3) + 1, self.M))
+        self.melting_objects: Dict[str, _Melting] = {}
+        with torch.no_grad(), torch.cuda.device(self.device):
+            for k, (raw, mesh) in melting.items():
+                r = _raw_on(raw, self.device)
+                self.melting_objects[k] = _Melting(r, mesh, mesh.closest(r["xyz"])[0])  # once: the same answer on every frame
+            ws = max([int(_L.gsr_mesh_isin_rows_bytes(m.ids.shape[0], m.mesh.F)) for m in self.melting_objects.values()], default=0)
+            self._isin_ws = torch.empty((max(ws, 4),), dtype=torch.uint8, device=self.device)
+            self._isin_count = torch.zeros((max(MELT_SUBSETS * len(melting), 1),), dtype=torch.int64, device=self.device)
         cap = self.P_scene + sum(o["xyz"].shape[0] for o in self.objects.values())
+        cap += MELT_SUBSETS * sum(m.ids.shape[0] for m in self.melting_objects.values())
         self.arrays = _alloc(cap, self.M, self.device)
         activate_into(scene, self.arrays, 0, None)  # once; the raw scene tensors are not kept
         self.count = self.P_scene
 
-    def compose(self, transforms: Mapping[str, Tuple] = ()) -> Dict[str, torch.Tensor]:
+    def _melting_plan(self, melting: Mapping[str, Sequence]) -> list:
+        """(obj_id, slot, centres) of the frame's melting meshes in the reference's order: object ids sorted, then the meshes in
+        the order given (``_obj`` before ``_obj_dup``)."""
+        plan = []
+        for obj_id in sorted(melting):
+            if obj_id not in self.melting_objects:
+                raise KeyError("unknown melting object %r" % (obj_id,))
+            centres = list(melting[obj_id])
+            if len(centres) > MELT_SUBSETS:
+                raise ValueError("melting[%r]: %d meshes, at most %d per object (_obj and _obj_dup)" % (obj_id, len(centres), MELT_SUBSETS))
+            plan += [(obj_id, slot, c) for slot, c in enumerate(centres)]
+        return plan
+
+    def compose(self, transforms: Mapping[str, Tuple] = (), melting: Optional[Mapping[str, Sequence]] = None) -> Dict[str, torch.Tensor]:
+        if melting is not None and len(dict(transforms)):
+            raise ValueError("transforms and melting are exclusive, as the reference's rigid-body and melting-mesh branches are")
         off = self.P_scene
+        if melting is not None:
+            off += self._compose_melting(self._melting_plan(melting))
         for obj_id, tf in dict(transforms).items():
             if obj_id not in self.objects:
                 raise KeyError("unknown object %r" % (obj_id,))
@@ -169,3 +236,28 @@ class ResidentScene:
             off += activate_into(self.objects[obj_id], self.arrays, off, xf)
         self.count = off
         return {k: v[:off] for k, v in self.arrays.items()}
+
+    def _compose_melting(self, plan: list) -> int:
+        """Select and activate the melting subsets behind the scene; returns the rows written."""
+        if not plan:
+            return 0
+        dev = self.device
+        stream = _lib.stream_ptr(dev)
+        K = len(RAW_KEYS)
+        with torch.no_grad(), torch.cuda.device(dev):
+            for j, (obj_id, slot, centres) in enumerate(plan):
+                m = self.melting_objects[obj_id]
+                tri_c = m.mesh.closest(centres)[0]
+                dst = m.bufs[slot]
+                src_p = (C.c_void_p * K)(*[m.raw[k].data_ptr() for k in RAW_KEYS])
+                dst_p = (C.c_void_p * K)(*[dst[k].data_ptr() for k in RAW_KEYS])
+                words = (C.c_int32 * K)(*[m.raw[k].numel() // max(m.ids.shape[0], 1) for k in RAW_KEYS])
+                _lib.check(_L.gsr_mesh_isin_rows(m.ids.shape[0], m.ids.data_ptr(), tri_c.shape[0], tri_c.data_ptr(), m.mesh.F, K, src_p, dst_p,
+                                                 words, self._isin_count[j:].data_ptr(), self._isin_ws.data_ptr(), self._isin_ws.numel(),
+                                                 stream), "gsr_mesh_isin_rows")
+            counts = self._isin_count[:len(plan)].tolist()  # the frame's one readback: the views need the row count
+        off = self.P_scene
+        for (obj_id, slot, _), n in zip(plan, counts):
+            sub = {k: v[:n] for k, v in self.melting_objects[obj_id].bufs[slot].items()}
+            off += activate_into(sub, self.arrays, off, None)
+        return off - self.P_scene

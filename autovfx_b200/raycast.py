@@ -9,10 +9,18 @@ The semantics are fixed (DESIGN.md §4): the watertight test (Woop, Benthin and 
 on its own; both faces; hits with t > 0 along the direction as given; the smallest t, ties to the lower triangle index.
 Degenerate triangles, triangles with a non-finite vertex, and zero, NaN or infinite rays never hit.  tests/raycast_ref.py
 restates the test in numpy, bit for bit.
+
+The same BVH answers open3d's ``RaycastingScene.compute_closest_points`` (INTEGRATION.md, "Closest triangles")::
+
+    tri, d2 = rm.closest(points)                          # device int64 [N] and float64 [N], no readback
+    triangle_ids = rm.compute_closest_points(points)["primitive_ids"]
+
+Ericson's closest-point test in float64, every operation rounded on its own; the smallest squared distance, ties to the lower
+triangle index; invalid triangles never win; a non-finite point gives -1.
 """
 from __future__ import annotations
 
-from typing import Optional, Tuple
+from typing import Dict, Optional, Tuple
 
 import numpy as np
 import torch
@@ -53,7 +61,7 @@ def _rows3(t: torch.Tensor, name: str) -> None:
 
 
 class RayMesh:
-    """A triangle mesh prepared for first-hit ray casts on one CUDA device.
+    """A triangle mesh prepared for first-hit ray casts and closest-triangle queries on one CUDA device.
 
     ``vertices``: float32 or float64 ``[V, 3]``; ``faces``: int32 or int64 ``[F, 3]`` with every index in ``[0, V)``, F < 2**31
     (trimesh's ``mesh.vertices`` / ``mesh.faces``).  numpy arrays are uploaded to the current CUDA device (or to the device of
@@ -138,6 +146,36 @@ class RayMesh:
             th = t[index_ray].unsqueeze(1)
             locations = o[index_ray].to(torch.float64) + th * d[index_ray].to(torch.float64)
         return locations, index_ray, tri[index_ray]
+
+    def closest(self, points) -> Tuple[torch.Tensor, torch.Tensor]:
+        """(tri int64 [N], d2 float64 [N]) on the device, no readback: the valid triangle closest to each point and the squared
+        distance to its closest point (Ericson's ClosestPtPointTriangle in float64, every operation rounded on its own), the
+        smallest d2 winning and ties going to the lower triangle index.  ``points``: ``[N, 3]`` numpy array or CUDA tensor,
+        float32 or float64 (widened exactly), other real dtypes converted to float64.  A point with a non-finite coordinate, or a
+        mesh without a valid triangle, gives -1 and +inf.  The kernel visits the points along a Morton curve (N < 2**31)."""
+        p = _host_or_cuda(points, "points")
+        _rows3(p, "points")
+        if p.dtype == torch.bool or p.is_complex():
+            raise ValueError("points must be a real array, not %s" % p.dtype)
+        p = _on(p, "points", self.device)
+        f64 = 0 if p.dtype == torch.float32 else 1
+        N = int(p.shape[0])
+        if N >= 2 ** 31:
+            raise ValueError("points: %d rows, at most 2**31 - 1 are supported" % N)
+        with torch.no_grad(), torch.cuda.device(self.device):
+            p = p.detach().contiguous() if f64 == 0 else p.detach().to(torch.float64).contiguous()
+            tri = torch.empty((N,), dtype=torch.int64, device=self.device)
+            d2 = torch.empty((N,), dtype=torch.float64, device=self.device)
+            ws = _lib.scratch_bytes(max(int(_L.gsr_mesh_closest_bytes(N)), 256), self.device)
+            _lib.check(_L.gsr_mesh_closest(self.F, self.bvh.data_ptr(), N, p.data_ptr(), f64, tri.data_ptr(), d2.data_ptr(), ws.data_ptr(),
+                                            ws.numel(), _lib.stream_ptr(self.device)), "gsr_mesh_closest")
+        return tri, d2
+
+    def compute_closest_points(self, query_points) -> Dict[str, torch.Tensor]:
+        """open3d's ``RaycastingScene.compute_closest_points`` for the one key AutoVFX reads: ``{"primitive_ids": tri}``, a device
+        int64 [N] tensor.  Where open3d returns its uint32 ``INVALID_ID`` (no valid triangle, a non-finite point) this returns -1.
+        open3d's other keys (``points``, ``geometry_ids``, ``primitive_uvs``, ``primitive_normals``) are not computed."""
+        return {"primitive_ids": self.closest(query_points)[0]}
 
 
 def inpaint_mask(planar: RayMesh, combined: RayMesh, rays_o, rays_d, w2c) -> Optional[torch.Tensor]:

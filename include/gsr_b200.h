@@ -757,7 +757,7 @@ size_t gsr_png_workspace_bytes(int32_t n, const gsr_png_image* images);
 int gsr_png_encode(const gsr_png_image* images, int32_t n, uint8_t* const* outputs, int64_t* sizes, void* workspace, size_t workspace_bytes,
                    void* stream);
 
-/* ---- first-hit ray casts against a triangle mesh (gsr_mesh.cu): an LBVH over F triangles, DESIGN.md §4 ---- */
+/* ---- first-hit ray casts and closest triangles on a triangle mesh (gsr_mesh.cu): an LBVH over F triangles, DESIGN.md §4 ---- */
 /* Bytes of the BVH buffer of F triangles (float32 boxes, float64 triangles in leaf order), and of gsr_mesh_build's scratch. */
 size_t gsr_mesh_bvh_bytes(int32_t F);
 size_t gsr_mesh_build_bytes(int32_t F);
@@ -779,6 +779,24 @@ int gsr_mesh_first_hit(int32_t F, const void* bvh, int64_t N, const void* origin
  * combined mesh is missed.  counts (8-byte aligned int64 [2]) = (planar hits, planar hits that also hit the combined mesh). */
 int gsr_mesh_inpaint_mask(int64_t N, const void* origins, const void* directions, int32_t f64, const int64_t* tri_planar, const double* t_planar,
                           const int64_t* tri_all, const double* t_all, const double* w2c, uint8_t* mask, int64_t* counts, void* stream);
+/* Bytes of gsr_mesh_closest's workspace for N points (0 when N is out of range). */
+size_t gsr_mesh_closest_bytes(int64_t N);
+/* Closest triangle of N < 2^31 points ([N,3], float32 if f64 == 0, float64 if f64 == 1, widened exactly) on a BVH built for F
+ * triangles, the queries processed along a Morton curve (workspace: 256-byte aligned device memory), the results in caller order:
+ * tri[i] the original index of the valid triangle with the smallest squared distance to point i (ties: the lower index); d2[i]
+ * (may be NULL) that squared distance.  Ericson's ClosestPtPointTriangle in float64, every operation rounded on its own
+ * (DESIGN.md §4).  A point with a non-finite coordinate, F == 0 or a mesh without a valid triangle gives -1 and +inf.
+ * Identical results on any stream and from run to run. */
+int gsr_mesh_closest(int32_t F, const void* bvh, int64_t N, const void* points, int32_t f64, int64_t* tri, double* d2, void* workspace,
+                     size_t workspace_bytes, void* stream);
+/* Bytes of gsr_mesh_isin_rows' workspace for N rows and F triangles (0 when out of range). */
+size_t gsr_mesh_isin_rows_bytes(int64_t N, int32_t F);
+/* np.isin(tri, query_tri) followed by boolean indexing, for the melting-mesh frame: row i (of N) is kept when 0 <= tri[i] < F and
+ * tri[i] is one of the Q entries of query_tri (entries outside [0, F) match nothing).  The kept rows of K <= 8 arrays, array k
+ * holding words[k] 32-bit words per row (src[k], dst[k]: host arrays of device pointers), are copied in row order to the front
+ * of dst[k], bit for bit; count (device int64) receives their number.  workspace: 4-byte aligned device memory. */
+int gsr_mesh_isin_rows(int64_t N, const int64_t* tri, int64_t Q, const int64_t* query_tri, int32_t F, int32_t K, const void* const* src,
+                       void* const* dst, const int32_t* words, int64_t* count, void* workspace, size_t workspace_bytes, void* stream);
 
 /* Device pointers into the workspaces of the last layout (P, capacity, W, H) — for parity tests that
  * compare per-stage buffers with the reference (SURVEY §4).  Pure pointer arithmetic, no CUDA calls. */
